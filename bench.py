@@ -67,7 +67,7 @@ def log(*a):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = (
         "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
@@ -167,18 +167,7 @@ def load_peaks() -> tuple[float, str]:
     f = ROOT / "MEASURED_PEAKS.json"
     if f.exists():
         return float(json.loads(f.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic(key: str, world: int) -> float | None:
-    """DRAM bytes per launch from the committed ncu --set full capture (N=1, default workload only)."""
-    for name in ("r02_traffic.json", "r01_traffic.json"):
-        f = ROOT / "profiles" / name
-        if world == 1 and f.exists():
-            v = json.loads(f.read_text()).get(key)
-            if v:
-                return float(v)
-    return None
+    return 3350.0, "NVIDIA H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 # ---------------------------------------------------------------------------
@@ -488,13 +477,19 @@ def main() -> None:
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--score-batch", type=int, default=16384,
                     help="users per scoring launch (all users are scored); a launch lasts at least as long as its "
-                         "heaviest query (2.6 ms at ML-25M shape), so small batches are tail-bound")
+                         "heaviest query, so small batches are tail-bound")
     ap.add_argument("--score-users", type=int, default=0, help="score only this many users (0 = all)")
     ap.add_argument("--variants", default="bf16,fp32", help="ALS gather dtypes to time (profiling runs pass one)")
     ap.add_argument("--profile", action="store_true", help="under ncu: honour a small --warmup, skip e2e/parity/CPU")
     ap.add_argument("--scale", type=float, default=1.0, help="scale-out workloads: fraction of the full size (smoke runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed paths computed to DIR/<name>.npy: the factor tables after the last "
+                         f"timed epoch of each ALS variant (a fixed sample of {DUMP_ROWS} rows per table), the item-kNN "
+                         "similarity rows and the recommend top-N (fixed row samples)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 0)
+    if args.dump_outputs and (args.impl != "ours" or args.workload != "ml25m" or args.gpus != 1):
+        ap.error("--dump-outputs covers the default workload on one GPU (--workload ml25m --impl ours --gpus 1)")
     if args.profile:
         args.no_parity = args.no_cpu = True
 
@@ -581,6 +576,8 @@ def main() -> None:
         e1.record()
         barrier()
         t_end = time.time()
+        if args.dump_outputs and rank == 0:
+            dump_factors(args.dump_outputs, tag, tr)
         clocks = sampler.stop(t_begin, t_end) if (rank == 0 and tag == "bf16") else None
         # the same epochs once more with CUDA events around every row-solve launch (the roofline's
         # kernel time; events cannot sit inside a captured graph, so this loop launches eagerly)
@@ -614,7 +611,7 @@ def main() -> None:
                 "bound": "hbm",
                 "kernel": tr.solve_kernel_name() + " (user + item launch of one epoch)",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": ncu_traffic("als_tc_kernel_epoch_bytes", world) if tag == "bf16" else None,
+                "traffic": None,  # DRAM bytes per launch: not measured (needs a hardware-counter profile)
                 "algorithmic_bytes": alg, "peak_source": peak_src,
             },
             "clocks": clocks,
@@ -735,7 +732,7 @@ def main() -> None:
                 "workload": "ML-25M-shaped synthetic ImplicitMFScorer features=64 bf16 gather (BASELINE configs[1])",
                 "n_users": inter.n_users, "n_items": inter.n_items, "nnz": inter.nnz, "features": K,
                 "weight": WEIGHT, "reg": REG, "parallelism": f"row-sharded x{world}" if world > 1 else "single GPU",
-                "l2": "inputs (2 CSR orientations 400 MB + factors) exceed the 126 MB L2; no explicit flush",
+                "l2": "inputs (2 CSR orientations 400 MB + factors) exceed the 50 MB L2; no explicit flush",
             },
             "roofline": head["roofline"], "clocks": head["clocks"], "e2e": head.get("e2e"),
             "cuda_graph": head.get("cuda_graph"),
@@ -757,6 +754,44 @@ def main() -> None:
         raise SystemExit(1)
 
 
+DUMP_ROWS = 32768
+
+
+def dump_factors(out_dir: str, tag: str, tr) -> None:
+    """The user and item factors the timed epochs produced: the same seeded row sample every run (ML-25M
+    shape: 2 variants x 2 tables x 32,768 rows x 64 floats = 32 MB)."""
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in (("users", tr.d_users), ("items", tr.d_items)):
+        n = int(t.shape[0])
+        rows = np.sort(np.random.default_rng(20240611).choice(n, min(n, DUMP_ROWS), replace=False))
+        sample = t[torch.from_numpy(rows).to(t.device)].float().cpu().numpy()
+        np.save(os.path.join(out_dir, f"als_{tag}_{name}.npy"), sample)
+        np.save(os.path.join(out_dir, f"als_{tag}_{name}_rows.npy"), rows.astype(np.float64))
+    log(f"[bench] ALS {tag}: factor sample written to {out_dir}")
+
+
+def _dump_rows(out_dir: str, name: str, indptr: np.ndarray, cols: np.ndarray, vals: np.ndarray | None, width: int) -> None:
+    """A seeded sample of the rows of a CSR-like result, padded to `width` (columns -1, values NaN), plus the
+    length of every row."""
+    os.makedirs(out_dir, exist_ok=True)
+    n = len(indptr) - 1
+    rows = np.sort(np.random.default_rng(20240611).choice(n, min(n, DUMP_ROWS // 8), replace=False))
+    c = np.full((len(rows), width), -1.0)
+    v = np.full((len(rows), width), np.nan, dtype=np.float32)
+    for i, r in enumerate(rows):
+        a, b = int(indptr[r]), int(indptr[r + 1])
+        c[i, : b - a] = cols[a:b]
+        if vals is not None:
+            v[i, : b - a] = vals[a:b]
+    np.save(os.path.join(out_dir, f"{name}_rows.npy"), rows.astype(np.float64))
+    np.save(os.path.join(out_dir, f"{name}_lengths.npy"), np.diff(indptr).astype(np.float64))
+    np.save(os.path.join(out_dir, f"{name}_cols.npy"), c)
+    if vals is not None:
+        np.save(os.path.join(out_dir, f"{name}_vals.npy"), v)
+
+
 def bench_recommend(args, tr, dev, peak, peak_src) -> dict:
     """
     SURVEY.md §8f N1/N2: top-100 of all items for a batch of users from the factors just trained —
@@ -767,7 +802,9 @@ def bench_recommend(args, tr, dev, peak, peak_src) -> dict:
 
     from lkpy_b200 import engine
 
-    n_top, batch = 100, min(131072, int(tr.d_users.shape[0]))  # one thread per user: large batches fill the GPU
+    # one thread per user: large batches fill the GPU; 32,768 users keep the [items x users] fp32 score matrix
+    # at 7.7 GB (ML-25M shape), which fits an 80 GB H100 next to the trainer's tables
+    n_top, batch = 100, min(32768, int(tr.d_users.shape[0]))
     q, p = tr.d_items, tr.d_users
     rng = np.random.default_rng(11)
     users = torch.from_numpy(np.sort(rng.choice(p.shape[0], batch, replace=False))).to(dev)
@@ -779,6 +816,7 @@ def bench_recommend(args, tr, dev, peak, peak_src) -> dict:
     reps = 3
     t_gemm = t_top = 0.0
     for _ in range(reps):
+        del s
         ev[0].record()
         s = q @ x.T
         ev[1].record()
@@ -787,6 +825,10 @@ def bench_recommend(args, tr, dev, peak, peak_src) -> dict:
         torch.cuda.synchronize()
         t_gemm += ev[0].elapsed_time(ev[1]) / reps
         t_top += ev[1].elapsed_time(ev[2]) / reps
+    if args.dump_outputs:  # top-N item positions of the sampled users (one row per user)
+        c, ix = cnt.cpu().numpy().astype(np.int64), idx.cpu().numpy()
+        _dump_rows(args.dump_outputs, "recommend_topn", np.concatenate([[0], np.cumsum(c)]),
+                   np.concatenate([ix[j, : c[j]] for j in range(len(c))]), None, n_top)
     n_items = q.shape[0]
     alg = float(n_items) * batch * 4  # the selection reads every score once
     achieved = alg / (t_top * 1e-3) / 1e9
@@ -1011,13 +1053,15 @@ def bench_knn(args, inter, dev, peak, peak_src, rank: int, world: int, parity: d
                      "ctas_per_sm": plan.geom.ctas_per_sm, "work_units": u["n_units"]},
         "roofline": {"bound": "hbm", "kernel": "knn_build_kernel", "achieved": achieved, "peak": peak,
                      "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": ncu_traffic("knn_build_kernel_bytes", world), "algorithmic_bytes": alg,
+                     "traffic": None, "algorithmic_bytes": alg,
                      "peak_source": peak_src},
         "_kui": kui, "_kiu": kiu, "_cost": cost,
     }  # fmt: skip
     log(f"[bench] kNN build: {ms:.1f} ms = {out['build_items_per_s']:.0f} items/s; accumulate kernel {kms:.1f} ms, "
         f"{achieved:.0f} GB/s algorithmic = {achieved / peak:.3f} of peak")
     check_parity(*csr)
+    if args.dump_outputs:
+        _dump_rows(args.dump_outputs, "knn_sim", csr[0].cpu().numpy(), csr[1].cpu().numpy(), csr[2].cpu().numpy(), KNN_SAVE)
 
     # ---- end to end through the plugin call: host CSR in -> host CSR out (item_train.rs:32-93)
     if not args.profile:
@@ -1076,7 +1120,7 @@ def bench_knn(args, inter, dev, peak, peak_src, rank: int, world: int, parity: d
             "users": scored, "targets_per_user": inter.n_items, "batch": B, "ms": total_ms,
             "users_per_s": scored / (total_ms * 1e-3), "scored_fraction": finite / max(scored * inter.n_items, 1),
             "roofline": {"bound": "hbm", "kernel": "knn_score_dense_kernel", "achieved": ach_s, "peak": peak, "unit": "GB/s",
-                         "frac": ach_s / peak, "traffic": ncu_traffic("knn_score_dense_kernel_v3_bytes_per_2048_users", world),
+                         "frac": ach_s / peak, "traffic": None,
                          "traffic_note": "per launch of 2,048 users (the ncu capture), not per launch of this run",
                          "algorithmic_bytes": alg_s, "peak_source": peak_src},
         }  # fmt: skip

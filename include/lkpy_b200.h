@@ -1,5 +1,5 @@
 /*
- * lkpy_b200.h — C ABI of the B200-native ALS / item-kNN engine.
+ * lkpy_b200.h — C ABI of the H100-native ALS / item-kNN engine.
  *
  * This is the drop-in boundary for the reference's native accelerator
  * `lenskit._accel` (PyO3 cdylib, src/accel/lib.rs:25-49) restricted to the two
@@ -68,8 +68,7 @@ LK_API int lk_device_info(int *sm_count, int *cc);
 /* Diagnostic switches (kernel variants kept for comparison; none changes results beyond rounding).
  * Each is also an environment variable of the same name, read once when the library first needs
  * it — never per launch; after that only lk_set_option changes it.  Names: LK_ALS_TC,
- * LK_ALS_TC_INTERLEAVE, LK_ALS_TC_OCC, LK_ALS_TCS, LK_ALS_GJ, LK_ALS_TF32, LK_ALS_FLAGS, LK_KNN_WARPS,
- * LK_KNN_CTAS, LK_KNN_SCORE_SEQ, LK_KNN_SCORE_CTAS (meaning: lkpy_b200/csrc/common.cuh, struct Options). */
+ * LK_ALS_TF32, LK_KNN_WARPS, LK_KNN_CTAS, LK_KNN_SCORE_SEQ, LK_KNN_SCORE_CTAS (meaning: lkpy_b200/csrc/common.cuh, struct Options). */
 LK_API int lk_set_option(const char *name, int value);
 LK_API int lk_get_option(const char *name, int *value);
 
@@ -127,7 +126,7 @@ typedef struct lk_als_args {
     int32_t vals_uniform;    /* 1 when every d_vals entry equals uniform_val (implicit feedback without
                                 ratings): lets the Gram run on the tensor cores as v * M^T M */
     float uniform_val;
-    unsigned long long *d_prof; /* optional [16] per-phase SM-cycle counters (diagnostics), or NULL */
+    unsigned long long *d_prof; /* reserved (ignored by the kernels), NULL */
     /* Cooperative cancel (the role of CancelAdapter, src/accel/als/implicit.rs:72-73, tasks/mod.rs:62-106):
      * optional device flag, read (uncached) every time a CTA fetches work; once non-zero no further rows
      * are started — rows already solved keep their new values, the rest their old ones.  Progress =

@@ -1,5 +1,5 @@
 """
-In-tree build of the CUDA library ``lkpy_b200/csrc/liblkpy_b200.so`` for sm_100a.
+In-tree build of the CUDA library ``lkpy_b200/csrc/liblkpy_b200.so`` for sm_90a (H100).
 
 ``nvcc`` cross-compiles without a GPU, so this runs in the CPU build container;
 the resulting ``.so`` is git-ignored but travels to the GPU box with the tree.
@@ -16,9 +16,9 @@ from pathlib import Path
 
 CSRC = Path(__file__).resolve().parent / "csrc"
 LIB = CSRC / "liblkpy_b200.so"
-SOURCES = ["capi.cu", "als_kernels.cu", "als_tc.cu", "als_tcx.cu", "als_tc128.cu", "knn_build.cu", "knn_score.cu", "topn.cu", "prep.cu"]
+SOURCES = ["capi.cu", "als_kernels.cu", "als_tc.cu", "knn_build.cu", "knn_score.cu", "topn.cu", "prep.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17", "--extended-lambda",
     "-Xcompiler", "-fPIC,-fvisibility=hidden",
 ]  # fmt: skip
@@ -36,8 +36,7 @@ def _stale() -> bool:
         return True
     t = LIB.stat().st_mtime
     deps = [CSRC / s for s in SOURCES] + [
-        CSRC / "common.cuh", CSRC / "als_common.cuh", CSRC / "tc_common.cuh", CSRC / "chol_tc.cuh",
-        CSRC / "chol_tc128.cuh",
+        CSRC / "common.cuh", CSRC / "als_common.cuh",
     ]  # fmt: skip
     deps.append(CSRC.parent.parent / "include" / "lkpy_b200.h")
     return any(d.stat().st_mtime > t for d in deps)

@@ -215,7 +215,7 @@ def require_device():
 
     if not torch.cuda.is_available():
         raise EngineError(
-            "lkpy_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback"
+            "lkpy_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback"
         )
     return torch.device("cuda", torch.cuda.current_device())
 

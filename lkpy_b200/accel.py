@@ -3,7 +3,7 @@ Drop-in surface of the reference's native accelerator module for the two hot
 paths — the same function names, argument meaning and error behaviour as
 ``lenskit._accel.als`` / ``lenskit._accel.knn`` (stubs
 ``src/lenskit/_accel/als.pyi``, ``knn.pyi``) and the ``AccelTask`` protocol of
-``src/lenskit/parallel/_task.py:60-100`` — executed on the B200 through the C
+``src/lenskit/parallel/_task.py:60-100`` — executed on the H100 through the C
 ABI.  A maintainer rebinding ``from lenskit._accel import als`` /
 ``from lenskit import _accel`` to this module gets the GPU engine under the
 unchanged Python components (see INTEGRATION.md).

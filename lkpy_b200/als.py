@@ -1,5 +1,5 @@
 """
-ALS scorers on the B200 engine — the component surface of ``lenskit.als``.
+ALS scorers on the H100 engine — the component surface of ``lenskit.als``.
 
 Mirrors (same names, config fields and aliases, training/epoch contract):
 
@@ -268,8 +268,8 @@ class ALSTrainerBase(ModelTrainer):
     def _chunk_nnz(self, k: int) -> int:
         weighted = self.MODE == _lib.LK_ALS_IMPLICIT and getattr(self.config, "use_ratings", False)
         bf16_uniform = self.config.gather_dtype == "bfloat16" and not weighted
-        # shorter parts where a tensor-core accumulator would otherwise take hundreds of round-toward-zero
-        # additions (engine.TF32_CHUNK_NNZ*): the tf32 paths make three per 8 rows, the bf16 path one per 16
+        # shorter parts for the tensor-core Gram at k = 128 and on the tf32 paths (engine.TF32_CHUNK_NNZ*: part
+        # lengths carried over from an earlier tensor-core design, not re-measured on the H100)
         if k == 128:
             return engine.TF32_CHUNK_NNZ if bf16_uniform else engine.TF32_CHUNK_NNZ_K128
         if k == 64 and not bf16_uniform:
@@ -330,15 +330,22 @@ class ALSTrainerBase(ModelTrainer):
         """Which row-solve kernel the configuration runs (bench.py's roofline label)."""
         k = self.config.embedding_size
         on = _lib.get_option("LK_ALS_TC") != 0
-        uniform = self.MODE != _lib.LK_ALS_IMPLICIT or not getattr(self.config, "use_ratings", False)
-        if on and k == 64 and self.bf16 and uniform:
-            return "als_tc_kernel"
         tf32 = _lib.get_option("LK_ALS_TF32") != 0
-        if on and k == 64 and tf32:
-            return "als_tcx_kernel"
-        if on and k == 128 and ((self.bf16 and uniform) or tf32):
-            return "als_tc128_kernel"
-        return "als_half_kernel"
+
+        def one(plan, other) -> str:
+            # the conditions under which launch_als_tc (als_tc.cu) takes the launch
+            weighted = self.MODE == _lib.LK_ALS_IMPLICIT and not plan.vals_uniform
+            if not on or k not in (64, 128) or other.data_ptr() % 16 != 0:
+                return "als_half_kernel"
+            if weighted and not plan.uniform_val >= 0.0:  # sqrt(v) needs non-negative confidences
+                return "als_half_kernel"
+            if (not self.bf16 or weighted) and not tf32:
+                return "als_half_kernel"
+            return "als_tc_kernel"
+
+        users = one(self.u_plan, self.d_items_bf16 if self.bf16 else self.d_items)
+        items = one(self.i_plan, self.d_users_bf16 if self.bf16 else self.d_users)
+        return users if users == items else f"{users} (user half) / {items} (item half)"
 
     def launches_per_epoch(self) -> int:
         """Kernels of this library launched by one epoch (two halves: OtOr partial + reduce + row solve)."""

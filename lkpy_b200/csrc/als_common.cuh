@@ -7,6 +7,26 @@
 
 namespace lk {
 
+// launch shape of the ALS kernels (als_kernels.cu, als_tc.cu): one CTA per chunk, one warp per 64x64
+// quadrant of the Gram
+template <int KP>
+struct AlsCfg {
+    static constexpr int QUADS = KP >= 64 ? KP / 64 : 1;
+    static constexpr int NW = QUADS * QUADS;  // warps per CTA
+    static constexpr int NT = NW * 32;
+    static constexpr int QS = KP >= 64 ? 64 : 32;  // quadrant edge
+    static constexpr int TM = QS / 4;              // accumulator rows per lane
+    static constexpr int TN = QS / 8;              // accumulator cols per lane
+    static constexpr int STAGE_ROWS = 32;
+    static constexpr int NSTAGE = 2;
+    static constexpr int LDA = KP + 4;   // Cholesky row stride (floats), 16B-aligned rows
+    static constexpr int RPT = KP / NT;  // Cholesky rows per thread
+    static constexpr int YPT = KP / NT;  // rhs elements per thread
+    static constexpr int SLOTF = KP * KP + KP;
+    // CTAs per SM the register file allows (168 regs x 32 lanes x NW warps)
+    static constexpr int OCC = KP >= 128 ? 3 : 12;
+};
+
 template <int NW>
 __device__ __forceinline__ void cta_sync()
 {

@@ -1,4 +1,4 @@
-// als_kernels.cu — ALS half-epoch for sm_100a.
+// als_kernels.cu — ALS half-epoch for sm_90a (SIMT kernel; the tensor-core kernel is als_tc.cu).
 //
 // Replaces the reference's per-row rayon task
 //   src/accel/als/implicit.rs:87-125  (train_row_solve, implicit feedback)
@@ -32,24 +32,6 @@
 #include "als_common.cuh"
 
 namespace lk {
-
-template <int KP>
-struct AlsCfg {
-    static constexpr int QUADS = KP >= 64 ? KP / 64 : 1;
-    static constexpr int NW = QUADS * QUADS;  // warps per CTA
-    static constexpr int NT = NW * 32;
-    static constexpr int QS = KP >= 64 ? 64 : 32;  // quadrant edge
-    static constexpr int TM = QS / 4;              // accumulator rows per lane
-    static constexpr int TN = QS / 8;              // accumulator cols per lane
-    static constexpr int STAGE_ROWS = 32;
-    static constexpr int NSTAGE = 2;
-    static constexpr int LDA = KP + 4;   // Cholesky row stride (floats), 16B-aligned rows
-    static constexpr int RPT = KP / NT;  // Cholesky rows per thread
-    static constexpr int YPT = KP / NT;  // rhs elements per thread
-    static constexpr int SLOTF = KP * KP + KP;
-    // CTAs per SM the register file allows (168 regs x 32 lanes x NW warps)
-    static constexpr int OCC = KP >= 128 ? 3 : 12;
-};
 
 template <int KP, typename ET>
 __host__ __device__ constexpr int als_smem_bytes()
@@ -168,8 +150,8 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, AlsCfg<KP>::OCC) als_half_kern
         fence_proxy_async();
         cta_sync<NW>();
 
-        // accumulators as column pairs: the inner product issues packed FFMA2
-        // (fma.rn.f32x2) — plain FFMA runs at half the fp32 rate on sm_100
+        // accumulators as column pairs (each component is one fma.rn, the same rounding as the
+        // reference's per-element update)
         float2 acc2[TM][TN / 2];
 #pragma unroll
         for (int i = 0; i < TM; i++)
@@ -250,10 +232,11 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, AlsCfg<KP>::OCC) als_half_kern
                 }
 #pragma unroll
                 for (int i = 0; i < TM; i++) {
-                    const float2 a2 = make_float2(ra[i], ra[i]);
 #pragma unroll
-                    for (int c = 0; c < TN / 2; c++)
-                        acc2[i][c] = __ffma2_rn(a2, make_float2(cb[2 * c], cb[2 * c + 1]), acc2[i][c]);
+                    for (int c = 0; c < TN / 2; c++) {
+                        acc2[i][c].x = fmaf(ra[i], cb[2 * c], acc2[i][c].x);
+                        acc2[i][c].y = fmaf(ra[i], cb[2 * c + 1], acc2[i][c].y);
+                    }
                 }
 #pragma unroll
                 for (int q = 0; q < C::YPT; q++)
@@ -447,9 +430,7 @@ __global__ void otor_reduce_kernel(const float *__restrict__ partial, int nblock
     }
 }
 
-int launch_als_tc(const lk_als_args &a, cudaStream_t st);   // als_tc.cu  (bf16 rows, uniform weights)
-int launch_als_tcx(const lk_als_args &a, cudaStream_t st);  // als_tcx.cu (fp32 rows / non-uniform weights, tf32 x3)
-int launch_als_tc128(const lk_als_args &a, cudaStream_t st);  // als_tc128.cu (k = 128: kind::f16 for bf16 rows with uniform weights, tf32 x3 otherwise)
+int launch_als_tc(const lk_als_args &a, cudaStream_t st);  // als_tc.cu (k = 64 / 128: bf16 MMA, or tf32 x3 for fp32 rows / non-uniform weights)
 
 static int pad_features(int k) { return k <= 32 ? 32 : k <= 64 ? 64 : k <= 128 ? 128 : -1; }
 
@@ -588,14 +569,10 @@ int lk_als_half_epoch(const lk_als_args *args, void *stream)
     LK_CUDA_TRY(cudaMemsetAsync(a.d_work_counter, 0, sizeof(int32_t), st));
     if (a.n_split_rows > 0)
         LK_CUDA_TRY(cudaMemsetAsync(a.d_split_counters, 0, sizeof(int32_t) * a.n_split_rows, st));
-    // k = 64: tensor-core kernel (als_tc.cu) unless switched off (option LK_ALS_TC = 0) or the
+    // k = 64 / 128: tensor-core kernel (als_tc.cu) unless switched off (option LK_ALS_TC = 0) or the
     // configuration is outside what it covers (returns 1: fall through to the SIMT kernel)
     if (options().als_tc != 0) {
-        int rc = launch_als_tc(a, st);
-        if (rc <= 0) return rc;
-        rc = launch_als_tcx(a, st);
-        if (rc <= 0) return rc;
-        rc = launch_als_tc128(a, st);
+        const int rc = launch_als_tc(a, st);
         if (rc <= 0) return rc;
     }
     if (a.other_dtype == LK_DTYPE_F32) return dispatch_k<float>(a, st);

@@ -1,760 +1,400 @@
-// als_tc.cu — ALS half-epoch with the Gram matrix on the 5th-gen tensor cores.
+// als_tc.cu — ALS half-epoch with the Gram matrix on the tensor cores (sm_90a, mma.sync).
 //
-// Same contract as als_half_kernel (als_kernels.cu; reference
-// src/accel/als/implicit.rs:87-125, explicit.rs:80-119) for the configuration the
-// headline metric is quoted on: k = 64, the opposite factor table gathered as
-// bf16 rows, and a Gram that is an unweighted (explicit) or uniformly weighted
-// (implicit, use_ratings=False: every confidence equals `weight`) contraction:
+// Same contract as als_half_kernel (als_kernels.cu; reference src/accel/als/implicit.rs:87-125,
+// explicit.rs:80-119) for k = 64 and k = 128, and the same shape of work: a persistent grid pulls
+// chunks from the host plan, one CTA owns one chunk, the gathered rows are staged through shared
+// memory by the TMA engine's bulk-copy path (cp.async.bulk + mbarrier), rows split over several chunks
+// park partial systems in global memory and the last part sums them in slot order, and the k x k system
+// is factored in shared memory (chol_solve, als_common.cuh).  What changes is the Gram:
 //
-//      G = M^T M            M = other[cols, :]   (n x 64, bf16, 128 B per row)
-//      implicit: A = OtOr + v*G      y = sum_j (v_j + 1) m_j
-//      explicit: A = G + reg*n*I     y = sum_j v_j m_j
+//      z_j = s_j * other[c_j, :]      s_j = 1 (uniform weights / explicit) or sqrt(v_j)
+//      G   = sum_j z_j z_j^T          on the tensor cores, fp32 accumulation in registers
+//      implicit: A = OtOr + c * G     c = v (uniform) or 1;   y = sum_j (v_j + 1) o_j
+//      explicit: A = G + reg * n * I                           y = sum_j v_j o_j
 //
-// G is a variable-length SYRK: D[64x64] += A[64 x K] * B[K x 64] with A = M^T and
-// B = M.  Both operands are the *same* shared-memory tile read MN-major (the
-// feature index is the contiguous one), so one gathered row of 64 bf16 is exactly
-// one 128-byte row of the canonical SWIZZLE_128B MN-major layout: the gather is
-// eight 16-byte cp.async per row with the chunk index XORed by (row & 7) — no
-// transposes, no repacking.  One tcgen05.mma (kind::f16, M=64, N=64, K=16) eats
-// 16 gathered rows (65,536 MACs); accumulation is fp32 in TMEM, and because the
-// operands *are* bf16 the products are exact — parity is against the oracle that
-// rounds the gathered rows to bf16 the same way.
-//
-// CTA = 4 warps working in lock-step groups of 4 row-chunks:
-//   phase 1  each warp gathers its own chunk through a 4-stage cp.async ring, one
-//            elected lane issues the MMAs into the warp's TMEM accumulator and
-//            commits them to mbarriers (stage free / accumulator full); with uniform
-//            weights the right-hand side is a second, 8-column MMA against a ones
-//            tile, otherwise it is accumulated on the SIMT side from the same tile;
-//   phase 2  (TCS, default) the systems stay in TMEM: in implicit mode the
-//            accumulators were preloaded with OtOr / v before the group started, so
-//            unsplit rows need nothing; explicit mode adds reg*n to the diagonal in
-//            place.  Chunks of split rows write their accumulator to a partial slot
-//            and the last part to arrive sums the slots in order (deterministic);
-//   phase 3  (TCS) blocked Cholesky of the four systems with the trailing updates
-//            on the tensor cores (chol_tc.cuh), write-back by the row-owner lanes.
-//   Without TCS (LK_ALS_TCS=0) phase 2 drains the accumulators into per-warp
-//   shared-memory systems and phase 3 is one chol_solve per warp (als_common.cuh).
-// A warp can only read its own quarter of the TMEM lanes: for M=64, rows
-// 16w..16w+15 of *every* accumulator.  Two M=64 accumulators share 64 TMEM columns
-// (lanes 0-15 / 16-31 of every quarter, the "interleaved" allocation), so a CTA
-// needs 128 columns (+32 for the right-hand sides).
+// Each warp owns a 64 x 64 quadrant of G as 4 x 8 m16n8 accumulator tiles (128 floats per lane, the
+// SIMT kernel's register footprint).  A = Z^T and B = Z are the same staged tile:
+//   * bf16 rows with unweighted / uniformly weighted Gram: mma.m16n8k16 bf16, operands loaded with
+//     ldmatrix.trans (the tile is feature-contiguous, the MMA wants pairs along the gathered rows).
+//     The products are exact; parity is against the oracle that rounds the gathered rows to bf16.
+//   * fp32 rows, or per-nonzero confidences: every z is split exactly into hi = z with the low 13
+//     mantissa bits cleared (a tf32 number) and lo = z - hi, and G is accumulated as
+//     hi.hi + hi.lo + lo.hi with three mma.m16n8k8 tf32 per 8 gathered rows.  The dropped lo.lo term
+//     and the tf32 truncation of lo are ~2^-22 relative per product, the size of the f32 rounding the
+//     reference's own sgemm makes.
+// Staged rows are KP + 8 elements apart, which makes both the ldmatrix row reads and the tf32 fragment
+// reads bank-conflict free.  Rows past the end of a chunk read as zero (a zero row in shared memory for
+// ldmatrix, a predicate for the scalar reads).
 
-#include "chol_tc.cuh"
+#include <algorithm>
+
+#include "als_common.cuh"
 
 namespace lk {
 
-namespace tc {
-constexpr int KP = 64;
-constexpr int WARPS = 4;
-constexpr int NT = WARPS * 32;
-constexpr int STAGE_ROWS = 32;
-constexpr int NSTAGE = 4;
-constexpr int ROW_BYTES = KP * 2;
-constexpr int STAGE_BYTES = STAGE_ROWS * ROW_BYTES;  // 4096
-constexpr int LDA = KP + 4;
-constexpr int WARP_BYTES = KP * LDA * 4;  // 17408 = 17 * 1024 >= NSTAGE * STAGE_BYTES
-static_assert(WARP_BYTES >= NSTAGE * STAGE_BYTES && WARP_BYTES % 1024 == 0, "stage ring must fit, 1 KB aligned");
-constexpr int TMEM_COLS = 128;
-constexpr int SLOTF = KP * KP + KP;
-constexpr int SMEM_BYTES = 1024 /*alignment slack*/ + WARPS * WARP_BYTES + 2 * WARPS * KP * 4 +
-                           (WARPS * NSTAGE + WARPS + 2) * 8 + 16 + 64 * 4 + 128 + 256 /* ones tile */;
-static_assert(ctc::WS_BYTES <= WARPS * WARP_BYTES, "the tensor-core solve workspace aliases the stage rings");
-constexpr int TMEM_Y_COLS = 32;  // second allocation: 64x8 right-hand-side accumulators
+template <int KP, typename ET, bool WEIGHTED>
+struct TcCfg {
+    using C = AlsCfg<KP>;
+    static constexpr bool BF16MMA = sizeof(ET) == 2 && !WEIGHTED;
+    static constexpr int SROW = KP + 8;  // staged row stride (elements)
+    static constexpr int STAGE_ELTS = C::STAGE_ROWS * SROW;
+    static constexpr int STAGES_BYTES = C::NSTAGE * STAGE_ELTS * (int)sizeof(ET);
+    static constexpr int CHOL_BYTES = KP * C::LDA * 4;
+    static constexpr int UNI = STAGES_BYTES > CHOL_BYTES ? STAGES_BYTES : CHOL_BYTES;
+    static constexpr int ZERO_BYTES = KP * 2;  // one zero bf16 row (ldmatrix target for rows past the end)
+    // union | y[KP] | dinv[KP] | mbarriers | misc | zero row
+    static constexpr int SMEM_BYTES = UNI + KP * 4 + KP * 4 + C::NSTAGE * 8 + 64 + ZERO_BYTES;
+    // operand fragments sit next to the 128 accumulators: fewer resident warps than the SIMT kernel, up to
+    // 255 registers each (8 one-warp CTAs per SM at k = 64, 2 four-warp CTAs at k = 128)
+    static constexpr int OCC = KP >= 128 ? 2 : 8;
+};
 
-// y = M^T w on the tensor cores too (uniform weights: w = (v+1) * ones): D2[64x8] += tile^T . B[16x8]
-// with B a constant 16x8 bf16 tile whose first column is 1 (MN-major, no swizzle: two 8-row core
-// matrices of 128 B).  Instruction descriptor as IDESC with N = 8; B's shared-memory descriptor:
-// LBO = 128 B between the 8-row groups along K, SBO unused, version 1, SWIZZLE_NONE.
-constexpr uint32_t IDESC_Y = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((8u >> 3) << 17) |
-                             ((64u >> 4) << 24);
-constexpr uint64_t DESC_Y_HI = (uint64_t(128 >> 4) << 16) | (uint64_t(128 >> 4) << 32) | (1ull << 46);
-
-using tcd::DESC_HI;
-using tcd::DESC_LBO;
-}  // namespace tc
-
-// interleave != 0: two accumulators share 64 columns (TMEM lanes 0-15 / 16-31 of each
-// quarter), 128 columns per CTA; interleave == 0: one accumulator per 64 columns, 256 per CTA.
-// TCS: the systems stay in TMEM and are solved by the blocked tensor-core Cholesky (chol_tc.cuh,
-// requires the interleaved allocation); otherwise they are drained to shared memory and solved
-// by one warp each (als_common.cuh).
-// GJ (with TCS): block Gauss-Jordan variant of the tensor-core solve (chol_tc.cuh).
-template <int MODE, bool TCS, bool GJ = false>
-__global__ void __launch_bounds__(tc::NT, 3) als_tc_kernel(lk_als_args a, const int interleave, const int flags)
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], uint32_t addr)
 {
-    using namespace tc;
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char *base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    // the warp index goes through a shuffle so that the compiler knows it is warp-uniform: addresses
-    // and descriptors derived from it then live in uniform registers and the tcgen05.mma issue needs
-    // no per-instruction broadcast
-    const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(FULL, tid >> 5, 0);
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+                 : "r"(addr));
+}
 
-    unsigned char *wreg = base + warp * WARP_BYTES;  // this warp's stage ring, later its 64x68 system
-    float *As = reinterpret_cast<float *>(wreg);
-    float *ys_all = reinterpret_cast<float *>(base + WARPS * WARP_BYTES);
-    float *ys = ys_all + warp * KP;
-    float *dinv = ys_all + WARPS * KP + warp * KP;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(ys_all + 2 * WARPS * KP);
-    uint64_t *stage_free = bars + warp * NSTAGE;  // [NSTAGE] of this warp
-    uint64_t *acc_full = bars + WARPS * NSTAGE;   // [WARPS]
-    uint64_t *solve_bar = acc_full + WARPS;       // trailing-update MMAs of the tensor-core solve
-    uint32_t *s_tmem = reinterpret_cast<uint32_t *>(solve_bar + 2);  // solve_bar[1]: second pass of the updates
-    int *s_misc = reinterpret_cast<int *>(s_tmem + 4);  // [0] group, then per-chunk metadata [8 + 8*c ...]
-    unsigned char *ones_tile = reinterpret_cast<unsigned char *>(s_misc + 64);
-    ones_tile += (128u - (smem_u32(ones_tile) & 127u)) & 127u;
-    // the right-hand side goes through the tensor cores when the weights are uniform
-    const bool ymma = (MODE == LK_ALS_IMPLICIT) && interleave != 0;
+__device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1)
+{
+    asm volatile(
+        "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+        "{%0, %1, %2, %3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
 
-    const __nv_bfloat16 *__restrict__ other = reinterpret_cast<const __nv_bfloat16 *>(a.d_other);
+__device__ __forceinline__ void mma_tf32_1688(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1)
+{
+    asm volatile(
+        "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+        "{%0, %1, %2, %3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+__device__ __forceinline__ float tc_elt(float v) { return v; }
+__device__ __forceinline__ float tc_elt(__nv_bfloat16 v) { return __bfloat162float(v); }
+
+// exact split of z into a tf32 number and the f32 remainder
+__device__ __forceinline__ void split_tf32(float z, uint32_t &hi, uint32_t &lo)
+{
+    hi = __float_as_uint(z) & 0xffffe000u;
+    lo = __float_as_uint(z - __uint_as_float(hi));
+}
+
+// MODE: LK_ALS_IMPLICIT / LK_ALS_EXPLICIT.  ET: float or __nv_bfloat16 rows of `other`.  WEIGHTED: implicit
+// mode with per-nonzero confidences (z = sqrt(v) o); otherwise the Gram is unweighted and scaled by the
+// uniform confidence (implicit) or not at all (explicit).
+template <int KP, typename ET, int MODE, bool WEIGHTED>
+__global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)) als_tc_kernel(lk_als_args a)
+{
+    using C = AlsCfg<KP>;
+    using T = TcCfg<KP, ET, WEIGHTED>;
+    constexpr int NW = C::NW, NT = C::NT, LDA = C::LDA, SROW = T::SROW;
+    constexpr bool IMPLICIT = MODE == LK_ALS_IMPLICIT;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    ET *stage0 = reinterpret_cast<ET *>(smem_raw);
+    float *As = reinterpret_cast<float *>(smem_raw);
+    float *ys = reinterpret_cast<float *>(smem_raw + T::UNI);
+    float *dinv = ys + KP;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(dinv + KP);
+    int *s_misc = reinterpret_cast<int *>(bars + C::NSTAGE);
+    unsigned char *zero_row = reinterpret_cast<unsigned char *>(s_misc + 16);
+
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g = lane >> 2, t = lane & 3;
     constexpr int k = KP;
+    const ET *__restrict__ other = reinterpret_cast<const ET *>(a.d_other);
+    constexpr uint32_t ROW_BYTES = (uint32_t)KP * sizeof(ET);
+    // Gram quadrant of this warp
+    const int qi = (warp / C::QUADS) * 64, qj = (warp % C::QUADS) * 64;
+    const float scale = (IMPLICIT && !WEIGHTED) ? a.uniform_val : 1.0f;
 
     if (tid == 0) {
-        for (int i = 0; i < WARPS * NSTAGE + WARPS; i++) mbar_init(&bars[i], 1);
-        mbar_init(solve_bar, 4);
-        mbar_init(solve_bar + 1, 4);
+        for (int s = 0; s < C::NSTAGE; s++) mbar_init(&bars[s], 1);
         mbar_fence_init();
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s_tmem)),
-                     "r"((uint32_t)(interleave ? TMEM_COLS : 2 * TMEM_COLS))
-                     : "memory");
-        if (ymma)
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                             smem_u32(s_tmem + 1)),
-                         "r"((uint32_t)TMEM_Y_COLS)
-                         : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid < 64) {
-        // ones tile: row r (16 B) = bf16 {1, 0, 0, 0, 0, 0, 0, 0}
-        reinterpret_cast<uint32_t *>(ones_tile)[tid] = (tid & 3) == 0 ? 0x00003f80u : 0u;
-    }
-    fence_proxy_async();
-    tmem_fence_before();
+    for (int i = tid; i < T::ZERO_BYTES / 16; i += NT) reinterpret_cast<uint4 *>(zero_row)[i] = make_uint4(0, 0, 0, 0);
     __syncthreads();
-    tmem_fence_after();
-    const uint32_t tmem_base = *s_tmem;
-    const uint32_t tmem_y = ymma ? s_tmem[1] : 0u;
-    // rhs accumulator of warp w: 8 columns per pair, same lane interleave as the Gram
-    const uint32_t my_yacc = tmem_y + ((uint32_t)((warp & 1) * 16) << 16) + (uint32_t)((warp >> 1) * 8);
-    const uint64_t ydesc = DESC_Y_HI | (uint64_t)((smem_u32(ones_tile) >> 4) & 0x3fffu);
-    // accumulator of warp w: columns 64*(w/2), lanes 16*(w%2) of every 32-lane quarter
-    const uint32_t my_acc = interleave
-                                ? tmem_base + ((uint32_t)((warp & 1) * 16) << 16) + (uint32_t)((warp >> 1) * 64)
-                                : tmem_base + (uint32_t)(warp * 64);
+    uint32_t phases = 0;
 
-    // optional per-phase cycle accounting (thread 0's view, barrier waits included)
-    long long t_prev = clock64();
-    auto prof = [&](int idx) {
-        if (a.d_prof != nullptr && tid == 0) {
-            const long long t = clock64();
-            atomicAdd(a.d_prof + idx, (unsigned long long)(t - t_prev));
-            t_prev = t;
-        }
-    };
-
-    uint32_t free_par = 0;  // bit s: parity of the number of commits issued on stage_free[s]
-    uint32_t full_par = 0;  // bit c: parity of the number of commits seen on acc_full[c]
-    uint32_t solve_par = 0;
-
-    // Tensor-core solve, implicit mode: the accumulators start every group holding OtOr / v, the Gram
-    // MMAs accumulate on top, and the finished accumulator is A / v — the drain pass (read 64x64,
-    // fma with OtOr, write back) disappears.  Warp w writes rows 16w..16w+15 of all four systems.
-    constexpr bool PRELOAD = TCS && MODE == LK_ALS_IMPLICIT;
-    auto preload_otor = [&]() {
-        const float rv = 1.0f / a.uniform_val;
-        const float4 *ot = reinterpret_cast<const float4 *>(a.d_otor + (16 * warp + (lane & 15)) * k);
-        uint32_t r[64];
-#pragma unroll
-        for (int q = 0; q < 16; q++) {
-            const float4 o = __ldg(ot + q);
-            r[4 * q + 0] = __float_as_uint(o.x * rv), r[4 * q + 1] = __float_as_uint(o.y * rv);
-            r[4 * q + 2] = __float_as_uint(o.z * rv), r[4 * q + 3] = __float_as_uint(o.w * rv);
-        }
-        const uint32_t t = tmem_base + ((uint32_t)(32 * warp) << 16);
-        ctc::tmem_st64(t, r);
-        ctc::tmem_st64(t + 64u, r);
-        tmem_fence_before();
-    };
-    if constexpr (PRELOAD) preload_otor();
-
-    // the index of the next group is fetched one group ahead (during the solve phase)
-    if (tid == 0) s_misc[0] = fetch_work(a.d_work_counter, a.d_cancel);
-    __syncthreads();
     for (;;) {
-        const int64_t g = __shfl_sync(FULL, s_misc[0], 0);
+        if (tid == 0) s_misc[0] = fetch_work(a.d_work_counter, a.d_cancel);
         __syncthreads();
-        if (g * WARPS >= a.n_chunks) break;
-        prof(0);
-        const int64_t ci = g * WARPS + warp;
-        const bool active = ci < a.n_chunks;
-        int row = -1, begin = 0, len = 0, nparts = 1, slot0 = 0, part = 0, split_idx = 0;
-        if (active) {
-            const int4 c0 = __ldg(reinterpret_cast<const int4 *>(a.d_chunks) + 2 * ci);
-            const int4 c1 = __ldg(reinterpret_cast<const int4 *>(a.d_chunks) + 2 * ci + 1);
-            row = c0.x, begin = c0.y, len = c0.z, nparts = c0.w;
-            slot0 = c1.x, part = c1.y, split_idx = c1.z;
-        }
-        // same value in every lane — say so (see `warp` above)
-        row = __shfl_sync(FULL, row, 0), begin = __shfl_sync(FULL, begin, 0), len = __shfl_sync(FULL, len, 0);
-        nparts = __shfl_sync(FULL, nparts, 0), slot0 = __shfl_sync(FULL, slot0, 0);
-        part = __shfl_sync(FULL, part, 0), split_idx = __shfl_sync(FULL, split_idx, 0);
-        const bool has_gram = active && len > 0;
-        // the row's full length is only needed for the explicit regulariser (reg * n): in implicit mode the
-        // two dependent loads would sit between the chunk record and the first index loads for nothing
-        int n_row = 0;
-        if (MODE == LK_ALS_EXPLICIT && active) n_row = __ldg(a.d_indptr + row + 1) - __ldg(a.d_indptr + row);
-        if (lane == 0) {
-            int *m = s_misc + 8 + 8 * warp;
-            m[0] = has_gram ? 1 : 0;
-            m[1] = nparts;
-            m[2] = slot0 + part;
-            m[3] = n_row;
-            m[4] = slot0;
-            m[5] = row;
-        }
+        const int64_t ci = s_misc[0];
+        __syncthreads();
+        if (ci >= a.n_chunks) break;
+        const int4 c0 = __ldg(reinterpret_cast<const int4 *>(a.d_chunks) + 2 * ci);
+        const int4 c1 = __ldg(reinterpret_cast<const int4 *>(a.d_chunks) + 2 * ci + 1);
+        const int row = c0.x, begin = c0.y, len = c0.z, nparts = c0.w;
+        const int slot0 = c1.x, part = c1.y, split_idx = c1.z;
+        float *thisrow = a.d_this + (size_t)row * k;
 
-        // ------------------------------------------------------------------
-        // phase 1: gather -> tcgen05.mma, y on the side
-        // ------------------------------------------------------------------
-        float y0 = 0.0f, y1 = 0.0f;  // features 2*lane, 2*lane+1
-        if (has_gram) {
-            const int n_it = (len + STAGE_ROWS - 1) / STAGE_ROWS;
-            const int32_t *cols = a.d_cols + begin;
-            const float *vals = a.d_vals + begin;
-            float vst[NSTAGE];  // value of row (it*32 + lane) for the stage in buffer s
-#pragma unroll
-            for (int s = 0; s < NSTAGE; s++) vst[s] = 0.0f;
-
-            // the indices are read once: with flags bit 0 they stream past L1 (no-allocate), which keeps the
-            // 16 KB OtOr matrix of the accumulator preload and the chunk records resident there; the values
-            // are not read at all when the right-hand side goes through the tensor cores (uniform weights)
-            const bool stream = (flags & 1) != 0;
-            auto fetch = [&](int it, int &c, float &v) {
-                const int idx = it * STAGE_ROWS + lane;
-                if (it < n_it && idx < len) {
-                    if (stream) {
-                        c = ld_stream_s32(cols + idx);
-                        v = ymma ? 0.0f : ld_stream_f32(vals + idx);
-                    } else {
-                        c = __ldg(cols + idx);
-                        v = __ldg(vals + idx);
-                    }
-                } else {
-                    c = 0;
-                    v = 0.0f;
-                }
-            };
-            // issue the gather of stage `it` (rows it*32 ..) into ring buffer s; c = this lane's column index
-            auto issue = [&](int it, int s, int c) {
-                if (it < n_it) {
-                    const int nrows = min(STAGE_ROWS, len - it * STAGE_ROWS);
-                    const int npad = (nrows + 15) & ~15;
-                    const uint32_t sbase = smem_u32(wreg + s * STAGE_BYTES);
-                    const int chunk = lane & 7;
-#pragma unroll
-                    for (int t = 0; t < STAGE_ROWS / 4; t++) {
-                        const int r = 4 * t + (lane >> 3);
-                        const int cr = __shfl_sync(FULL, c, r);
-                        const uint32_t dst = sbase + r * ROW_BYTES + ((chunk ^ (r & 7)) << 4);
-                        if (r < nrows) {
-                            cp_async16(dst, other + (size_t)cr * k + chunk * 8);
-                        } else if (r < npad) {
-                            asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};" ::"r"(dst), "r"(0) : "memory");
-                        }
-                    }
-                }
-                cp_async_commit();
-            };
-
-            // Column indices run NSTAGE stages ahead of the gathers that need them (a ring of one index per
-            // stage and lane): with a distance of one stage every gather issue waited out the DRAM latency
-            // of its own index load (~2.5 k cycles per 32-row stage measured), which bounded the phase.
-            int cq[NSTAGE];
-            float vq[NSTAGE];
-#pragma unroll
-            for (int j = 0; j < NSTAGE - 1; j++) fetch(j, cq[j], vq[j]);
-#pragma unroll
-            for (int j = 0; j < NSTAGE - 1; j++) {
-                issue(j, j, cq[j]);
-                vst[j] = vq[j];
+        if (len == 0 && nparts == 1) {
+            // empty row: x = 0, contributes nothing to the delta (implicit.rs:98-101)
+            for (int i = tid; i < k; i += NT) {
+                thisrow[i] = 0.0f;
+                for (int r = 0; r < a.n_replicas; r++)
+                    a.d_replicas[r][(size_t)(a.replica_row0 + row) * k + i] = 0.0f;
             }
-            fetch(NSTAGE - 1, cq[NSTAGE - 1], vq[NSTAGE - 1]);
-#pragma unroll
-            for (int j = 0; j < NSTAGE - 1; j++) fetch(NSTAGE + j, cq[j], vq[j]);
-
-            for (int it0 = 0; it0 < n_it; it0 += NSTAGE) {
-#pragma unroll
-                for (int s = 0; s < NSTAGE; s++) {
-                    const int it = it0 + s;
-                    if (it < n_it) {
-                        // 1. refill the buffer that stage it-1 used (stage it+NSTAGE-1 goes there)
-                        const int sj = (s + NSTAGE - 1) % NSTAGE;  // constant after unrolling
-                        const int j = it + NSTAGE - 1;
-                        if (j < n_it && j >= NSTAGE) {
-                            // the MMAs of iteration it-1 were the last commit on this buffer
-                            mbar_wait(&stage_free[sj], ((free_par >> sj) & 1u) ^ 1u);
-                        }
-                        issue(j, sj, cq[sj]);
-                        if (j < n_it) vst[sj] = vq[sj];
-                        fetch(j + NSTAGE, cq[sj], vq[sj]);  // the slot is free again: index of stage j + NSTAGE
-                        // 2. stage `it` has landed
-                        cp_async_wait<NSTAGE - 1>();
-                        fence_proxy_async();
-                        __syncwarp();
-                        const int nrows = min(STAGE_ROWS, len - it * STAGE_ROWS);
-                        // 3. tensor cores: 16 rows per instruction
-                        if (ctc::elect_one()) {
-                            tmem_fence_after();
-                            const uint32_t sbase = smem_u32(wreg + s * STAGE_BYTES);
-                            const int nk = (nrows + 15) >> 4;
-                            for (int kk = 0; kk < nk; kk++) {
-                                const uint64_t desc =
-                                    DESC_HI | DESC_LBO | (uint64_t)(((sbase + kk * 2048) >> 4) & 0x3fffu);
-                                umma_bf16_64x64x16(my_acc, desc, (PRELOAD || it > 0 || kk > 0) ? 1u : 0u);
-                                if (ymma) umma_bf16_ab(my_yacc, desc, ydesc, IDESC_Y, (it > 0 || kk > 0) ? 1u : 0u);
-                            }
-                            umma_commit(&stage_free[s]);
-                            if (it == n_it - 1) umma_commit(&acc_full[warp]);
-                        }
-                        free_par ^= (1u << s);
-                        // 4. right-hand side from the same tile on the SIMT side when it cannot go
-                        //    through the tensor cores: lane owns features 2*lane, 2*lane+1
-                        if (!ymma) {
-                            const unsigned char *st = wreg + s * STAGE_BYTES;
-                            const int chunk = lane >> 2, within = (lane & 3) * 4;
-                            for (int r = 0; r < nrows; r++) {
-                                float w = __shfl_sync(FULL, vst[s], r);
-                                if constexpr (MODE == LK_ALS_IMPLICIT) w += 1.0f;
-                                const uint32_t two = *reinterpret_cast<const uint32_t *>(
-                                    st + r * ROW_BYTES + ((chunk ^ (r & 7)) << 4) + within);
-                                y0 = fmaf(__uint_as_float(two << 16), w, y0);
-                                y1 = fmaf(__uint_as_float(two & 0xffff0000u), w, y1);
-                            }
-                        }
-                        __syncwarp();
-                    }
-                }
-            }
-            cp_async_wait<0>();
-        }
-        __syncthreads();  // every warp has issued its MMAs; chunk metadata is visible
-        prof(1);
-
-        // ------------------------------------------------------------------
-        // phase 2: drain the accumulators into the per-warp systems
-        // ------------------------------------------------------------------
-        int gram[WARPS], parts[WARPS], slotc[WARPS], nrowc[WARPS];
-#pragma unroll
-        for (int c = 0; c < WARPS; c++) {
-            const int *m = s_misc + 8 + 8 * c;
-            gram[c] = m[0], parts[c] = m[1], slotc[c] = m[2], nrowc[c] = m[3];
-        }
-#pragma unroll
-        for (int c = 0; c < WARPS; c++) {
-            if (gram[c]) {
-                full_par ^= (1u << c);
-                mbar_wait(&acc_full[c], ((full_par >> c) & 1u) ^ 1u);
-            }
-        }
-        tmem_fence_after();
-        prof(2);
-        if constexpr (TCS) {
-            // ------------------------------------------------------------------
-            // phase 2': finish the systems in place in TMEM (A = v*G + OtOr, or G + reg*n*I)
-            // ------------------------------------------------------------------
-            // next group: every thread has read s_misc[0] (barrier at the loop top), so it can be replaced
-            // now; the value is visible to all warps after the barrier that closes this phase
-            if (tid == 0) s_misc[0] = fetch_work(a.d_work_counter, a.d_cancel);
-            const ctc::Workspace ws = ctc::carve(base);  // aliases the stage rings: all their MMAs have completed
-            const int r16 = lane & 15, hh = lane >> 4;
-            const int gi = 16 * warp + r16;  // Gram row / feature held by this lane (of system 2p + hh)
-            const uint32_t lane_taddr = tmem_base + ((uint32_t)(32 * warp) << 16);
-            const bool anysplit = parts[0] > 1 || parts[1] > 1 || parts[2] > 1 || parts[3] > 1;
-            float *dsum = reinterpret_cast<float *>(s_misc + 44);  // [warp][system] partial |delta|^2
-            float yv[2] = {0.0f, 0.0f};
-            if (tid < 4) ws.bad[tid] = 0;
-            if (has_gram && !ymma) {  // SIMT right-hand side of this warp's chunk
-                if (nparts == 1) {
-                    ys[2 * lane] = y0;
-                    ys[2 * lane + 1] = y1;
-                } else {
-                    float *slot = a.d_partials + (size_t)(slot0 + part) * SLOTF + KP * KP;
-                    __stcg(reinterpret_cast<float2 *>(slot) + lane, make_float2(y0, y1));
-                }
-            }
-#pragma unroll
-            for (int p = 0; p < 2; p++) {
-                if (!(gram[2 * p] || gram[2 * p + 1])) continue;
-                if constexpr (MODE == LK_ALS_IMPLICIT) {
-                    // the accumulators were preloaded with OtOr / v (preload_otor): unsplit rows are
-                    // complete as they stand — the system solved is (A / v) x = y / v
-                    if (!((gram[2 * p] && parts[2 * p] > 1) || (gram[2 * p + 1] && parts[2 * p + 1] > 1))) continue;
-                }
-                const int c = 2 * p + hh;
-                uint32_t r[64];
-                tmem_ld_32x32b_x64(lane_taddr + (uint32_t)(p * 64), r);
-                if (gram[c]) {
-                    if (parts[c] == 1) {
-                        if constexpr (MODE == LK_ALS_EXPLICIT) {
-                            const float regn = a.reg * (float)nrowc[c];
-#pragma unroll
-                            for (int i = 0; i < 64; i++)
-                                if (i == gi) r[i] = __float_as_uint(__uint_as_float(r[i]) + regn);
-                        }
-                    } else {
-                        float *slot = a.d_partials + (size_t)slotc[c] * SLOTF + gi * KP;
-#pragma unroll
-                        for (int q = 0; q < 16; q++)
-                            __stcg(reinterpret_cast<float4 *>(slot) + q,
-                                   make_float4(__uint_as_float(r[4 * q + 0]), __uint_as_float(r[4 * q + 1]),
-                                               __uint_as_float(r[4 * q + 2]), __uint_as_float(r[4 * q + 3])));
-                    }
-                }
-                if (MODE == LK_ALS_EXPLICIT &&
-                    ((gram[2 * p] && parts[2 * p] == 1) || (gram[2 * p + 1] && parts[2 * p + 1] == 1)))
-                    ctc::tmem_st64(lane_taddr + (uint32_t)(p * 64), r);
-            }
-            if (ymma) {
-                // unsplit rows: y / v (see above); partial slots keep the unscaled (v + 1) * column sums
-                const float w1 = a.uniform_val + 1.0f;
-                const float rv = 1.0f / a.uniform_val;
-#pragma unroll
-                for (int p = 0; p < 2; p++) {
-                    if (!(gram[2 * p] || gram[2 * p + 1])) continue;
-                    uint32_t ry[8];
-                    tmem_ld_32x32b_x8(tmem_y + ((uint32_t)(32 * warp) << 16) + (uint32_t)(p * 8), ry);
-                    const int c = 2 * p + hh;
-                    if (gram[c]) {
-                        const float yy = w1 * __uint_as_float(ry[0]);
-                        if (parts[c] == 1)
-                            yv[p] = yy * rv;
-                        else
-                            __stcg(a.d_partials + (size_t)slotc[c] * SLOTF + KP * KP + gi, yy);
-                    }
-                }
-            }
-            tmem_fence_before();
-            if (anysplit) __threadfence();  // partial slots only
-            __syncthreads();
-            tmem_fence_after();
-            prof(3);
-            uint32_t solve_mask = 0;
-#pragma unroll
-            for (int c = 0; c < WARPS; c++)
-                if (gram[c] && parts[c] == 1) solve_mask |= 1u << c;
-            if (!ymma) {
-#pragma unroll
-                for (int p = 0; p < 2; p++) {
-                    const int c = 2 * p + hh;
-                    if (gram[c] && parts[c] == 1) yv[p] = ys_all[c * KP + gi];
-                }
-            }
-            // split rows: the last part to arrive sums the slots in order, straight into TMEM
-            if (anysplit) {
-                if (lane == 0)
-                    s_misc[40 + warp] =
-                        (active && nparts > 1 && atomicAdd(a.d_split_counters + split_idx, 1) == nparts - 1) ? 1 : 0;
-                __syncthreads();
-#pragma unroll
-                for (int c = 0; c < WARPS; c++) {
-                    if (!(parts[c] > 1 && s_misc[40 + c])) continue;
-                    __threadfence();
-                    const int p = c >> 1;
-                    const int slot0c = s_misc[8 + 8 * c + 4];
-                    uint32_t r[64];
-                    tmem_ld_32x32b_x64(lane_taddr + (uint32_t)(p * 64), r);
-                    if (hh == (c & 1)) {
-                        const float regn = a.reg * (float)nrowc[c];
-#pragma unroll
-                        for (int q = 0; q < 16; q++) {
-                            float4 sacc = make_float4(0.f, 0.f, 0.f, 0.f);
-                            for (int pp = 0; pp < parts[c]; pp++) {
-                                const float4 t = __ldcg(
-                                    reinterpret_cast<const float4 *>(a.d_partials + (size_t)(slot0c + pp) * SLOTF + gi * KP) +
-                                    q);
-                                sacc.x += t.x, sacc.y += t.y, sacc.z += t.z, sacc.w += t.w;
-                            }
-                            if constexpr (MODE == LK_ALS_IMPLICIT) {
-                                // every part carries one copy of the preloaded OtOr / v: keep exactly one
-                                const float4 o = __ldg(reinterpret_cast<const float4 *>(a.d_otor + gi * k) + q);
-                                const float extra = (float)(parts[c] - 1) / a.uniform_val;
-                                sacc.x = fmaf(-extra, o.x, sacc.x), sacc.y = fmaf(-extra, o.y, sacc.y);
-                                sacc.z = fmaf(-extra, o.z, sacc.z), sacc.w = fmaf(-extra, o.w, sacc.w);
-                            } else {
-                                if (4 * q + 0 == gi) sacc.x += regn;
-                                if (4 * q + 1 == gi) sacc.y += regn;
-                                if (4 * q + 2 == gi) sacc.z += regn;
-                                if (4 * q + 3 == gi) sacc.w += regn;
-                            }
-                            r[4 * q + 0] = __float_as_uint(sacc.x), r[4 * q + 1] = __float_as_uint(sacc.y);
-                            r[4 * q + 2] = __float_as_uint(sacc.z), r[4 * q + 3] = __float_as_uint(sacc.w);
-                        }
-                        float sy = 0.0f;
-                        for (int pp = 0; pp < parts[c]; pp++)
-                            sy += __ldcg(a.d_partials + (size_t)(slot0c + pp) * SLOTF + KP * KP + gi);
-                        yv[p] = (MODE == LK_ALS_IMPLICIT) ? sy / a.uniform_val : sy;
-                    }
-                    ctc::tmem_st64(lane_taddr + (uint32_t)(p * 64), r);
-                    solve_mask |= 1u << c;
-                }
-            }
-            prof(4);
-
-            // ------------------------------------------------------------------
-            // phase 3': blocked Cholesky on the tensor cores, write-back
-            // ------------------------------------------------------------------
-            if (solve_mask) {
-                // old values of the rows about to be written: fetched before the solve, not waited for after it
-                float xold[2] = {0.0f, 0.0f};
-#pragma unroll
-                for (int p = 0; p < 2; p++) {
-                    const int c = 2 * p + hh;
-                    if ((solve_mask >> c) & 1u) xold[p] = a.d_this[(size_t)s_misc[8 + 8 * c + 5] * k + gi];
-                }
-                ctc::solve4<false, GJ>(tmem_base, yv, ws, solve_bar, solve_par, tid);
-                __syncthreads();  // pivot flags
-                prof(7);
-                float dpart[2] = {0.0f, 0.0f};
-#pragma unroll
-                for (int p = 0; p < 2; p++) {
-                    const int c = 2 * p + hh;
-                    if ((solve_mask >> c) & 1u) {
-                        const int rowc = s_misc[8 + 8 * c + 5];
-                        if (ws.bad[c]) {
-                            if (warp == 0 && r16 == 0) atomicCAS(a.d_status, 0, rowc + 1);
-                        } else {
-                            float *tr = a.d_this + (size_t)rowc * k;
-                            const float xn = yv[p];
-                            const float d = xn - xold[p];
-                            dpart[p] = d * d;
-                            tr[gi] = xn;
-                            for (int rr = 0; rr < a.n_replicas; rr++)
-                                a.d_replicas[rr][(size_t)(a.replica_row0 + rowc) * k + gi] = xn;
-                        }
-                    }
-                }
-#pragma unroll
-                for (int p = 0; p < 2; p++) {
-                    float v = dpart[p];
-#pragma unroll
-                    for (int w = 8; w >= 1; w >>= 1) v += __shfl_xor_sync(FULL, v, w, 16);
-                    if (r16 == 0) dsum[warp * 4 + 2 * p + hh] = v;
-                }
-            }
-            if (active && len == 0 && nparts == 1) {
-                // empty row: x = 0, no delta (implicit.rs:98-101)
-                float *thisrow = a.d_this + (size_t)row * k;
-                for (int i = lane; i < k; i += 32) {
-                    thisrow[i] = 0.0f;
-                    for (int rr = 0; rr < a.n_replicas; rr++)
-                        a.d_replicas[rr][(size_t)(a.replica_row0 + row) * k + i] = 0.0f;
-                }
-            }
-            prof(8);
-            if constexpr (PRELOAD) preload_otor();  // accumulators of the next group (this warp's rows)
-            prof(5);
-            __syncthreads();  // the workspace aliases the stage rings of the next group
-            if (tid < 4 && ((solve_mask >> tid) & 1u)) {
-                const float t = ((dsum[tid] + dsum[4 + tid]) + dsum[8 + tid]) + dsum[12 + tid];
-                if (t != 0.0f) atomicAdd(a.d_sqdelta, (double)t);
-            }
-            prof(6);
             continue;
         }
-        const int n_loads = interleave ? 2 : 4;
-        for (int p = 0; p < n_loads; p++) {
-            if (interleave ? !(gram[2 * p] || gram[2 * p + 1]) : !gram[p]) continue;
-            uint32_t r[64];
-            tmem_ld_32x32b_x64(tmem_base + ((uint32_t)(32 * warp) << 16) + (uint32_t)(p * 64), r);
-            const int c = interleave ? 2 * p + (lane >> 4) : p;
-            const int gi = 16 * warp + (lane & 15);  // Gram row held by this lane
-            if (gram[c] && (interleave || lane < 16)) {
-                if (parts[c] == 1) {
-                    float *Ac = reinterpret_cast<float *>(base + c * WARP_BYTES) + gi * LDA;
-                    if constexpr (MODE == LK_ALS_IMPLICIT) {
-                        const float v = a.uniform_val;
-                        const float4 *ot = reinterpret_cast<const float4 *>(a.d_otor + gi * k);
+
+        float acc[4][8][4];
 #pragma unroll
-                        for (int q = 0; q < 16; q++) {
-                            const float4 o = __ldg(ot + q);
-                            float4 t;
-                            t.x = fmaf(v, __uint_as_float(r[4 * q + 0]), o.x);
-                            t.y = fmaf(v, __uint_as_float(r[4 * q + 1]), o.y);
-                            t.z = fmaf(v, __uint_as_float(r[4 * q + 2]), o.z);
-                            t.w = fmaf(v, __uint_as_float(r[4 * q + 3]), o.w);
-                            *reinterpret_cast<float4 *>(Ac + 4 * q) = t;
-                        }
-                    } else {
-                        const float regn = a.reg * (float)nrowc[c];
+        for (int mi = 0; mi < 4; mi++)
 #pragma unroll
-                        for (int q = 0; q < 16; q++) {
-                            float4 t = make_float4(__uint_as_float(r[4 * q + 0]), __uint_as_float(r[4 * q + 1]),
-                                                   __uint_as_float(r[4 * q + 2]), __uint_as_float(r[4 * q + 3]));
-                            if (gi >> 2 == q) {
-                                if ((gi & 3) == 0) t.x += regn;
-                                if ((gi & 3) == 1) t.y += regn;
-                                if ((gi & 3) == 2) t.z += regn;
-                                if ((gi & 3) == 3) t.w += regn;
-                            }
-                            *reinterpret_cast<float4 *>(Ac + 4 * q) = t;
+            for (int nj = 0; nj < 8; nj++)
+#pragma unroll
+                for (int r = 0; r < 4; r++) acc[mi][nj][r] = 0.0f;
+        float yacc[C::YPT];
+#pragma unroll
+        for (int q = 0; q < C::YPT; q++) yacc[q] = 0.0f;
+
+        const int n_it = (len + 31) >> 5;
+        const int32_t *cols = a.d_cols + begin;
+        const float *vals = a.d_vals + begin;
+        int cA = -1, cB = -1, cC = -1;
+        float vA = 0.f, vB = 0.f, vC = 0.f;
+        if (lane < len) {
+            cA = __ldg(cols + lane);
+            vA = __ldg(vals + lane);
+        }
+        if (32 + lane < len) {
+            cB = __ldg(cols + 32 + lane);
+            vB = __ldg(vals + 32 + lane);
+        }
+
+        auto issue = [&](int it, int c) {
+            const int s = it & 1;
+            const int nrows = min(32, len - it * 32);
+            ET *dst = stage0 + s * T::STAGE_ELTS;
+            if (warp == 0) {
+                if (lane == 0) mbar_arrive_expect_tx(&bars[s], (uint32_t)nrows * ROW_BYTES);
+                if (lane < nrows) bulk_g2s(dst + lane * SROW, other + (size_t)c * k, ROW_BYTES, &bars[s]);
+            }
+        };
+
+        issue(0, cA);
+        for (int it = 0; it < n_it; it++) {
+            const int s = it & 1;
+            // column indices two stages ahead
+            if ((it + 2) * 32 + lane < len) {
+                cC = __ldg(cols + (it + 2) * 32 + lane);
+                vC = __ldg(vals + (it + 2) * 32 + lane);
+            } else {
+                cC = -1;
+                vC = 0.f;
+            }
+            if (it + 1 < n_it) issue(it + 1, cB);
+            mbar_wait(&bars[s], (phases >> s) & 1u);
+            phases ^= (1u << s);
+            const int nrows = min(32, len - it * 32);
+            const ET *st = stage0 + s * T::STAGE_ELTS;
+
+            // right-hand side, as the SIMT kernel computes it
+            for (int r = 0; r < nrows; r++) {
+                const float v = __shfl_sync(FULL, vA, r);
+                const float w = IMPLICIT ? v + 1.0f : v;
+#pragma unroll
+                for (int q = 0; q < C::YPT; q++) yacc[q] = fmaf(tc_elt(st[r * SROW + tid + q * NT]), w, yacc[q]);
+            }
+
+            if constexpr (T::BF16MMA) {
+                const uint32_t sbase = smem_u32(st), zaddr = smem_u32(zero_row);
+                const int lr = lane & 7, lm = lane >> 3;
+                for (int k0 = 0; k0 < nrows; k0 += 16) {
+                    // A = Z^T: matrices (rows k0.., m0), (k0.., m0+8), (k0+8.., m0), (k0+8.., m0+8)
+                    uint32_t af[4][4], bfr[4][4];
+                    const int ra = k0 + lr + 8 * (lm >> 1);
+#pragma unroll
+                    for (int mi = 0; mi < 4; mi++) {
+                        const int col = qi + 16 * mi + 8 * (lm & 1);
+                        ldmatrix_x4_trans(af[mi], ra < nrows ? sbase + (uint32_t)((ra * SROW + col) * 2) : zaddr);
+                    }
+                    // B = Z: matrices (rows k0.., n0), (k0+8.., n0), (k0.., n0+8), (k0+8.., n0+8)
+                    const int rb = k0 + lr + 8 * (lm & 1);
+#pragma unroll
+                    for (int np = 0; np < 4; np++) {
+                        const int col = qj + 16 * np + 8 * (lm >> 1);
+                        ldmatrix_x4_trans(bfr[np], rb < nrows ? sbase + (uint32_t)((rb * SROW + col) * 2) : zaddr);
+                    }
+#pragma unroll
+                    for (int mi = 0; mi < 4; mi++)
+#pragma unroll
+                        for (int nj = 0; nj < 8; nj++)
+                            mma_bf16_16816(acc[mi][nj], af[mi], bfr[nj >> 1][2 * (nj & 1)], bfr[nj >> 1][2 * (nj & 1) + 1]);
+                }
+            } else {
+                const float sq = WEIGHTED ? sqrtf(vA) : 1.0f;  // rows past the end carry v = 0
+                for (int k0 = 0; k0 < nrows; k0 += 8) {
+                    const int r0 = k0 + t, r1 = k0 + t + 4;
+                    const bool ok0 = r0 < nrows, ok1 = r1 < nrows;
+                    const float s0 = WEIGHTED ? __shfl_sync(FULL, sq, r0) : 1.0f;
+                    const float s1 = WEIGHTED ? __shfl_sync(FULL, sq, r1) : 1.0f;
+                    const ET *p0 = st + r0 * SROW, *p1 = st + r1 * SROW;
+                    auto z = [&](bool ok, const ET *p, float s, int c) { return ok ? s * tc_elt(p[c]) : 0.0f; };
+                    uint32_t bh[8][2], bl[8][2];
+#pragma unroll
+                    for (int nj = 0; nj < 8; nj++) {
+                        split_tf32(z(ok0, p0, s0, qj + 8 * nj + g), bh[nj][0], bl[nj][0]);
+                        split_tf32(z(ok1, p1, s1, qj + 8 * nj + g), bh[nj][1], bl[nj][1]);
+                    }
+#pragma unroll
+                    for (int mi = 0; mi < 4; mi++) {
+                        uint32_t ah[4], al[4];
+                        const int m0 = qi + 16 * mi + g;
+                        split_tf32(z(ok0, p0, s0, m0), ah[0], al[0]);
+                        split_tf32(z(ok0, p0, s0, m0 + 8), ah[1], al[1]);
+                        split_tf32(z(ok1, p1, s1, m0), ah[2], al[2]);
+                        split_tf32(z(ok1, p1, s1, m0 + 8), ah[3], al[3]);
+#pragma unroll
+                        for (int nj = 0; nj < 8; nj++) {
+                            mma_tf32_1688(acc[mi][nj], ah, bh[nj][0], bh[nj][1]);
+                            mma_tf32_1688(acc[mi][nj], ah, bl[nj][0], bl[nj][1]);
+                            mma_tf32_1688(acc[mi][nj], al, bh[nj][0], bh[nj][1]);
                         }
                     }
-                } else {
-                    float *slot = a.d_partials + (size_t)slotc[c] * SLOTF + gi * KP;
-#pragma unroll
-                    for (int q = 0; q < 16; q++)
-                        __stcg(reinterpret_cast<float4 *>(slot) + q,
-                               make_float4(__uint_as_float(r[4 * q + 0]), __uint_as_float(r[4 * q + 1]),
-                                           __uint_as_float(r[4 * q + 2]), __uint_as_float(r[4 * q + 3])));
                 }
             }
+            cta_sync<NW>();  // everyone is done with stage s before it is re-armed
+            cA = cB;
+            vA = vB;
+            cB = cC;
+            vB = vC;
         }
-        if (ymma) {
-            // right-hand sides from their TMEM accumulators: y = (v + 1) * column sums
-            const float w1 = a.uniform_val + 1.0f;
+
+        // accumulator (mi, nj, r) holds G[qi + 16 mi + g + 8 (r / 2)][qj + 8 nj + 2 t + r % 2]
+        if (scale != 1.0f) {
 #pragma unroll
-            for (int p = 0; p < 2; p++) {
-                if (!(gram[2 * p] || gram[2 * p + 1])) continue;
-                uint32_t ry[8];
-                tmem_ld_32x32b_x8(tmem_y + ((uint32_t)(32 * warp) << 16) + (uint32_t)(p * 8), ry);
-                const int c = 2 * p + (lane >> 4);
-                const int gi = 16 * warp + (lane & 15);
-                if (gram[c]) {
-                    const float yy = w1 * __uint_as_float(ry[0]);
-                    if (parts[c] == 1)
-                        ys_all[c * KP + gi] = yy;
-                    else
-                        __stcg(a.d_partials + (size_t)slotc[c] * SLOTF + KP * KP + gi, yy);
+            for (int mi = 0; mi < 4; mi++)
+#pragma unroll
+                for (int nj = 0; nj < 8; nj++)
+#pragma unroll
+                    for (int r = 0; r < 4; r++) acc[mi][nj][r] *= scale;
+        }
+
+        // ---- rows split over several chunks: park the partial, last part reduces
+        if (nparts > 1) {
+            float *slot = a.d_partials + (size_t)(slot0 + part) * C::SLOTF;
+#pragma unroll
+            for (int mi = 0; mi < 4; mi++)
+#pragma unroll
+                for (int nj = 0; nj < 8; nj++)
+#pragma unroll
+                    for (int h = 0; h < 2; h++)
+                        __stcg(reinterpret_cast<float2 *>(slot + (qi + 16 * mi + g + 8 * h) * KP + qj + 8 * nj + 2 * t),
+                               make_float2(acc[mi][nj][2 * h], acc[mi][nj][2 * h + 1]));
+#pragma unroll
+            for (int q = 0; q < C::YPT; q++) __stcg(slot + KP * KP + tid + q * NT, yacc[q]);
+            __threadfence();
+            __syncthreads();
+            if (tid == 0) {
+                int old = atomicAdd(a.d_split_counters + split_idx, 1);
+                s_misc[1] = (old == nparts - 1);
+            }
+            __syncthreads();
+            const bool last = s_misc[1] != 0;
+            __syncthreads();
+            if (!last) continue;
+            __threadfence();
+#pragma unroll
+            for (int mi = 0; mi < 4; mi++)
+#pragma unroll
+                for (int nj = 0; nj < 8; nj++)
+#pragma unroll
+                    for (int r = 0; r < 4; r++) acc[mi][nj][r] = 0.0f;
+#pragma unroll
+            for (int q = 0; q < C::YPT; q++) yacc[q] = 0.0f;
+            for (int p = 0; p < nparts; p++) {
+                const float *sp = a.d_partials + (size_t)(slot0 + p) * C::SLOTF;
+#pragma unroll
+                for (int mi = 0; mi < 4; mi++)
+#pragma unroll
+                    for (int nj = 0; nj < 8; nj++)
+#pragma unroll
+                        for (int h = 0; h < 2; h++) {
+                            const float2 v = __ldcg(
+                                reinterpret_cast<const float2 *>(sp + (qi + 16 * mi + g + 8 * h) * KP + qj + 8 * nj + 2 * t));
+                            acc[mi][nj][2 * h] += v.x;
+                            acc[mi][nj][2 * h + 1] += v.y;
+                        }
+#pragma unroll
+                for (int q = 0; q < C::YPT; q++) yacc[q] += __ldcg(sp + KP * KP + tid + q * NT);
+            }
+        }
+
+        // ---- assemble A (+ OtOr | + reg*n*I) and y in shared memory
+        const int n_row = __ldg(a.d_indptr + row + 1) - __ldg(a.d_indptr + row);
+        const float regn = a.reg * (float)n_row;
+#pragma unroll
+        for (int mi = 0; mi < 4; mi++)
+#pragma unroll
+            for (int nj = 0; nj < 8; nj++)
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const int gi = qi + 16 * mi + g + 8 * h, gc = qj + 8 * nj + 2 * t;
+                    float v0 = acc[mi][nj][2 * h], v1 = acc[mi][nj][2 * h + 1];
+                    if constexpr (IMPLICIT) {
+                        const float2 o = __ldg(reinterpret_cast<const float2 *>(a.d_otor + gi * k + gc));
+                        v0 = o.x + v0;  // a = otor + mtm (implicit.rs:115)
+                        v1 = o.y + v1;
+                    } else {
+                        if (gi == gc) v0 += regn;  // explicit.rs:106-108
+                        if (gi == gc + 1) v1 += regn;
+                    }
+                    *reinterpret_cast<float2 *>(As + gi * LDA + gc) = make_float2(v0, v1);
                 }
-            }
-        }
-        tmem_fence_before();
-        // right-hand side of this warp's chunk (SIMT path)
-        if (has_gram && !ymma) {
-            if (nparts == 1) {
-                ys[2 * lane] = y0;
-                ys[2 * lane + 1] = y1;
-            } else {
-                float *slot = a.d_partials + (size_t)(slot0 + part) * SLOTF + KP * KP;
-                __stcg(reinterpret_cast<float2 *>(slot) + lane, make_float2(y0, y1));
-            }
-        }
-        if (parts[0] > 1 || parts[1] > 1 || parts[2] > 1 || parts[3] > 1) __threadfence();  // partial slots only
+#pragma unroll
+        for (int q = 0; q < C::YPT; q++) ys[tid + q * NT] = yacc[q];
+        cta_sync<NW>();
+
+        // ---- Cholesky + triangular solves in shared memory, then write the row
+        const bool bad = chol_solve<KP, NW>(As, ys, dinv, tid);
+        write_row<KP, NW>(a, row, thisrow, ys, tid, bad);
+        // the next chunk's bulk copies (async proxy) overwrite this buffer
+        fence_proxy_async();
         __syncthreads();
-        prof(3);
-
-        // split rows: the last part to arrive sums the slots in order
-        bool solve = has_gram && nparts == 1;
-        if (active && nparts > 1) {
-            int last = 0;
-            if (lane == 0) last = (atomicAdd(a.d_split_counters + split_idx, 1) == nparts - 1) ? 1 : 0;
-            last = __shfl_sync(FULL, last, 0);
-            if (last) {
-                __threadfence();
-                const float regn = a.reg * (float)n_row;
-                for (int idx = lane; idx < KP * KP; idx += 32) {
-                    float s = 0.0f;
-                    for (int p = 0; p < nparts; p++) s += __ldcg(a.d_partials + (size_t)(slot0 + p) * SLOTF + idx);
-                    const int gi = idx >> 6, gc = idx & 63;
-                    if constexpr (MODE == LK_ALS_IMPLICIT)
-                        s = fmaf(a.uniform_val, s, __ldg(a.d_otor + idx));
-                    else if (gi == gc)
-                        s += regn;
-                    As[gi * LDA + gc] = s;
-                }
-                for (int f = lane; f < KP; f += 32) {
-                    float s = 0.0f;
-                    for (int p = 0; p < nparts; p++)
-                        s += __ldcg(a.d_partials + (size_t)(slot0 + p) * SLOTF + KP * KP + f);
-                    ys[f] = s;
-                }
-                solve = true;
-            }
-        }
-        __syncwarp();
-        prof(4);
-
-        // ------------------------------------------------------------------
-        // phase 3: per-warp Cholesky solve and write-back
-        // ------------------------------------------------------------------
-        if (tid == 0) s_misc[0] = fetch_work(a.d_work_counter, a.d_cancel);  // next group, read after the closing barrier
-        if (active) {
-            float *thisrow = a.d_this + (size_t)row * k;
-            if (solve) {
-                const bool bad = chol_solve<KP, 1>(As, ys, dinv, lane);
-                write_row<KP, 1>(a, row, thisrow, ys, lane, bad);
-            } else if (len == 0 && nparts == 1) {
-                // empty row: x = 0, no delta (implicit.rs:98-101)
-                for (int i = lane; i < k; i += 32) {
-                    thisrow[i] = 0.0f;
-                    for (int rr = 0; rr < a.n_replicas; rr++)
-                        a.d_replicas[rr][(size_t)(a.replica_row0 + row) * k + i] = 0.0f;
-                }
-            }
-        }
-        prof(5);
-        __syncthreads();  // the systems alias the stage rings of the next group
-        prof(6);
-    }
-
-    tmem_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        if (ymma)
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_y),
-                         "r"((uint32_t)tc::TMEM_Y_COLS)
-                         : "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                     "r"((uint32_t)(interleave ? tc::TMEM_COLS : 2 * tc::TMEM_COLS))
-                     : "memory");
     }
 }
 
-// returns LK_OK when the tensor-core kernel took the launch, 1 when the caller
-// should fall back to the SIMT kernel
-int launch_als_tc(const lk_als_args &a, cudaStream_t st)
+template <int KP, typename ET, int MODE, bool WEIGHTED>
+static int launch_tc(const lk_als_args &a, cudaStream_t st)
 {
-    if (a.k != tc::KP || a.other_dtype != LK_DTYPE_BF16) return 1;
-    if (a.mode == LK_ALS_IMPLICIT && !a.vals_uniform) return 1;
-    if (reinterpret_cast<uintptr_t>(a.d_other) % 16 != 0) return 1;
-    const Options &opt = options();
-    const int interleave = opt.als_tc_interleave != 0;
-    const int cols = interleave ? tc::TMEM_COLS : 2 * tc::TMEM_COLS;
-    const int smem = tc::SMEM_BYTES;
-    int64_t groups = (a.n_chunks + tc::WARPS - 1) / tc::WARPS;
-    // 3 CTAs per SM by shared memory (73 KB) and registers; TMEM allows 512 / cols.  (The occupancy
-    // API returned 1 for the user-half launch on the B200 box, so the design figure is used.)
-    int occ = 3;
-    if (opt.als_tc_occ > 0) occ = std::max(1, std::min(3, opt.als_tc_occ));  // diagnostics
-    // LK_ALS_TCS=0 keeps the per-warp shared-memory solve (diagnostics); default: tensor-core solve
-    const bool tcs_opt = interleave != 0 && opt.als_tcs != 0;
-    bool tcs = tcs_opt;
-    // the tensor-core path solves (A / v) x = y / v: not for a zero confidence weight
-    if (a.mode == LK_ALS_IMPLICIT && !(fabsf(a.uniform_val) > 1e-20f)) tcs = false;
-    occ = std::max(1, std::min(occ, 512 / (cols + tc::TMEM_Y_COLS)));
-    const int64_t grid = std::max<int64_t>(1, std::min<int64_t>((int64_t)sm_count() * occ, groups));
-    auto launch = [&](auto kern) -> int {
-        LK_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        kern<<<(unsigned)grid, tc::NT, smem, st>>>(a, interleave, opt.als_flags);
-        return LK_OK;
-    };
-    // LK_ALS_GJ=1: block Gauss-Jordan instead of blocked Cholesky + block back substitution (experiment)
-    const bool gj = opt.als_gj != 0;
-    int rc;
-    if (a.mode == LK_ALS_IMPLICIT)
-        rc = !tcs  ? launch(als_tc_kernel<LK_ALS_IMPLICIT, false>)
-             : gj  ? launch(als_tc_kernel<LK_ALS_IMPLICIT, true, true>)
-                   : launch(als_tc_kernel<LK_ALS_IMPLICIT, true, false>);
-    else
-        rc = !tcs  ? launch(als_tc_kernel<LK_ALS_EXPLICIT, false>)
-             : gj  ? launch(als_tc_kernel<LK_ALS_EXPLICIT, true, true>)
-                   : launch(als_tc_kernel<LK_ALS_EXPLICIT, true, false>);
-    if (rc != LK_OK) return rc;
+    using T = TcCfg<KP, ET, WEIGHTED>;
+    auto kern = als_tc_kernel<KP, ET, MODE, WEIGHTED>;
+    LK_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SMEM_BYTES));
+    int occ = 0;
+    LK_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, AlsCfg<KP>::NT, T::SMEM_BYTES));
+    const int64_t grid = std::max<int64_t>(1, std::min<int64_t>((int64_t)sm_count() * std::max(occ, 1), a.n_chunks));
+    kern<<<(unsigned)grid, AlsCfg<KP>::NT, T::SMEM_BYTES, st>>>(a);
     LK_CUDA_TRY(cudaGetLastError());
     return LK_OK;
+}
+
+template <int KP, typename ET>
+static int dispatch_tc(const lk_als_args &a, cudaStream_t st, bool weighted)
+{
+    if (a.mode == LK_ALS_EXPLICIT) return launch_tc<KP, ET, LK_ALS_EXPLICIT, false>(a, st);
+    return weighted ? launch_tc<KP, ET, LK_ALS_IMPLICIT, true>(a, st) : launch_tc<KP, ET, LK_ALS_IMPLICIT, false>(a, st);
+}
+
+// returns LK_OK when the tensor-core kernel took the launch, 1 when the caller should use the SIMT kernel
+int launch_als_tc(const lk_als_args &a, cudaStream_t st)
+{
+    if (a.k != 64 && a.k != 128) return 1;
+    if (reinterpret_cast<uintptr_t>(a.d_other) % 16 != 0) return 1;
+    const bool f32 = a.other_dtype == LK_DTYPE_F32;
+    const bool weighted = a.mode == LK_ALS_IMPLICIT && !a.vals_uniform;
+    // the weighted Gram uses z = sqrt(v) o: confidences must not be negative (the plan passes the minimum)
+    if (weighted && !(a.uniform_val >= 0.0f)) return 1;
+    // LK_ALS_TF32 = 0: fp32 rows and per-nonzero confidences stay on the SIMT kernel
+    if ((f32 || weighted) && options().als_tf32 == 0) return 1;
+    if (a.k == 64)
+        return f32 ? dispatch_tc<64, float>(a, st, weighted) : dispatch_tc<64, __nv_bfloat16>(a, st, weighted);
+    return f32 ? dispatch_tc<128, float>(a, st, weighted) : dispatch_tc<128, __nv_bfloat16>(a, st, weighted);
 }
 
 }  // namespace lk

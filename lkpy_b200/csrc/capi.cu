@@ -28,12 +28,7 @@ struct OptionDef {
 };
 static const OptionDef OPTION_DEFS[] = {
     {"LK_ALS_TC", &Options::als_tc},
-    {"LK_ALS_TC_INTERLEAVE", &Options::als_tc_interleave},
-    {"LK_ALS_TC_OCC", &Options::als_tc_occ},
-    {"LK_ALS_TCS", &Options::als_tcs},
-    {"LK_ALS_GJ", &Options::als_gj},
     {"LK_ALS_TF32", &Options::als_tf32},
-    {"LK_ALS_FLAGS", &Options::als_flags},
     {"LK_KNN_WARPS", &Options::knn_warps},
     {"LK_KNN_CTAS", &Options::knn_ctas},
     {"LK_KNN_SCORE_SEQ", &Options::knn_score_seq},
@@ -61,7 +56,7 @@ int sm_count()
             cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
             cached = n;
         else
-            return 148;
+            return 132;  // H100 SXM
     }
     return cached;
 }

@@ -1,4 +1,4 @@
-// common.cuh — shared device/host helpers for the sm_100a kernels.
+// common.cuh — shared device/host helpers for the sm_90a kernels.
 #pragma once
 
 #include <cuda_bf16.h>
@@ -38,12 +38,7 @@ int sm_count();
 // first use and afterwards only through lk_set_option.  -1 = "not set, use the built-in choice".
 struct Options {
     int als_tc = 1;             // 0: SIMT ALS kernel even where the tensor-core kernel applies
-    int als_tc_interleave = 1;  // 0: one accumulator per 64 TMEM columns (shared-memory solve only)
-    int als_tc_occ = -1;        // cap on resident CTAs per SM of the tensor-core kernel
-    int als_tcs = 1;            // 0: drain the systems to shared memory, one warp per solve
-    int als_gj = 1;             // 0: blocked Cholesky + block back substitution instead of block Gauss-Jordan (als_tc.cu)
     int als_tf32 = 1;           // 0: fp32 / non-uniformly weighted rows stay on the SIMT kernel
-    int als_flags = 1;          // als_tc_kernel: bit 0 streaming (L1 no-allocate) index loads
     int knn_warps = -1;         // warps per CTA of the kNN build (8, 16, 32)
     int knn_ctas = -1;          // resident CTAs per SM of the kNN build
     int knn_score_seq = 0;      // 1: sequential scoring kernel even with a contribution pool

@@ -1,4 +1,4 @@
-// knn_build.cu — item-item similarity build for sm_100a.
+// knn_build.cu — item-item similarity build for sm_90a.
 //
 // Replaces src/accel/knn/item_train.rs:65-152 (ItemSimTask::invoke, sim_row):
 // row i of IU * UI by Gustavson accumulation, `>= min_sim` filter, optional
@@ -251,7 +251,7 @@ __global__ void __launch_bounds__(W * 32, 1024 / (W * 32)) knn_build_kernel(lk_k
                     // users in ascending order, one user per round: the lanes of one user hit distinct columns.
                     // (Grouping lanes by column instead — __match_any_sync, or one ballot per column bit — was
                     // measured slower on ML-25M-shaped data: a popular column is present in most users'
-                    // segments, so the rounds per batch stay near the number of users; profiles/r02_experiments.md.)
+                    // segments, so the rounds per batch stay near the number of users.)
                     unsigned pend = __ballot_sync(FULL, valid);
                     while (pend) {
                         const int leader = __ffs(pend) - 1;

@@ -1,4 +1,4 @@
-// knn_score.cu — batched item-kNN neighbourhood scoring for sm_100a.
+// knn_score.cu — batched item-kNN neighbourhood scoring for sm_90a.
 //
 // Replaces src/accel/knn/item_score.rs:22-111 (score_explicit / score_implicit)
 // and the ScoreAccumulator of src/accel/knn/accum.rs:16-239, batched over many

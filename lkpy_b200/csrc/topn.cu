@@ -1,4 +1,4 @@
-// topn.cu — batched top-N selection for sm_100a.
+// topn.cu — batched top-N selection for sm_90a.
 //
 // Replaces lenskit._accel.data.argtopn (src/accel/data/sorting.rs:131-170) — the
 // step behind ItemList.top_n / TopNRanker (src/lenskit/data/_items.py:942-998,

@@ -4,7 +4,7 @@ Interaction-matrix inputs for the ALS / item-kNN hot paths.
 Two sources, both host-side (NumPy) and both setup rather than hot path:
 
 * ``load_ml_small()`` — the reference's vendored ``ml-latest-small`` ratings
-  (``/root/reference/data/ml-latest-small/ratings.csv``; 671 users x 9,066
+  (LensKit's ``data/ml-latest-small/ratings.csv``, stored as tests/golden/ml_small.npz; 671 users x 9,066
   items, 100,004 ratings) repacked by ``tests/golden/make_golden.py`` into a
   compact ``.npz`` fixture, with ids numbered by sorted unique id the way the
   reference's ``Vocabulary`` does for ``from_interactions_df`` input

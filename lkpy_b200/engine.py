@@ -20,13 +20,12 @@ from ._lib import LkAlsArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnScoreArgs, check, l
 from .data import InteractionCSR
 
 DEFAULT_CHUNK_NNZ = 4096
-#: rows of the fp32 / weighted tensor-core path (als_tcx.cu) are cut shorter: a tcgen05 accumulator adds with
-#: round-toward-zero, three times per 8 gathered rows on that path, so the error of a partial Gram grows with
-#: its length (measured ~2.3e-8 relative per nonzero); parts are summed with round-to-nearest by the CUDA cores
+#: rows of the fp32 / weighted tensor-core path (als_tc.cu, tf32 x3) are cut shorter, and the parts are summed with
+#: round-to-nearest by the CUDA cores.  These lengths were chosen for an earlier tensor-core design whose
+#: accumulators truncated; they are carried over unmeasured for the mma.sync accumulator of the H100 kernel
 TF32_CHUNK_NNZ = 1024
-#: fp32 rows / per-nonzero weights at k = 128: the 128x128 solve amplifies the same Gram bias further — 1024-nonzero
-#: parts put the 100 M-interaction item rows at 2.0e-4 (8 GPUs, profiles/r02_als100m_n8.json), a quarter of that
-#: length keeps them inside the 1e-4 tolerance
+#: fp32 rows / per-nonzero weights at k = 128: a quarter of that length (carried over the same way; it kept the
+#: 100 M-interaction item rows inside the 1e-4 tolerance on that design)
 TF32_CHUNK_NNZ_K128 = 256
 #: engine limits the reference does not have (DESIGN.md §6): validated up front by the configs
 ALS_MAX_FEATURES = 128

@@ -1,5 +1,5 @@
 """
-Item-kNN scorer on the B200 engine — the component surface of
+Item-kNN scorer on the H100 engine — the component surface of
 ``lenskit.knn.item.ItemKNNScorer`` (``src/lenskit/knn/item.py:41-295``).
 
 Same config fields / aliases (``max_nbrs``/``nnbrs``/``k``, ``min_nbrs``,

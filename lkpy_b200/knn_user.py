@@ -1,5 +1,5 @@
 """
-User-kNN scorer on the B200 engine (SURVEY.md §8f N3) — the component surface of
+User-kNN scorer on the H100 engine (SURVEY.md §8f N3) — the component surface of
 ``lenskit.knn.user.UserKNNScorer`` (``src/lenskit/knn/user.py:41-300``).
 
 Training memorises the centred ratings and the unit-normalised user vectors exactly as the reference

@@ -11,7 +11,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100, sm_90a); run with -m gpu on a GPU machine")
 
 
 def pytest_collection_modifyitems(config, items):

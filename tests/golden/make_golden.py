@@ -2,7 +2,7 @@
 """
 Generate the committed golden fixtures in this directory.
 
-Run in the build container only (needs ``/root/reference``); nothing at test,
+Run with ``LENSKIT_REFERENCE_SRC`` naming a LensKit source checkout; nothing at test,
 smoke or bench time reads the reference tree.  The reference package cannot be
 imported as a whole here (its Rust extension ``lenskit._accel`` is not built and
 several Python dependencies are absent), so the pure-Python reference functions
@@ -29,6 +29,7 @@ knn_prep.npz            ItemKNNScorer._center_ratings / _normalize_rows
 
 from __future__ import annotations
 
+import os
 import ast
 import hashlib
 import shutil
@@ -42,7 +43,7 @@ import scipy.sparse.linalg as spla
 from scipy.linalg import cho_factor, cho_solve
 from scipy.sparse import coo_array, sparray
 
-REF = Path("/root/reference")
+REF = Path(os.environ["LENSKIT_REFERENCE_SRC"])  # a LensKit source checkout
 OUT = Path(__file__).resolve().parent
 
 

@@ -1,8 +1,8 @@
 """
 Test harness: the reference's OWN Python classes for the hot path — ``lenskit.training``,
 ``lenskit.pipeline.components.Component``, ``lenskit.data.matrix.SparseRowArray``, ``ItemList``, ``Vocabulary``,
-``RecQuery``, ``basic.bias.BiasModel``, ``lenskit.als._common / _implicit / _explicit``, ``lenskit.knn.item / user`` — loaded from ``/root/reference`` file
-by file, with ``lenskit._accel`` bound to ``lkpy_b200.accel`` exactly as INTEGRATION.md §1 describes.
+``RecQuery``, ``basic.bias.BiasModel``, ``lenskit.als._common / _implicit / _explicit``, ``lenskit.knn.item / user`` — loaded from a LensKit
+source checkout (see ``reference_root``) file by file, with ``lenskit._accel`` bound to ``lkpy_b200.accel`` exactly as INTEGRATION.md §1 describes.
 
 The reference package cannot be imported as a whole here (its ``__init__`` needs ``lazy_loader`` /
 ``structlog``, its data layer needs the Rust extension's ``IDIndex`` / ``CoordinateTable``), so the modules
@@ -12,13 +12,14 @@ the Rust helpers of the data model (``IDIndex``, ``scatter_array`` ...), and the
 trainers read (``Dataset.interactions().matrix().scipy(...)``, the vocabularies).
 Everything between the user's ``scorer.train(dataset)`` and the accelerator call is the reference's code.
 
-Build-container only: ``/root/reference`` does not exist on the GPU box (the tests that use this skip there).
+Without such a checkout the tests that use this compare against their recorded golden data instead.
 """
 
 from __future__ import annotations
 
 import contextlib
 import importlib.util
+import os
 import sys
 import types
 from pathlib import Path
@@ -26,11 +27,27 @@ from pathlib import Path
 import numpy as np
 from scipy.sparse import coo_array
 
-REF_SRC = Path("/root/reference/src/lenskit")
+def reference_root() -> Path | None:
+    """The lenskit/lkpy checkout to load from: ``$LENSKIT_REFERENCE_SRC`` if set, otherwise a directory named
+    ``reference`` next to this repository or next to one of its parent directories."""
+    env = os.environ.get("LENSKIT_REFERENCE_SRC")
+    here = Path(__file__).resolve().parent.parent
+    cands = [Path(env)] if env else [p / "reference" for p in here.parents]
+    for c in cands:
+        try:
+            if (c / "src" / "lenskit" / "als" / "_implicit.py").is_file():
+                return c
+        except OSError:  # an unreadable directory on the way
+            continue
+    return None
+
+
+_ROOT = reference_root()
+REF_SRC = (_ROOT or Path("reference")) / "src" / "lenskit"
 
 
 def available() -> bool:
-    return (REF_SRC / "als" / "_implicit.py").exists()
+    return _ROOT is not None
 
 
 # ---------------------------------------------------------------------------

@@ -1,6 +1,6 @@
 """
-GPU parity of als_tc128.cu — k = 128 on the tensor cores (three M=64 accumulators per system, the
-128x128 systems solved in TMEM by chol_tc128.cuh; BASELINE configs[3]) — against the f64 oracle that
+GPU parity of als_tc.cu at k = 128 (four warps, one 64x64 Gram quadrant each, the 128x128 system solved
+in shared memory; BASELINE configs[3]) — against the f64 oracle that
 rounds the gathered rows to bf16 the same way, and against the SIMT kernel on the same inputs.
 """
 

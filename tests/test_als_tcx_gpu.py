@@ -1,7 +1,7 @@
 """
-GPU parity of als_tcx.cu (k = 64) and of the tf32 gather path of als_tc128.cu (k = 128) — the tensor-core
-ALS kernels for fp32 gathered rows and non-uniform confidence weights (tf32 hi/lo split Gram, three MMAs
-per accumulator and 8 rows) — against the f64 oracle with
+GPU parity of the tf32 gather path of als_tc.cu at k = 64 and k = 128 — the tensor-core ALS kernel for fp32
+gathered rows and non-uniform confidence weights (tf32 hi/lo split Gram, three MMAs per accumulator tile and
+8 rows) — against the f64 oracle with
 UNROUNDED inputs (fp32 rows: the reference's own arithmetic, north-star tolerance 1e-4) and against
 the SIMT kernel on the same inputs.
 """
@@ -56,7 +56,7 @@ def _matrices(inter, kind, rng):
 @pytest.mark.parametrize("kind", ["implicit", "weighted", "explicit"])
 def test_tcx_parity(cuda_lib, lk_options, kind, bf16, k):
     if kind == "implicit" and bf16:
-        pytest.skip("bf16 rows with uniform weights are the kind::f16 configuration (als_tc.cu, als_tc128.cu)")
+        pytest.skip("bf16 rows with uniform weights take the bf16 MMAs (test_als_tc_gpu.py, test_als_tc128_gpu.py)")
     inter = small_synth(900, 500, 40000, seed=21)
     rng = np.random.default_rng(21)
     p = (rng.standard_normal((inter.n_users, k)) * 0.1).astype(np.float32)
@@ -73,8 +73,8 @@ def test_tcx_parity(cuda_lib, lk_options, kind, bf16, k):
         assert np.all(got[np.diff(csr.indptr) == 0] == 0.0)
         lk_options("LK_ALS_TC", 0)  # the SIMT kernel on the same inputs
         simt, _, _ = _run(mode, csr, this, other, 0.1, bf16)
-        # tcgen05 accumulators add with round-toward-zero (three accumulations per 8 rows here): the
-        # tensor-core Gram sits a few 1e-5 from true f32 arithmetic, inside the 1e-4 north-star tolerance
+        # the tf32 x3 Gram drops the lo.lo term and truncates lo: it sits a few 1e-5 from true f32
+        # arithmetic, inside the 1e-4 north-star tolerance
         assert rel_fro(got, simt) < 6e-5, rel_fro(got, simt)
 
 
@@ -110,9 +110,9 @@ def test_tcx_split_rows_deterministic(cuda_lib, lk_options, kind, k):
     ref, _ = _oracle(mode, iu, q, p, 0.1)
     assert rel_fro(a, ref) < 1e-4
     c, _, _ = _run(mode, iu, q, p, 0.1, chunk_nnz=1 << 20)
-    # split (32-nonzero parts added with round-to-nearest) vs unsplit (one round-toward-zero accumulation chain
-    # per row): the difference is the accumulator's truncation bias (1.4e-5 measured at k = 128 with uniform
-    # weights, more with sqrt(v)-scaled rows); both sit inside the 1e-4 tolerance against the oracle above
+    # split (32-nonzero parts added with round-to-nearest) vs unsplit (one tensor-core accumulation chain per
+    # row): the accumulation orders differ, and the 128x128 solve amplifies that more than the 64x64 one; both
+    # sit inside the 1e-4 tolerance against the oracle above
     assert rel_fro(a, c) < (1e-5 if k == 64 else 1e-4)
 
 

@@ -30,12 +30,12 @@ def test_header_symbols_exported(cuda_lib):
     assert cuda_lib.lk_als_max_features() == 128
 
 
-def test_library_is_sm100a():
+def test_library_is_sm90a():
     _build.build()
     out = subprocess.run(["cuobjdump", "-lelf", str(_build.LIB)], capture_output=True, text=True)
     if out.returncode != 0:
         pytest.skip("cuobjdump unavailable")
-    assert "sm_100a" in out.stdout
+    assert "sm_90a" in out.stdout
 
 
 def test_no_fallback_without_device():

@@ -57,8 +57,7 @@ def test_als_half_steps_at_ml25m_shape(cuda_lib, ml25m, gather):
 @pytest.mark.parametrize("gather", ["bf16", "fp32"])
 def test_als_item_half_step_k128_at_ml25m_shape(cuda_lib, ml25m, gather):
     """features = 128 (BASELINE configs[3]'s width) on the long item rows of the ML-25M shape: the
-    three-accumulator Gram and the 128x128 in-TMEM solve of als_tc128.cu, kind::f16 (bf16 rows) and tf32 x3
-    (fp32 rows), parts as long as the trainers plan them (ALSTrainerBase._chunk_nnz)."""
+    tensor-core Gram of als_tc.cu (bf16 MMAs for bf16 rows, tf32 x3 for fp32 rows), parts as long as the trainers plan them (ALSTrainerBase._chunk_nnz)."""
     dev = _lib.require_device()
     k = 128
     _ui, iu = data.als_implicit_matrices(ml25m, WEIGHT)

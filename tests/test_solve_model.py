@@ -1,11 +1,11 @@
 """
-NumPy model of the in-TMEM solve of chol_tc.cuh (CPU only): blocked Cholesky, block size 16, whose
-rank-16 trailing updates are computed the way the tensor cores compute them — operands split into
-tf32 `hi` (low 13 mantissa bits cleared) and `lo = x - hi` (truncated to tf32 again by the MMA),
-products hi·hi + hi·lo + lo·hi accumulated in f32 — and the block Gauss-Jordan variant.  The model
-pins the numerical claims DESIGN.md §4.1 makes for the kernel (the GPU tests check the kernel itself):
-the three-term split is as accurate as an f32 Cholesky, a two-term split is not, and Gauss-Jordan
-costs at most a small factor on badly conditioned systems.
+NumPy model of the tf32 three-term split that als_tc.cu uses for fp32-accurate Grams on the tensor cores
+(CPU only): operands split into tf32 `hi` (low 13 mantissa bits cleared) and `lo = x - hi` (truncated to
+tf32 again by the MMA), products hi·hi + hi·lo + lo·hi accumulated in f32.  The model applies the split in
+a harsher setting than the kernel's Gram: the rank-16 trailing updates of a blocked Cholesky (and a block
+Gauss-Jordan variant), where its error compounds over every update.  No kernel factors that way; the
+kernel's own accuracy is checked by the GPU tests.  What the model shows about the arithmetic: the
+three-term split is as accurate as f32, a two-term split is not.
 """
 
 import numpy as np
@@ -104,8 +104,7 @@ def test_three_term_split_matches_f32_cholesky(cond):
         e_gj.append(_err(solve_blocked(A, y, 3, gauss_jordan=True), A, y))
         e_two.append(_err(solve_blocked(A, y, 2), A, y))
     m_l, m_m, m_g, m_2 = map(np.mean, (e_lapack, e_model, e_gj, e_two))
-    # (the model truncates `lo` to tf32 as well, the harshest reading of the hardware; the kernel's measured
-    # error is that of the f32 shared-memory Cholesky to three digits, tools/chol_tc_bench.cu)
+    # (the model truncates `lo` to tf32 as well, the harshest reading of the hardware)
     assert m_m < 5.0 * m_l + 1e-6, (m_m, m_l)  # f32-level accuracy
     assert m_g < 6.0 * m_l + 1e-6, (m_g, m_l)  # Gauss-Jordan: a small factor at most
     assert m_2 > 10.0 * m_m, (m_2, m_m)  # dropping lo.hi is a 2^-12 relative error per product: visible
@@ -115,7 +114,7 @@ def test_model_agrees_with_plain_solution_on_als_like_system():
     rng = np.random.default_rng(1)
     Q = (rng.standard_normal((3000, 64)) * 0.1).astype(f32)
     M = Q[rng.choice(3000, 150, replace=False)]
-    A = ((Q.T @ Q + 0.1 * np.eye(64)) / 40.0 + M.T @ M).astype(f32)  # A / v with the preloaded OtOr / v
+    A = ((Q.T @ Q + 0.1 * np.eye(64)) / 40.0 + M.T @ M).astype(f32)  # an implicit-ALS system scaled by 1 / v
     y = (41.0 / 40.0 * M.sum(0)).astype(f32)
     for gj in (False, True):
         assert _err(solve_blocked(A, y, 3, gauss_jordan=gj), A, y) < 5e-6

@@ -1,6 +1,6 @@
 """Summarise an .ncu-rep (ncu --set full) into the handful of numbers DESIGN.md / bench.py quote.
 
-usage: python tools/ncu_summary.py gpurun_out/x.ncu-rep [more.ncu-rep ...] > profiles/rNN_x.md
+usage: python tools/ncu_summary.py x.ncu-rep [more.ncu-rep ...] > summary.md
 """
 import csv
 import io
