@@ -68,7 +68,7 @@ LK_API int lk_device_info(int *sm_count, int *cc);
 /* Diagnostic switches (kernel variants kept for comparison; none changes results beyond rounding).
  * Each is also an environment variable of the same name, read once when the library first needs
  * it — never per launch; after that only lk_set_option changes it.  Names: LK_ALS_TC,
- * LK_ALS_TF32, LK_KNN_WARPS, LK_KNN_CTAS, LK_KNN_SCORE_SEQ, LK_KNN_SCORE_CTAS (meaning: lkpy_b200/csrc/common.cuh, struct Options). */
+ * LK_ALS_TF32, LK_KNN_WARPS, LK_KNN_CTAS, LK_KNN_SCORE_CTAS (meaning: lkpy_b200/csrc/common.cuh, struct Options). */
 LK_API int lk_set_option(const char *name, int value);
 LK_API int lk_get_option(const char *name, int *value);
 
@@ -126,7 +126,6 @@ typedef struct lk_als_args {
     int32_t vals_uniform;    /* 1 when every d_vals entry equals uniform_val (implicit feedback without
                                 ratings): lets the Gram run on the tensor cores as v * M^T M */
     float uniform_val;
-    unsigned long long *d_prof; /* reserved (ignored by the kernels), NULL */
     /* Cooperative cancel (the role of CancelAdapter, src/accel/als/implicit.rs:72-73, tasks/mod.rs:62-106):
      * optional device flag, read (uncached) every time a CTA fetches work; once non-zero no further rows
      * are started — rows already solved keep their new values, the rest their old ones.  Progress =
@@ -255,23 +254,15 @@ typedef struct lk_knn_score_args {
     int32_t *d_slotmap;          /* [slotmap_warps * n_items], all -1 on entry and on exit */
     int64_t slotmap_warps;       /* warps that work on the batch, one slot-map row each: 1..lk_knn_score_warps()
                                     (more is not used); min(n_queries, lk_knn_score_warps()) is enough */
-    float *d_acc_ws, *d_acc_tw;  /* [n_targets] accumulator scratch */
-    int32_t *d_acc_cnt;          /* [n_targets] */
+    int32_t *d_list_off, *d_list_cur; /* [n_targets] each: a target's contribution-list offset and fill cursor */
+    int32_t *d_list_cnt;         /* [n_targets]: contributions per target */
     float *d_scores;             /* [n_targets] NaN = null (Arrow null in the reference) */
     int32_t *d_counts;           /* [n_targets] -1 = null */
     int32_t *d_work_counter;     /* [1] zeroed by the call */
     int32_t *d_status;           /* [1] 0 ok; 2 NaN similarity */
-    /* Per-warp heap states for the targets that receive more than max_nbrs contributions
-     * (accum.rs:100-117): [slotmap_warps * heap_floats_per_warp] 32-bit words, 8-byte aligned;
-     * one target takes 2 + 2*(max_nbrs+1) words.  Optional (NULL / 0): targets that do not fit are
-     * replayed one at a time from the query's history instead (same result, much slower for long
-     * histories). */
-    float *d_heap_scratch;
-    int64_t heap_floats_per_warp;
-    /* Contribution pool (optional; with it the list-based kernel runs: per-target contribution
-     * lists built in parallel, sorted by history position, replayed — same bits, no sequential
-     * walk over the history).  pool_entries 16-byte entries, at least the number of
-     * (reference item, similarity-row entry) pairs of the whole batch:
+    /* Contribution pool (required): per-target contribution lists are built in parallel, sorted by
+     * history position and replayed through the accumulator.  pool_entries 16-byte entries, at least
+     * the number of (reference item, similarity-row entry) pairs of the whole batch:
      * sum over valid d_ref_items r of (d_sim_indptr[r+1] - d_sim_indptr[r]); d_pool_cursor [1]
      * is zeroed by the call.  Status 3 = pool too small. */
     void *d_pool;
@@ -286,15 +277,11 @@ typedef struct lk_knn_score_args {
     int32_t user_mode;
     int32_t n_matrix_rows;       /* user mode: rows of the rating matrix (item mode: unused, = n_items) */
     /* Dense mode — d_tgt_indptr == NULL and d_tgt_items == NULL: every query is scored against ALL
-     * items in index order; d_scores / d_counts are [n_queries * n_items] and written exactly once, d_acc_cnt
-     * is not used, the contribution pool is required.  A CTA handles a query and keeps its state per CTA:
-     * d_slotmap provides one n_items row per CTA (slotmap_warps >= lk_knn_score_dense_ctas()) that must be
-     * all ZERO on entry and is left all zero (item -> touched-target number), d_acc_ws / d_acc_tw one
-     * n_items row per CTA each ([min(n_queries, lk_knn_score_dense_ctas()) * n_items] 32-bit words:
-     * list offsets / cursors by touched-target number). */
-    int32_t *d_deferred;         /* dense mode, optional: [n_queries] order in which the queries are handed to the CTAs
-                                  * (a permutation; longest histories first keeps the tail of the launch short) */
-    int32_t *d_n_deferred;       /* reserved (unused) */
+     * items in index order; d_scores / d_counts are [n_queries * n_items] and written exactly once, d_list_cnt
+     * is not used.  A CTA handles a query and keeps its state per CTA: d_slotmap provides one n_items row per
+     * CTA (slotmap_warps >= lk_knn_score_dense_ctas()) that must be all ZERO on entry and is left all zero
+     * (item -> touched-target number), d_list_off / d_list_cur one n_items row per CTA each
+     * ([min(n_queries, lk_knn_score_dense_ctas()) * n_items]: list offsets / cursors by touched-target number). */
 } lk_knn_score_args;
 
 /* largest number of warps the scoring grid runs (one slotmap row each) */

@@ -57,7 +57,6 @@ class LkAlsArgs(C.Structure):
         ("d_status", vp),
         ("vals_uniform", C.c_int32),
         ("uniform_val", C.c_float),
-        ("d_prof", vp),
         ("d_cancel", vp),
     ]
 
@@ -123,22 +122,18 @@ class LkKnnScoreArgs(C.Structure):
         ("min_nbrs", C.c_int32),
         ("d_slotmap", vp),
         ("slotmap_warps", C.c_int64),
-        ("d_acc_ws", vp),
-        ("d_acc_tw", vp),
-        ("d_acc_cnt", vp),
+        ("d_list_off", vp),
+        ("d_list_cur", vp),
+        ("d_list_cnt", vp),
         ("d_scores", vp),
         ("d_counts", vp),
         ("d_work_counter", vp),
         ("d_status", vp),
-        ("d_heap_scratch", vp),
-        ("heap_floats_per_warp", C.c_int64),
         ("d_pool", vp),
         ("pool_entries", C.c_int64),
         ("d_pool_cursor", vp),
         ("user_mode", C.c_int32),
         ("n_matrix_rows", C.c_int32),
-        ("d_deferred", vp),
-        ("d_n_deferred", vp),
     ]
 
 

@@ -31,7 +31,6 @@ static const OptionDef OPTION_DEFS[] = {
     {"LK_ALS_TF32", &Options::als_tf32},
     {"LK_KNN_WARPS", &Options::knn_warps},
     {"LK_KNN_CTAS", &Options::knn_ctas},
-    {"LK_KNN_SCORE_SEQ", &Options::knn_score_seq},
     {"LK_KNN_SCORE_CTAS", &Options::knn_score_ctas},
 };
 
@@ -65,7 +64,7 @@ int sm_count()
 
 extern "C" {
 
-int lk_version(void) { return 100; }
+int lk_version(void) { return 101; }
 
 const char *lk_last_error(void) { return lk::g_err; }
 

@@ -41,7 +41,6 @@ struct Options {
     int als_tf32 = 1;           // 0: fp32 / non-uniformly weighted rows stay on the SIMT kernel
     int knn_warps = -1;         // warps per CTA of the kNN build (8, 16, 32)
     int knn_ctas = -1;          // resident CTAs per SM of the kNN build
-    int knn_score_seq = 0;      // 1: sequential scoring kernel even with a contribution pool
     int knn_score_ctas = -1;    // resident CTAs per SM of the dense (all-items) scoring kernel (1..3)
 };
 Options &options();

@@ -8,18 +8,23 @@
 //   * reference items are visited in history order, each one's similarity row
 //     in column order; a target's accumulator takes the first `max_nbrs`
 //     contributions as a vector (accum.rs:86-98) whose sums are taken in push
-//     order — reproduced here by running sums updated in the same order;
+//     order;
 //   * a target that receives more than `max_nbrs` contributions switches to a
-//     min-heap (accum.rs:73-82,100-117).  Those targets are re-scored by a
-//     per-lane emulation of the Rust std BinaryHeap element movement so that
-//     the survivor set under ties and the summation order match;
+//     min-heap (accum.rs:73-82,100-117), emulated with the Rust std BinaryHeap
+//     element movement so that the survivor set under ties and the summation
+//     order match;
 //   * null (negative) reference items are skipped, null targets give NaN / -1.
 //
-// One warp owns one query: lanes spread over the entries of a similarity row,
-// history entries are processed one after the other (order is the contract).
-// A per-warp `slotmap` (n_items ints, kept at -1 between queries) maps item ->
-// position in the query's target list, so cost is proportional to the
-// contributions and the target list, never to n_items.
+// Neither kernel walks the history one entry after the other.  The contributions
+// of a query are counted and scattered in parallel into one list per target in a
+// contribution pool; each list is then sorted by history position and replayed
+// through the accumulator by one thread (replay_list), which restores the order
+// the reference sees.
+//   * knn_score_lists_kernel (explicit target lists): one warp owns one query.  A
+//     per-warp `slotmap` (n_items ints, kept at -1 between queries) maps item ->
+//     position in the query's target list, so cost is proportional to the
+//     contributions and the target list, never to n_items.
+//   * knn_score_dense_kernel (every query against all items): one CTA per query.
 
 #include <algorithm>
 
@@ -102,45 +107,56 @@ __device__ void acc_push(AccEnt *d, int &len, int &is_heap, const AccEnt e, cons
     }
 }
 
-// per-target heap state kept in the per-warp scratch of lk_knn_score_args::d_heap_scratch:
-// [len, is_heap, (w, v) x (limit + 1)] as 32-bit words
-__device__ __forceinline__ int heap_state_words(int limit) { return 2 + 2 * (limit + 1); }
+// ---------------------------------------------------------------------------------------------
+// Target-list kernel: the contributions are counted per target with the 32 lanes working on 32 history
+// entries at once, a prefix sum lays the targets' lists out in the pool, a second parallel pass fills the
+// lists (chunks of 32 history entries are committed in order, so a list is sorted up to displacements
+// inside one chunk), and every target then replays its list (replay_list).  A query's cost does not grow
+// with the length of its history times a global-memory round trip.
+// ---------------------------------------------------------------------------------------------
+struct __align__(16) PoolEnt {
+    int32_t pos;  // index of the reference item in the query's history
+    float sim, rv;
+    int32_t pad;
+};
 
-// exact ScoreAccumulator replay for one (query, target) pair (fallback when the per-warp heap
-// scratch is absent or full)
-__device__ void rescore_exact(const lk_knn_score_args &a, int64_t r0, int64_t r1, int t, float *out_ws,
-                              float *out_tw, int *out_len)
+// One target's contribution list [n entries] through a ScoreAccumulator: sorted by history position in
+// place (insertion sort: the lists arrive nearly sorted), then summed in push order while it fits the vector
+// state (accum.rs:86-98, 196-231), or replayed through the BinaryHeap movement past `limit` and summed in
+// heap-array order.  Returns the accumulator's length; ws is only summed with explicit feedback.
+__device__ __forceinline__ int replay_list(PoolEnt *L, const int n, const int limit, const bool explicit_fb,
+                                           float &ws, float &tw)
 {
-    AccEnt d[SCORE_MAX_NBRS + 1];
-    int len = 0;
-    int is_heap = 0;
-    const int limit = a.max_nbrs;
-    const int n_rows = a.user_mode ? a.n_matrix_rows : a.n_items;
-    for (int64_t p = r0; p < r1; p++) {
-        const int r = a.d_ref_items[p];
-        if (r < 0 || r >= n_rows) continue;
-        int64_t lo = a.d_sim_indptr[r], hi = a.d_sim_indptr[r + 1];
-        const int64_t end = hi;
-        while (lo < hi) {
-            const int64_t mid = (lo + hi) >> 1;
-            if (a.d_sim_cols[mid] < t) lo = mid + 1; else hi = mid;
+    for (int i = 1; i < n; i++) {
+        const PoolEnt key = L[i];
+        int j = i - 1;
+        while (j >= 0 && L[j].pos > key.pos) {
+            L[j + 1] = L[j];
+            j--;
         }
-        if (lo >= end || a.d_sim_cols[lo] != t) continue;
-        const float mv = a.d_sim_vals ? a.d_sim_vals[lo] : 0.0f, hv = a.d_ref_vals ? a.d_ref_vals[p] : 0.0f;
-        AccEnt e;
-        e.w = a.user_mode ? hv : mv;
-        e.v = a.user_mode ? mv : hv;
-        acc_push(d, len, is_heap, e, limit);
+        L[j + 1] = key;
     }
-    float tw = 0.0f, ws = 0.0f;
+    ws = 0.0f, tw = 0.0f;
+    if (n <= limit) {
+        for (int i = 0; i < n; i++) tw = __fadd_rn(tw, L[i].sim);
+        if (explicit_fb)
+            for (int i = 0; i < n; i++) ws = __fadd_rn(ws, __fmul_rn(L[i].sim, L[i].rv));
+        return n;
+    }
+    AccEnt d[SCORE_MAX_NBRS + 1];
+    int len = 0, is_heap = 0;
+    for (int i = 0; i < n; i++) {
+        AccEnt ent;
+        ent.w = L[i].sim;
+        ent.v = L[i].rv;
+        acc_push(d, len, is_heap, ent, limit);
+    }
     for (int i = 0; i < len; i++) tw = __fadd_rn(tw, d[i].w);
     for (int i = 0; i < len; i++) ws = __fadd_rn(ws, __fmul_rn(d[i].w, d[i].v));
-    *out_ws = ws;
-    *out_tw = tw;
-    *out_len = len;
+    return len;
 }
 
-__global__ void __launch_bounds__(256) knn_score_kernel(lk_knn_score_args a)
+__global__ void __launch_bounds__(256) knn_score_lists_kernel(lk_knn_score_args a)
 {
     const int lane = threadIdx.x & 31;
     const int gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -153,164 +169,7 @@ __global__ void __launch_bounds__(256) knn_score_kernel(lk_knn_score_args a)
     const int n_rows = user_mode ? a.n_matrix_rows : a.n_items;
     const bool explicit_fb = user_mode ? a.d_sim_vals != nullptr : a.d_ref_vals != nullptr;
     const float qnan = __int_as_float(0x7fc00000);
-    const int hwords = heap_state_words(a.max_nbrs);
-    uint32_t *heap_base = a.d_heap_scratch != nullptr
-                              ? reinterpret_cast<uint32_t *>(a.d_heap_scratch) + (size_t)gwarp * a.heap_floats_per_warp
-                              : nullptr;
-    const int heap_cap = a.d_heap_scratch != nullptr ? (int)(a.heap_floats_per_warp / hwords) : 0;
-
-    for (;;) {
-        int q = 0;
-        if (lane == 0) q = atomicAdd(a.d_work_counter, 1);
-        q = __shfl_sync(FULL, q, 0);
-        if (q >= a.n_queries) break;
-        const int64_t t0 = a.d_tgt_indptr[q], t1 = a.d_tgt_indptr[q + 1];
-        const int64_t r0 = a.d_ref_indptr[q], r1 = a.d_ref_indptr[q + 1];
-
-        // 1. register the targets, zero their accumulator state
-        for (int64_t x = t0 + lane; x < t1; x += 32) {
-            const int t = a.d_tgt_items[x];
-            a.d_acc_ws[x] = 0.0f;
-            a.d_acc_tw[x] = 0.0f;
-            a.d_acc_cnt[x] = 0;
-            if (t >= 0 && t < a.n_items) slotmap[t] = (int32_t)(x - t0);
-        }
-        __syncwarp();
-
-        // 2. contributions in history order; one similarity row's entries hit distinct targets
-        for (int64_t p = r0; p < r1; p++) {
-            const int r = a.d_ref_items[p];
-            if (r < 0 || r >= n_rows) continue;  // null reference item (SURVEY.md App. A)
-            const float hv = a.d_ref_vals ? a.d_ref_vals[p] : 0.0f;
-            const int64_t s0 = a.d_sim_indptr[r], s1 = a.d_sim_indptr[r + 1];
-            for (int64_t e = s0 + lane; e < s1; e += 32) {
-                const int t = a.d_sim_cols[e];
-                const int32_t slot = slotmap[t];
-                if (slot >= 0) {
-                    const float mv = a.d_sim_vals ? a.d_sim_vals[e] : 0.0f;
-                    const float sim = user_mode ? hv : mv, rv = user_mode ? mv : hv;
-                    if (sim != sim) atomicCAS(a.d_status, 0, 2);  // "similarity is null" (accum.rs:146-152)
-                    const int64_t x = t0 + slot;
-                    const int c = a.d_acc_cnt[x];
-                    if (c < a.max_nbrs) {  // vector state: sums in push order
-                        a.d_acc_tw[x] = __fadd_rn(a.d_acc_tw[x], sim);
-                        if (explicit_fb) a.d_acc_ws[x] = __fadd_rn(a.d_acc_ws[x], __fmul_rn(sim, rv));
-                    }
-                    a.d_acc_cnt[x] = c + 1;
-                }
-            }
-            __syncwarp();
-        }
-
-        // 2b. targets that received more than max_nbrs contributions have left the vector state:
-        //     give each a heap in this warp's scratch (marker -(index+2) in its count) and run the
-        //     history once more, every lane pushing its entry into its target's heap — the same
-        //     element movement as the reference's accumulator, in the same order.  Targets that do
-        //     not fit the scratch keep their count and are replayed one by one in step 3.
-        if (heap_base != nullptr) {
-            int n_tracked = 0;  // warp-uniform running count
-            for (int64_t x0 = t0; x0 < t1; x0 += 32) {
-                const int64_t x = x0 + lane;
-                const bool over = x < t1 && a.d_acc_cnt[x] > a.max_nbrs;
-                const unsigned m = __ballot_sync(FULL, over);
-                if (m == 0u) continue;
-                const int idx = n_tracked + __popc(m & ((1u << lane) - 1u));
-                if (over && idx < heap_cap) {
-                    a.d_acc_cnt[x] = -(idx + 2);
-                    uint32_t *hs = heap_base + (size_t)idx * hwords;
-                    hs[0] = 0u, hs[1] = 0u;
-                }
-                n_tracked += __popc(m);
-            }
-            __syncwarp();
-            if (n_tracked > 0) {
-                for (int64_t p = r0; p < r1; p++) {
-                    const int r = a.d_ref_items[p];
-                    if (r < 0 || r >= n_rows) continue;
-                    const float hv = a.d_ref_vals ? a.d_ref_vals[p] : 0.0f;
-                    const int64_t s0 = a.d_sim_indptr[r], s1 = a.d_sim_indptr[r + 1];
-                    for (int64_t e = s0 + lane; e < s1; e += 32) {
-                        const int32_t slot = slotmap[a.d_sim_cols[e]];
-                        if (slot < 0) continue;
-                        const int mk = a.d_acc_cnt[t0 + slot];
-                        if (mk > -2) continue;
-                        uint32_t *hs = heap_base + (size_t)(-mk - 2) * hwords;
-                        int len = (int)hs[0], is_heap = (int)hs[1];
-                        const float mv = a.d_sim_vals ? a.d_sim_vals[e] : 0.0f;
-                        AccEnt ent;
-                        ent.w = user_mode ? hv : mv;
-                        ent.v = user_mode ? mv : hv;
-                        acc_push(reinterpret_cast<AccEnt *>(hs + 2), len, is_heap, ent, a.max_nbrs);
-                        hs[0] = (uint32_t)len, hs[1] = (uint32_t)is_heap;
-                    }
-                    __syncwarp();
-                }
-            }
-        }
-
-        // 3. finalise every target position (duplicate targets read the registered slot)
-        for (int64_t x = t0 + lane; x < t1; x += 32) {
-            const int t = a.d_tgt_items[x];
-            float score = qnan;
-            int count = -1;
-            if (t >= 0 && t < a.n_items) {
-                const int64_t xs = t0 + slotmap[t];
-                int c = a.d_acc_cnt[xs];
-                float ws = a.d_acc_ws[xs], tw = a.d_acc_tw[xs];
-                if (c <= -2) {  // heap state built in step 2b: sums in heap-array order
-                    const uint32_t *hs = heap_base + (size_t)(-c - 2) * hwords;
-                    const AccEnt *d = reinterpret_cast<const AccEnt *>(hs + 2);
-                    c = (int)hs[0];
-                    tw = 0.0f, ws = 0.0f;
-                    for (int i = 0; i < c; i++) tw = __fadd_rn(tw, d[i].w);
-                    for (int i = 0; i < c; i++) ws = __fadd_rn(ws, __fmul_rn(d[i].w, d[i].v));
-                } else if (c > a.max_nbrs) {
-                    rescore_exact(a, r0, r1, t, &ws, &tw, &c);  // heap state, replayed from scratch
-                }
-                count = c;
-                if (c >= a.min_nbrs) score = explicit_fb ? ws / tw : tw;
-            }
-            a.d_scores[x] = score;
-            a.d_counts[x] = count;
-        }
-        __syncwarp();
-        for (int64_t x = t0 + lane; x < t1; x += 32) {
-            const int t = a.d_tgt_items[x];
-            if (t >= 0 && t < a.n_items) slotmap[t] = -1;
-        }
-        __syncwarp();
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// List-based variant (used when lk_knn_score_args::d_pool is given): no sequential walk over the
-// history.  Contributions are counted per target with the 32 lanes working on 32 history entries at
-// once, a prefix sum lays the targets' lists out in a pool, a second parallel pass fills the lists
-// (chunks of 32 history entries are committed in order, so a list is sorted up to displacements
-// inside one chunk), and every target then sorts its list by history position and replays it
-// through the accumulator — vector sums in push order, BinaryHeap movement past max_nbrs — exactly
-// as the sequential kernel does.  A query's cost no longer grows with the length of its history
-// times a global-memory round trip.
-// ---------------------------------------------------------------------------------------------
-struct __align__(16) PoolEnt {
-    int32_t pos;  // index of the reference item in the query's history
-    float sim, rv;
-    int32_t pad;
-};
-
-__global__ void __launch_bounds__(256) knn_score_lists_kernel(lk_knn_score_args a)
-{
-    const int lane = threadIdx.x & 31;
-    const int gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (gwarp >= a.slotmap_warps) return;  // one slot-map row per working warp
-    int32_t *slotmap = a.d_slotmap + (size_t)gwarp * a.n_items;
-    const bool user_mode = a.user_mode != 0;  // see knn_score_kernel
-    const int n_rows = user_mode ? a.n_matrix_rows : a.n_items;
-    const bool explicit_fb = user_mode ? a.d_sim_vals != nullptr : a.d_ref_vals != nullptr;
-    const float qnan = __int_as_float(0x7fc00000);
-    int32_t *acc_cnt = a.d_acc_cnt;
-    int32_t *acc_off = reinterpret_cast<int32_t *>(a.d_acc_ws);  // list offset of a target (scratch reuse)
-    int32_t *acc_cur = reinterpret_cast<int32_t *>(a.d_acc_tw);  // fill cursor of a target
+    int32_t *list_cnt = a.d_list_cnt, *list_off = a.d_list_off, *list_cur = a.d_list_cur;
     PoolEnt *pool = reinterpret_cast<PoolEnt *>(a.d_pool);
     const int limit = a.max_nbrs;
 
@@ -335,7 +194,7 @@ __global__ void __launch_bounds__(256) knn_score_lists_kernel(lk_knn_score_args 
             for (int u = 0; u < UB; u++) {
                 const int64_t x = xb + 32 * u;
                 if (x < t1) {
-                    acc_cnt[x] = 0;
+                    list_cnt[x] = 0;
                     if (tt[u] >= 0 && tt[u] < a.n_items) slotmap[tt[u]] = (int32_t)(x - t0);
                 }
             }
@@ -364,7 +223,7 @@ __global__ void __launch_bounds__(256) knn_score_lists_kernel(lk_knn_score_args 
                         for (int u = 0; u < UB; u++) {
                             if (sl[u] >= 0) {
                                 if (sv[u] != sv[u]) atomicCAS(a.d_status, 0, 2);  // "similarity is null"
-                                atomicAdd(&acc_cnt[t0 + sl[u]], 1);
+                                atomicAdd(&list_cnt[t0 + sl[u]], 1);
                             }
                         }
                     }
@@ -380,15 +239,15 @@ __global__ void __launch_bounds__(256) knn_score_lists_kernel(lk_knn_score_args 
 #pragma unroll
             for (int u = 0; u < UB; u++) {
                 const int64_t x = x0 + 32 * u + lane;
-                cc[u] = x < t1 ? __ldcg(&acc_cnt[x]) : 0;
+                cc[u] = x < t1 ? __ldcg(&list_cnt[x]) : 0;
             }
 #pragma unroll
             for (int u = 0; u < UB; u++) {
                 const int64_t x = x0 + 32 * u + lane;
                 const int incl = warp_incl_scan(cc[u], lane);
                 if (x < t1) {
-                    acc_off[x] = running + incl - cc[u];
-                    acc_cur[x] = 0;
+                    list_off[x] = running + incl - cc[u];
+                    list_cur[x] = 0;
                 }
                 running += __shfl_sync(FULL, incl, 31);
             }
@@ -421,8 +280,8 @@ __global__ void __launch_bounds__(256) knn_score_lists_kernel(lk_knn_score_args 
                             for (int u = 0; u < UB; u++) sl[u] = cc[u] >= 0 ? slotmap[cc[u]] : -1;
 #pragma unroll
                             for (int u = 0; u < UB; u++) {
-                                of[u] = sl[u] >= 0 ? acc_off[t0 + sl[u]] : 0;
-                                kp[u] = sl[u] >= 0 ? atomicAdd(&acc_cur[t0 + sl[u]], 1) : 0;
+                                of[u] = sl[u] >= 0 ? list_off[t0 + sl[u]] : 0;
+                                kp[u] = sl[u] >= 0 ? atomicAdd(&list_cur[t0 + sl[u]], 1) : 0;
                             }
 #pragma unroll
                             for (int u = 0; u < UB; u++) {
@@ -456,7 +315,7 @@ __global__ void __launch_bounds__(256) knn_score_lists_kernel(lk_knn_score_args 
 #pragma unroll
             for (int u = 0; u < UB; u++) {
                 const int64_t x = xb + 32 * u;
-                nn[u] = (fits && sm[u] >= 0 && t0 + sm[u] == x) ? __ldcg(&acc_cnt[x]) : 0;
+                nn[u] = (fits && sm[u] >= 0 && t0 + sm[u] == x) ? __ldcg(&list_cnt[x]) : 0;
             }
 #pragma unroll
             for (int u = 0; u < UB; u++) {
@@ -471,38 +330,10 @@ __global__ void __launch_bounds__(256) knn_score_lists_kernel(lk_knn_score_args 
                     any_dup = true;
                     continue;
                 }
-                const int n = nn[u];
                 float ws = 0.0f, tw = 0.0f;
-                int c = n;
-                if (n > 0) {
-                    PoolEnt *L = pool + base + (unsigned long long)acc_off[x];
-                    for (int i = 1; i < n; i++) {  // insertion sort: displacements stay inside a 32-entry chunk
-                        const PoolEnt key = L[i];
-                        int j = i - 1;
-                        while (j >= 0 && L[j].pos > key.pos) {
-                            L[j + 1] = L[j];
-                            j--;
-                        }
-                        L[j + 1] = key;
-                    }
-                    if (n <= limit) {  // vector state: sums in push order (accum.rs:86-98, 196-231)
-                        for (int i = 0; i < n; i++) tw = __fadd_rn(tw, L[i].sim);
-                        if (explicit_fb)
-                            for (int i = 0; i < n; i++) ws = __fadd_rn(ws, __fmul_rn(L[i].sim, L[i].rv));
-                    } else {
-                        AccEnt d[SCORE_MAX_NBRS + 1];
-                        int len = 0, is_heap = 0;
-                        for (int i = 0; i < n; i++) {
-                            AccEnt ent;
-                            ent.w = L[i].sim;
-                            ent.v = L[i].rv;
-                            acc_push(d, len, is_heap, ent, limit);
-                        }
-                        for (int i = 0; i < len; i++) tw = __fadd_rn(tw, d[i].w);
-                        for (int i = 0; i < len; i++) ws = __fadd_rn(ws, __fmul_rn(d[i].w, d[i].v));
-                        c = len;
-                    }
-                }
+                int c = 0;
+                if (nn[u] > 0)
+                    c = replay_list(pool + base + (unsigned long long)list_off[x], nn[u], limit, explicit_fb, ws, tw);
                 a.d_counts[x] = c;
                 a.d_scores[x] = (c >= a.min_nbrs) ? (explicit_fb ? ws / tw : tw) : qnan;
             }
@@ -548,8 +379,7 @@ __global__ void __launch_bounds__(256) knn_score_lists_kernel(lk_knn_score_args 
 //      pool; the slot map entry becomes the touched-target number;
 //   3. fill: the same flattened walk appends (history position, weight, value) to the lists;
 //   4. replay: one thread per touched target sorts its list by history position and runs it through the
-//      accumulator (vector sums in push order / BinaryHeap movement past max_nbrs) — the same bits as the
-//      sequential walk;
+//      accumulator (replay_list, as in the list kernel);
 //   5. one coalesced pass writes the score and count rows — the result where the slot map has an entry,
 //      NaN / 0 elsewhere — and clears the slot map for the next query.
 // (Round-2 v2 counted on the output row itself and kept [n_queries x n_items] offset / cursor rows: 2.1 MB
@@ -598,8 +428,8 @@ __global__ void __launch_bounds__(DENSE_THREADS) knn_score_dense_kernel(lk_knn_s
     PoolEnt *pool = reinterpret_cast<PoolEnt *>(a.d_pool);
     // per-CTA state, reused by every query this CTA handles
     int32_t *slot = a.d_slotmap + (size_t)blockIdx.x * NI;  // all zero between queries
-    int32_t *offs = reinterpret_cast<int32_t *>(a.d_acc_ws) + (size_t)blockIdx.x * NI;  // [touched target] list offset, later score bits
-    int32_t *curs = reinterpret_cast<int32_t *>(a.d_acc_tw) + (size_t)blockIdx.x * NI;  // [touched target] list cursor, later count
+    int32_t *offs = a.d_list_off + (size_t)blockIdx.x * NI;  // [touched target] list offset, later score bits
+    int32_t *curs = a.d_list_cur + (size_t)blockIdx.x * NI;  // [touched target] list cursor, later count
     constexpr int CU = 4;  // contributions per thread and step of the flattened walk
 
     for (;;) {
@@ -609,7 +439,7 @@ __global__ void __launch_bounds__(DENSE_THREADS) knn_score_dense_kernel(lk_knn_s
         }
         __syncthreads();
         if (s_q >= a.n_queries) break;
-        const int q = a.d_deferred ? a.d_deferred[s_q] : s_q;  // optional hand-out order (heaviest queries first)
+        const int q = s_q;
         const int64_t r0 = a.d_ref_indptr[q], r1 = a.d_ref_indptr[q + 1];
         float *scores = a.d_scores + (int64_t)q * NI;
         int32_t *counts = a.d_counts + (int64_t)q * NI;
@@ -767,36 +597,8 @@ __global__ void __launch_bounds__(DENSE_THREADS) knn_score_dense_kernel(lk_knn_s
           for (int v = 0; v < RU; v++) {
             const int i = i0 + v * DENSE_THREADS;
             if (i >= n_active) break;
-            const int n = nn[v];
-            PoolEnt *L = pool + base + (unsigned long long)oo[v];
-            for (int u = 1; u < n; u++) {  // insertion sort by history position
-                const PoolEnt key = L[u];
-                int j = u - 1;
-                while (j >= 0 && L[j].pos > key.pos) {
-                    L[j + 1] = L[j];
-                    j--;
-                }
-                L[j + 1] = key;
-            }
-            float ws = 0.0f, tw = 0.0f;
-            int c = n;
-            if (n <= limit) {  // vector state: sums in push order (accum.rs:86-98, 196-231)
-                for (int u = 0; u < n; u++) tw = __fadd_rn(tw, L[u].sim);
-                if (explicit_fb)
-                    for (int u = 0; u < n; u++) ws = __fadd_rn(ws, __fmul_rn(L[u].sim, L[u].rv));
-            } else {
-                AccEnt d[SCORE_MAX_NBRS + 1];
-                int len = 0, is_heap = 0;
-                for (int u = 0; u < n; u++) {
-                    AccEnt ent;
-                    ent.w = L[u].sim;
-                    ent.v = L[u].rv;
-                    acc_push(d, len, is_heap, ent, limit);
-                }
-                for (int u = 0; u < len; u++) tw = __fadd_rn(tw, d[u].w);
-                for (int u = 0; u < len; u++) ws = __fadd_rn(ws, __fmul_rn(d[u].w, d[u].v));
-                c = len;
-            }
+            float ws, tw;
+            const int c = replay_list(pool + base + (unsigned long long)oo[v], nn[v], limit, explicit_fb, ws, tw);
             __stcg(&curs[i], c);
             __stcg(&offs[i], __float_as_int(c >= a.min_nbrs ? (explicit_fb ? ws / tw : tw) : qnan));
           }
@@ -852,25 +654,26 @@ int lk_knn_score_batch(const lk_knn_score_args *args, void *stream)
     LK_REQUIRE(a.max_nbrs >= 1 && a.max_nbrs <= SCORE_MAX_NBRS, LK_ERR_UNSUPPORTED,
                "max_nbrs must be in 1..%d", SCORE_MAX_NBRS);
     const bool dense = a.d_tgt_items == nullptr && a.d_tgt_indptr == nullptr;  // every query against all items
-    LK_REQUIRE(a.d_sim_indptr && a.d_sim_cols && a.d_ref_indptr && a.d_ref_items && a.d_acc_ws && a.d_acc_tw &&
+    LK_REQUIRE(a.d_sim_indptr && a.d_sim_cols && a.d_ref_indptr && a.d_ref_items && a.d_list_off && a.d_list_cur &&
                    a.d_scores && a.d_counts && a.d_work_counter && a.d_status,
                LK_ERR_INVALID, "lk_knn_score_batch: null pointer");
-    LK_REQUIRE(dense || (a.d_tgt_indptr && a.d_tgt_items && a.d_slotmap && a.d_acc_cnt), LK_ERR_INVALID,
+    LK_REQUIRE(a.d_pool && a.d_pool_cursor, LK_ERR_INVALID,
+               "lk_knn_score_batch: the contribution pool (d_pool, d_pool_cursor) is required");
+    LK_REQUIRE(reinterpret_cast<uintptr_t>(a.d_pool) % 16 == 0 && a.pool_entries >= 0, LK_ERR_INVALID,
+               "lk_knn_score_batch: bad contribution pool");
+    LK_REQUIRE(dense || (a.d_tgt_indptr && a.d_tgt_items && a.d_slotmap && a.d_list_cnt), LK_ERR_INVALID,
                "lk_knn_score_batch: null pointer (target lists)");
-    LK_REQUIRE(!dense || (a.d_pool && a.d_pool_cursor && a.d_slotmap && a.slotmap_warps >= lk_knn_score_dense_ctas()),
-               LK_ERR_INVALID,
-               "lk_knn_score_batch: the dense (all-items) mode needs the contribution pool and one n_items row of "
-               "d_slotmap per CTA (lk_knn_score_dense_ctas)");
+    LK_REQUIRE(!dense || (a.d_slotmap && a.slotmap_warps >= lk_knn_score_dense_ctas()), LK_ERR_INVALID,
+               "lk_knn_score_batch: the dense (all-items) mode needs one n_items row of d_slotmap per CTA "
+               "(lk_knn_score_dense_ctas)");
     LK_REQUIRE(a.user_mode ? a.d_ref_vals != nullptr : a.d_sim_vals != nullptr, LK_ERR_INVALID,
                "lk_knn_score_batch: the weights (similarities) are missing");
     LK_REQUIRE(dense || a.slotmap_warps >= 1, LK_ERR_INVALID, "slotmap too small");
     if (a.n_queries == 0) return LK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     LK_CUDA_TRY(cudaMemsetAsync(a.d_work_counter, 0, sizeof(int32_t), st));
+    LK_CUDA_TRY(cudaMemsetAsync(a.d_pool_cursor, 0, sizeof(unsigned long long), st));
     if (dense) {
-        LK_REQUIRE(reinterpret_cast<uintptr_t>(a.d_pool) % 16 == 0 && a.pool_entries >= 0, LK_ERR_INVALID,
-                   "lk_knn_score_batch: bad contribution pool");
-        LK_CUDA_TRY(cudaMemsetAsync(a.d_pool_cursor, 0, sizeof(unsigned long long), st));
         // the per-CTA slot maps (n_items ints each) should stay in L2 next to the similarity matrix: two CTAs
         // per SM instead of three when three rows per SM would take more than half of it
         const Options &opt = options();
@@ -886,15 +689,7 @@ int lk_knn_score_batch(const lk_knn_score_args *args, void *stream)
     // as many warps as there are slot-map rows (the caller sizes them to the batch), at most the full grid
     const int64_t warps = std::min<int64_t>(a.slotmap_warps, lk_knn_score_warps());
     const int blocks = (int)((warps + 7) / 8);
-    // with a contribution pool the list-based kernel runs (LK_KNN_SCORE_SEQ=1 forces the sequential one)
-    if (a.d_pool != nullptr && a.d_pool_cursor != nullptr && options().knn_score_seq != 1) {
-        LK_REQUIRE(reinterpret_cast<uintptr_t>(a.d_pool) % 16 == 0 && a.pool_entries >= 0, LK_ERR_INVALID,
-                   "lk_knn_score_batch: bad contribution pool");
-        LK_CUDA_TRY(cudaMemsetAsync(a.d_pool_cursor, 0, sizeof(unsigned long long), st));
-        knn_score_lists_kernel<<<blocks, 256, 0, st>>>(a);
-    } else {
-        knn_score_kernel<<<blocks, 256, 0, st>>>(a);
-    }
+    knn_score_lists_kernel<<<blocks, 256, 0, st>>>(a);
     LK_CUDA_TRY(cudaGetLastError());
     return LK_OK;
 }

@@ -31,8 +31,6 @@ TF32_CHUNK_NNZ_K128 = 256
 ALS_MAX_FEATURES = 128
 KNN_SCORE_MAX_NBRS = 128
 KNN_MERGE_SMEM_LIMIT = 200 * 1024  # n_halves * save_nbrs * 16 B must fit (lk_knn_merge_topk)
-#: optional int64[8] device tensor receiving per-phase cycle counters of the ALS kernels (diagnostics)
-PROF_BUFFER = None
 
 
 @dataclass
@@ -213,7 +211,6 @@ def als_half_epoch(
     a.d_status = ptr(plan.status)
     a.vals_uniform = 1 if plan.vals_uniform else 0
     a.uniform_val = plan.uniform_val
-    a.d_prof = ptr(PROF_BUFFER)
     a.d_cancel = ptr(cancel)  # optional device flag: non-zero stops the hand-out of rows (cooperative cancel)
     check(lib().lk_als_half_epoch(C.byref(a), stream_ptr()), "lk_als_half_epoch")
 
@@ -458,22 +455,12 @@ class KnnScorerState:
     work_counter: torch.Tensor
     status: torch.Tensor
     slotmap: torch.Tensor | None = None  # [warps, n_items] int32, all -1 between calls; grown on demand
-    heap_scratch: dict = field(default_factory=dict)  # (max_nbrs, warps) -> per-warp heap states
+    scratch: dict = field(default_factory=dict)  # contribution pool and cursor, the dense kernel's per-CTA rows
     lock: object = field(default_factory=threading.Lock)  # the mutable device state above is per-state
     #: user-kNN scoring (user_score.rs:21-98): the matrix is users x items ratings, a query's "history" is its
     #: neighbour list and carries the weights (lk_knn_score_args.user_mode)
     user_mode: bool = False
     n_rows: int = 0
-    HEAP_TARGETS_PER_WARP = 2048
-    USE_LISTS = True  # list-based kernel (parallel over the history); False: the sequential kernel
-    #: dense kernel: batches of at least this many queries are handed out longest history first.  Off by default:
-    #: measured 3.0 vs 2.7 ms per 4,096 ML-25M-shaped users (the heaviest queries, started together, contend for
-    #: L2), and a random position costs a wide batch less than that (tools/score_prof.py toggles it)
-    DENSE_LPT_MIN_QUERIES = 1 << 30
-
-    def kernel_name(self) -> str:
-        lists = self.USE_LISTS and _lib.get_option("LK_KNN_SCORE_SEQ") != 1
-        return "knn_score_lists_kernel" if lists else "knn_score_kernel"
 
     def _slotmap(self, n_queries: int) -> tuple[torch.Tensor, int]:
         """One slot-map row per working warp: min(n_queries, full grid) rows (a single query takes
@@ -483,16 +470,6 @@ class KnnScorerState:
             self.slotmap = None
             self.slotmap = torch.full((warps, self.n_items), -1, dtype=torch.int32, device=self.sim_cols.device)
         return self.slotmap, int(self.slotmap.shape[0])
-
-    def _heap(self, max_nbrs: int, warps: int) -> tuple[torch.Tensor, int]:
-        """Heap states of the sequential kernel (only allocated when that kernel will run)."""
-        per_warp = self.HEAP_TARGETS_PER_WARP * (2 + 2 * (int(max_nbrs) + 1))
-        key = int(max_nbrs)
-        t = self.heap_scratch.get(key)
-        if t is None or t.numel() < warps * per_warp:
-            t = torch.empty(warps * per_warp, dtype=torch.float32, device=self.sim_cols.device)
-            self.heap_scratch[key] = t
-        return t, per_warp
 
     @classmethod
     def create(cls, n_items: int, indptr, cols, vals, device=None, user_mode: bool = False) -> "KnnScorerState":
@@ -529,10 +506,15 @@ class KnnScorerState:
         min_nbrs: int,
     ) -> tuple[torch.Tensor, torch.Tensor]:
         """Score a batch of queries; returns (scores with NaN nulls, counts with -1 nulls)."""
-        if not 1 <= int(max_nbrs) <= KNN_SCORE_MAX_NBRS:
-            raise ValueError(f"max_nbrs must be in 1..{KNN_SCORE_MAX_NBRS}")
-        with self.lock:  # status word, work counter, pool and slot maps are shared by the callers of one state
-            return self._score_locked(ref_indptr, ref_items, ref_vals, tgt_indptr, tgt_items, max_nbrs, min_nbrs)
+        nt = tgt_items.numel()
+        lists = torch.empty((3, nt), dtype=torch.int32, device=self.sim_cols.device)  # offset, cursor, count
+
+        def target_lists(a: LkKnnScoreArgs) -> None:
+            slotmap, a.slotmap_warps = self._slotmap(ref_indptr.numel() - 1)
+            a.d_tgt_indptr, a.d_tgt_items, a.d_slotmap = ptr(tgt_indptr), ptr(tgt_items), ptr(slotmap)
+            a.d_list_off, a.d_list_cur, a.d_list_cnt = ptr(lists[0]), ptr(lists[1]), ptr(lists[2])
+
+        return self._launch((nt,), ref_indptr, ref_items, ref_vals, max_nbrs, min_nbrs, target_lists)
 
     def _pool_for(self, ref_items: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
         """Contribution pool: one 16-byte entry per (history entry, matrix-row entry) pair of the batch."""
@@ -542,12 +524,12 @@ class KnnScorerState:
         ok = (r >= 0) & (r < n_rows)
         rr = r.clamp(0, n_rows - 1)
         total = int(((self.sim_indptr[rr + 1] - self.sim_indptr[rr]) * ok).sum().item())
-        pool = self.heap_scratch.get("pool")
+        pool = self.scratch.get("pool")
         if pool is None or pool.numel() < 4 * max(total, 1):
             pool = torch.empty(4 * max(total, 1), dtype=torch.int32, device=dev)
-            self.heap_scratch["pool"] = pool
-            self.heap_scratch["pool_cursor"] = torch.zeros(1, dtype=torch.int64, device=dev)
-        return pool, self.heap_scratch["pool_cursor"]
+            self.scratch["pool"] = pool
+            self.scratch["pool_cursor"] = torch.zeros(1, dtype=torch.int64, device=dev)
+        return pool, self.scratch["pool_cursor"]
 
     def score_all_items(
         self, ref_indptr: torch.Tensor, ref_items: torch.Tensor, ref_vals: torch.Tensor | None, max_nbrs: int, min_nbrs: int
@@ -557,95 +539,63 @@ class KnnScorerState:
         with NaN nulls, counts [n_queries, n_items]).  Runs ``knn_score_dense_kernel`` — a CTA per query,
         cost proportional to the contributions plus one streaming fill of the output.
         """
-        if not 1 <= int(max_nbrs) <= KNN_SCORE_MAX_NBRS:
-            raise ValueError(f"max_nbrs must be in 1..{KNN_SCORE_MAX_NBRS}")
-        with self.lock:
-            dev = self.sim_cols.device
-            nq, ni = ref_indptr.numel() - 1, self.n_items
-            scores = torch.empty((nq, ni), dtype=torch.float32, device=dev)
-            counts = torch.empty((nq, ni), dtype=torch.int32, device=dev)
+
+        def per_cta_rows(a: LkKnnScoreArgs) -> None:
             ctas = int(lib().lk_knn_score_dense_ctas())
             # per-CTA state of the dense kernel: a slot map (item -> touched-target number; zero between queries
             # and between launches) and two compact rows indexed by touched-target number
-            ws = self.heap_scratch.get("dense_ws")
-            if ws is None:
-                ws = self.heap_scratch["dense_ws"] = (
-                    torch.empty(ctas * ni, dtype=torch.int32, device=dev), torch.empty(ctas * ni, dtype=torch.int32, device=dev),
-                    torch.zeros(ctas * ni, dtype=torch.int32, device=dev),
+            rows = self.scratch.get("dense")
+            if rows is None:
+                dev, n = self.sim_cols.device, ctas * self.n_items
+                rows = self.scratch["dense"] = (
+                    torch.empty(n, dtype=torch.int32, device=dev), torch.empty(n, dtype=torch.int32, device=dev),
+                    torch.zeros(n, dtype=torch.int32, device=dev),
                 )  # fmt: skip
-            off, cur, spill = ws
-            self.status.zero_()
-            pool, cursor = self._pool_for(ref_items)
+            off, cur, slotmap = rows
+            a.d_list_off, a.d_list_cur = ptr(off), ptr(cur)
+            a.d_slotmap, a.slotmap_warps = ptr(slotmap), ctas
+
+        shape = (ref_indptr.numel() - 1, self.n_items)
+        return self._launch(shape, ref_indptr, ref_items, ref_vals, max_nbrs, min_nbrs, per_cta_rows)
+
+    def _launch(self, out_shape, ref_indptr, ref_items, ref_vals, max_nbrs, min_nbrs, fill_mode):
+        """What both modes share: the ``max_nbrs`` check, the outputs, the common ``lk_knn_score_args`` fields, the
+        launch, the wait and the status word.  ``fill_mode(args)`` sets the mode's own fields (with the lock held;
+        the scratch they point to must outlive this call)."""
+        if not 1 <= int(max_nbrs) <= KNN_SCORE_MAX_NBRS:
+            raise ValueError(f"max_nbrs must be in 1..{KNN_SCORE_MAX_NBRS}")
+        dev = self.sim_cols.device
+        scores = torch.empty(out_shape, dtype=torch.float32, device=dev)
+        counts = torch.empty(out_shape, dtype=torch.int32, device=dev)
+        if scores.numel() == 0:  # no targets (or no queries): nothing to score
+            return scores, counts
+        if ref_items.numel() == 0:
+            # every history is empty: the address of an empty tensor is NULL, which the library rejects; the
+            # kernels never read these placeholders because the indptr bounds every read
+            ref_items = torch.full((1,), -1, dtype=torch.int32, device=dev)
+            ref_vals = None if ref_vals is None else torch.zeros(1, dtype=torch.float32, device=dev)
+        with self.lock:  # status word, work counter, pool and slot maps are shared by the callers of one state
             a = LkKnnScoreArgs()
-            a.n_items = ni
+            fill_mode(a)
+            pool, cursor = self._pool_for(ref_items)
+            a.n_items = self.n_items
             a.d_sim_indptr, a.d_sim_cols, a.d_sim_vals = ptr(self.sim_indptr), ptr(self.sim_cols), ptr(self.sim_vals)
-            a.n_queries = nq
+            a.n_queries = ref_indptr.numel() - 1
             a.d_ref_indptr, a.d_ref_items, a.d_ref_vals = ptr(ref_indptr), ptr(ref_items), ptr(ref_vals)
             a.max_nbrs, a.min_nbrs = int(max_nbrs), int(min_nbrs)
-            a.d_acc_ws, a.d_acc_tw = ptr(off), ptr(cur)
             a.d_scores, a.d_counts = ptr(scores), ptr(counts)
             a.d_work_counter, a.d_status = ptr(self.work_counter), ptr(self.status)
             a.user_mode, a.n_matrix_rows = (1 if self.user_mode else 0), self.n_rows
             a.d_pool, a.pool_entries, a.d_pool_cursor = ptr(pool), pool.numel() // 4, ptr(cursor)
-            a.d_slotmap, a.slotmap_warps = ptr(spill), ctas  # per-CTA slot maps (all zero between launches)
-            order = None
-            if nq >= self.DENSE_LPT_MIN_QUERIES:
-                # longest histories first: a query costs what its history contributes, and the launch ends with
-                # its last query
-                order = torch.argsort(ref_indptr[1:] - ref_indptr[:-1], descending=True).to(torch.int32)
-                a.d_deferred = ptr(order)
+            self.status.zero_()
             check(lib().lk_knn_score_batch(C.byref(a), stream_ptr()), "lk_knn_score_batch")
             torch.cuda.current_stream().synchronize()
             st = int(self.status.item())
-            if st == 2:
-                raise ValueError("similarity is null")
-            if st == 3:
-                raise _lib.EngineError("lk_knn_score_batch: contribution pool too small")
-        return scores, counts
-
-    def _score_locked(self, ref_indptr, ref_items, ref_vals, tgt_indptr, tgt_items, max_nbrs, min_nbrs):
-        dev = self.sim_cols.device
-        nq = ref_indptr.numel() - 1
-        nt = tgt_items.numel()
-        scores = torch.empty(max(nt, 1), dtype=torch.float32, device=dev)
-        counts = torch.empty(max(nt, 1), dtype=torch.int32, device=dev)
-        acc_ws = torch.empty(max(nt, 1), dtype=torch.float32, device=dev)
-        acc_tw = torch.empty(max(nt, 1), dtype=torch.float32, device=dev)
-        acc_cnt = torch.empty(max(nt, 1), dtype=torch.int32, device=dev)
-        self.status.zero_()
-        slotmap, warps = self._slotmap(nq)
-        a = LkKnnScoreArgs()
-        a.n_items = self.n_items
-        a.d_sim_indptr, a.d_sim_cols, a.d_sim_vals = ptr(self.sim_indptr), ptr(self.sim_cols), ptr(self.sim_vals)
-        a.n_queries = nq
-        a.d_ref_indptr, a.d_ref_items, a.d_ref_vals = ptr(ref_indptr), ptr(ref_items), ptr(ref_vals)
-        a.d_tgt_indptr, a.d_tgt_items = ptr(tgt_indptr), ptr(tgt_items)
-        a.max_nbrs, a.min_nbrs = int(max_nbrs), int(min_nbrs)
-        a.d_slotmap, a.slotmap_warps = ptr(slotmap), warps
-        a.d_acc_ws, a.d_acc_tw, a.d_acc_cnt = ptr(acc_ws), ptr(acc_tw), ptr(acc_cnt)
-        a.d_scores, a.d_counts = ptr(scores), ptr(counts)
-        a.d_work_counter, a.d_status = ptr(self.work_counter), ptr(self.status)
-        a.user_mode, a.n_matrix_rows = (1 if self.user_mode else 0), self.n_rows
-        use_lists = self.USE_LISTS and ref_items.numel() > 0 and _lib.get_option("LK_KNN_SCORE_SEQ") != 1
-        if use_lists:
-            # contribution pool for the list-based kernel: one 16-byte entry per (reference item,
-            # similarity-row entry) pair of the batch
-            pool, cursor = self._pool_for(ref_items)
-            a.d_pool, a.pool_entries = ptr(pool), pool.numel() // 4
-            a.d_pool_cursor = ptr(cursor)
-        else:
-            # the sequential kernel is the one that reads the per-warp heap states
-            heap, per_warp = self._heap(max_nbrs, warps)
-            a.d_heap_scratch, a.heap_floats_per_warp = ptr(heap), per_warp
-        check(lib().lk_knn_score_batch(C.byref(a), stream_ptr()), "lk_knn_score_batch")
-        # keep scratch alive until the stream has consumed it
-        torch.cuda.current_stream().synchronize()
-        st = int(self.status.item())
         if st == 2:
             raise ValueError("similarity is null")
         if st == 3:
             raise _lib.EngineError("lk_knn_score_batch: contribution pool too small")
-        return scores[:nt], counts[:nt]
+        return scores, counts
 
 
 # ---------------------------------------------------------------------------

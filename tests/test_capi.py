@@ -26,7 +26,7 @@ def test_header_symbols_exported(cuda_lib):
     nm = subprocess.run(["nm", "-D", "--defined-only", str(_build.LIB)], capture_output=True, text=True, check=True)
     exported = set(re.findall(r"\bT (lk_\w+)", nm.stdout))
     assert declared <= exported, declared - exported
-    assert cuda_lib.lk_version() >= 100
+    assert cuda_lib.lk_version() >= 101
     assert cuda_lib.lk_als_max_features() == 128
 
 

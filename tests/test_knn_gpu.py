@@ -140,17 +140,6 @@ def _score_gpu(S, queries, max_nbrs, min_nbrs, explicit=True):
     return sc.cpu().numpy(), ct.cpu().numpy(), tgt_ptr
 
 
-@pytest.mark.parametrize("heap_cap", [2048, 2, 0])
-def test_score_heap_scratch_sizes(cuda_lib, ml_small, monkeypatch, heap_cap):
-    """Targets beyond max_nbrs keep their heap in the per-warp scratch (step 2b of the kernel); when
-    it is too small (2 targets) or absent (0) the rest is replayed one by one — same bits either way."""
-    monkeypatch.setattr(engine.KnnScorerState, "HEAP_TARGETS_PER_WARP", heap_cap)
-    monkeypatch.setattr(engine.KnnScorerState, "USE_LISTS", False)  # the sequential kernel
-    test_score_matches_oracle_exactly(cuda_lib, ml_small, True, 5, None)
-    test_score_matches_oracle_exactly(cuda_lib, ml_small, False, 3, None)
-    test_score_matches_oracle_exactly(cuda_lib, ml_small, True, 20, 20)
-
-
 @pytest.mark.parametrize("explicit", [True, False])
 @pytest.mark.parametrize("max_nbrs,save_nbrs", [(20, None), (5, None), (20, 20), (3, 50)])
 def test_score_matches_oracle_exactly(cuda_lib, ml_small, explicit, max_nbrs, save_nbrs):
@@ -225,6 +214,51 @@ def test_score_all_items_dense_kernel(cuda_lib, ml_small, explicit, max_nbrs, sa
         assert np.array_equal(np.isnan(sc[qi]), np.isnan(osc))
         ok = ~np.isnan(osc)
         assert np.array_equal(sc[qi][ok].view(np.int32), osc[ok].view(np.int32))
+
+
+def test_score_empty_histories_and_no_targets(cuda_lib, ml_small):
+    """Zero-length inputs give the oracle's answer, in item and user mode: a batch whose histories (neighbour
+    lists) are all empty scores every target as having no neighbours, and a call with no targets (or, for all
+    items, no queries) returns empty results."""
+    ui, iu, _ = data.knn_item_matrices(ml_small, True)
+    S = oracle.knn_build(ui, iu, 1e-6, 20)
+    R = ml_small.coo().tocsr().astype(np.float32)
+    dev = _lib.require_device()
+    t = lambda a: torch.from_numpy(np.asarray(a)).to(dev)  # noqa: E731
+    none_i, none_f = np.zeros(0, np.int32), np.zeros(0, np.float32)
+    hist_i, hist_f = np.array([1, 5, 30], np.int32), np.array([0.5, -1.0, 0.25], np.float32)
+    ti = np.array([3, -1, 7, 31, 5, 3], np.int32)
+
+    def check(got, ref):
+        sc, ct = (x.cpu().numpy() for x in got)
+        osc, oct_ = ref
+        assert sc.shape == osc.shape and np.array_equal(ct, oct_)
+        assert np.array_equal(np.isnan(sc), np.isnan(osc))
+        ok = ~np.isnan(osc)
+        assert np.array_equal(sc[ok].view(np.int32), osc[ok].view(np.int32))
+
+    item = engine.KnnScorerState.create(S.shape[0], S.indptr, S.indices, S.data, dev)
+    for explicit in (True, False):
+        rv = none_f if explicit else None
+        got = item.score(t([0, 0, 0]), t(none_i), None if rv is None else t(rv), t([0, 4, 6]), t(ti), 20, 1)
+        check(got, oracle.knn_score(S, none_i, rv, ti, 20, 1))
+        hv = hist_f if explicit else None
+        got = item.score(t([0, 3]), t(hist_i), None if hv is None else t(hv), t([0, 0]), t(none_i), 20, 1)
+        check(got, oracle.knn_score(S, hist_i, hv, none_i, 20, 1))
+        sc, ct = item.score_all_items(t([0, 0, 0]), t(none_i), None if rv is None else t(rv), 20, 1)
+        all_items = np.arange(S.shape[0], dtype=np.int32)
+        for q in range(2):
+            check((sc[q], ct[q]), oracle.knn_score(S, none_i, rv, all_items, 20, 1))
+        sc, ct = item.score_all_items(t([0]), t(none_i), None if rv is None else t(rv), 20, 1)
+        assert sc.shape == ct.shape == (0, S.shape[0])
+
+    for explicit in (True, False):
+        user = engine.KnnScorerState.create(R.shape[1], R.indptr, R.indices, R.data if explicit else None, dev,
+                                            user_mode=True)  # fmt: skip
+        got = user.score(t([0, 0]), t(none_i), t(none_f), t([0, 6]), t(ti), 20, 1)
+        check(got, oracle.user_score(R, none_i, none_f, ti, 20, 1, explicit))
+        got = user.score(t([0, 3]), t(hist_i), t(np.abs(hist_f)), t([0, 0]), t(none_i), 20, 1)
+        check(got, oracle.user_score(R, hist_i, np.abs(hist_f), none_i, 20, 1, explicit))
 
 
 def test_golden_predictions_end_to_end(cuda_lib, ml_small):

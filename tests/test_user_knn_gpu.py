@@ -28,10 +28,8 @@ def _bits_equal(got_s, got_c, ref_s, ref_c):
 
 
 @pytest.mark.parametrize("explicit", [True, False])
-@pytest.mark.parametrize("max_nbrs", [20, 3])
-@pytest.mark.parametrize("lists", [True, False])
-def test_user_score_matches_oracle_exactly(cuda_lib, ml_small, explicit, max_nbrs, lists, monkeypatch):
-    monkeypatch.setattr(engine.KnnScorerState, "USE_LISTS", lists)
+@pytest.mark.parametrize("max_nbrs", [20, 3, 1, 128])  # 1 and 128: the smallest and largest accumulator
+def test_user_score_matches_oracle_exactly(cuda_lib, ml_small, explicit, max_nbrs):
     m = UserKNNScorer(feedback="explicit" if explicit else "implicit", max_nbrs=max_nbrs)
     m.train(Dataset(ml_small))
     R = m.user_ratings

@@ -24,8 +24,7 @@ ref_ptr = t(R.indptr[: n_q + 1].astype(np.int64))
 ri = t(R.indices[:a1].astype(np.int32))
 rv = t((R.data[:a1] - means.cpu().numpy()[R.indices[:a1]]).astype(np.float32))
 for ctas in ([int(x) for x in sys.argv[2].split(",")] if len(sys.argv) > 2 else [-1]):
-    _lib.set_option("LK_KNN_SCORE_CTAS", abs(ctas) if ctas != -1 else -1)
-    engine.KnnScorerState.DENSE_LPT_MIN_QUERIES = 2 if ctas >= -1 else 1 << 30  # a negative count other than -1: index order
+    _lib.set_option("LK_KNN_SCORE_CTAS", ctas)
     for rep in range(2):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
