@@ -13,6 +13,7 @@
  *   POSV::solve (LAPACK sposv)                    src/accel/als/solve.rs:65-106     in-kernel Cholesky
  *   _accel.knn.compute_similarities               src/accel/knn/item_train.rs:32-93 lk_knn_geometry + lk_knn_build
  *   _accel.knn.score_explicit / score_implicit    src/accel/knn/item_score.rs:22-111 lk_knn_score_batch
+ *   UserKNNScorer neighbours (SciPy, host)        src/lenskit/knn/user.py:189-214   lk_uknn_search
  *   _accel.data.argtopn (SURVEY.md 8f, "next")    src/accel/data/sorting.rs:131-170 lk_topn_columns
  *
  * Conventions
@@ -218,6 +219,64 @@ LK_API int lk_knn_merge_topk(const lk_knn_build_args *args, int32_t *d_out_cols,
  * d_out_indptr [n_items+1] (int64, exclusive scan of the per-row counts). */
 LK_API int lk_knn_pool_to_csr(const lk_knn_build_args *args, const int64_t *d_out_indptr,
                        int32_t *d_out_cols, float *d_out_vals, void *stream);
+
+/* ------------------------------------------------------------------------- */
+/* user-kNN neighbour search (batched)                                        */
+/* ------------------------------------------------------------------------- */
+
+/*
+ * The neighbour step of UserKNNScorer (src/lenskit/knn/user.py:189-214): for a batch of sparse query
+ * vectors x_q, the users v with sim(q, v) = sum over the query's items i, ASCENDING, of VT[i,v] * x_q[i]
+ * >= min_sim and v != self(q), in ascending v, with (float)sim as the weight.  VT is the item-major copy
+ * of the f64 user_vectors matrix.  Every sum is accumulated in f64 in ascending item order with an
+ * unfused multiply and add per step, starting from +0.0 — the order and rounding of SciPy's f64
+ * `user_vectors @ x` (items outside the query only add +-0.0, which cannot change a nonzero sum), so the
+ * neighbour set and the f32 weights are those of the reference bit for bit.  The comparison with min_sim
+ * is made on the f64 sum.  See knn_user.cu.
+ *
+ * Geometry: the f64 accumulators of one query are tiled over the users; a CTA holds n_halves-th of them
+ * (geom.warps sub-tiles of geom.tile_cols users).  In lk_knn_geom's own terms VT plays UI: its rows
+ * (items) are geom.n_users and its columns (users) geom.n_items, so lk_knn_tile_pointers over VT with
+ * this geometry gives d_tile_ptr [n_items * (n_subtiles+1)].  ctas_per_sm 0 = default (2).
+ */
+LK_API int lk_uknn_geometry(int32_t n_users, int32_t n_items, int32_t ctas_per_sm, lk_knn_geom *geom);
+
+typedef struct lk_uknn_search_args {
+    lk_knn_geom geom;                 /* lk_uknn_geometry */
+    const int32_t *d_vt_indptr;       /* [n_items+1] VT: items x users */
+    const int32_t *d_vt_users;        /* [nnz] users ascending within an item */
+    const double *d_vt_vals;          /* [nnz] user_vectors values (f64) */
+    const int32_t *d_tile_ptr;        /* lk_knn_tile_pointers(geom, d_vt_indptr, d_vt_users) */
+    int32_t n_queries;                /* B; B * geom.n_halves < 2^31 */
+    const int64_t *d_q_begin;         /* [B] query q is entries [d_q_begin[q], d_q_end[q]) of d_q_items / d_q_vals */
+    const int64_t *d_q_end;           /* [B] (e.g. rows of the row-major user_vectors, or an uploaded CSR) */
+    const int32_t *d_q_items;         /* items strictly ascending within a query, in [0, n_items) */
+    const double *d_q_vals;           /* f64 query values */
+    const int32_t *d_q_self;          /* [B] user excluded from query q's neighbours, or -1; NULL = none */
+    double min_sim;                   /* keep sim >= min_sim, compared in f64; > 0 */
+    /* work units: unit id = q * n_halves + h (query q, user tile h); d_sched [n_work] lists the units to
+     * process, most expensive first.  Units not listed produce nothing (their d_part_cnt stays as given). */
+    const int32_t *d_sched;
+    int64_t n_work;
+    /* survivors, bump-allocated per unit in tile order */
+    int32_t *d_pool_rows;             /* [pool_capacity] neighbour user */
+    float *d_pool_sims;               /* [pool_capacity] (float)sim */
+    int64_t pool_capacity;            /* e.g. sum over q of min(lk_uknn_query_cost(q), n_users) */
+    int64_t *d_pool_off;              /* [B * n_halves] offset of the unit's segment */
+    int32_t *d_part_cnt;              /* [B * n_halves] length of the unit's segment */
+    unsigned long long *d_pool_cursor; /* [1] zeroed by the call */
+    int32_t *d_work_counter;          /* [1] zeroed by the call */
+    int32_t *d_status;                /* [1] zeroed by the call; 1 = pool overflow (then nothing is usable) */
+} lk_uknn_search_args;
+
+/* d_cost [B] (int64): sum over the query's items of |VT row| — the products of its search. */
+LK_API int lk_uknn_query_cost(const lk_uknn_search_args *args, int64_t *d_cost, void *stream);
+LK_API int lk_uknn_search(const lk_uknn_search_args *args, void *stream);
+/* Gather the pool segments into CSR: d_out_indptr [B+1] (int64, exclusive scan of the per-query sums of
+ * d_part_cnt) -> d_out_rows / d_out_sims, rows ascending within a query.  This is the neighbour-list layout
+ * lk_knn_score_batch takes in user mode (d_ref_indptr / d_ref_items / d_ref_vals). */
+LK_API int lk_uknn_pool_to_csr(const lk_uknn_search_args *args, const int64_t *d_out_indptr, int32_t *d_out_rows,
+                               float *d_out_sims, void *stream);
 
 /* ------------------------------------------------------------------------- */
 /* item-kNN input preparation (SURVEY.md 8f N4)                               */

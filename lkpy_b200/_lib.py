@@ -137,6 +137,33 @@ class LkKnnScoreArgs(C.Structure):
     ]
 
 
+class LkUknnSearchArgs(C.Structure):
+    _fields_ = [
+        ("geom", LkKnnGeom),
+        ("d_vt_indptr", vp),
+        ("d_vt_users", vp),
+        ("d_vt_vals", vp),
+        ("d_tile_ptr", vp),
+        ("n_queries", C.c_int32),
+        ("d_q_begin", vp),
+        ("d_q_end", vp),
+        ("d_q_items", vp),
+        ("d_q_vals", vp),
+        ("d_q_self", vp),
+        ("min_sim", C.c_double),
+        ("d_sched", vp),
+        ("n_work", C.c_int64),
+        ("d_pool_rows", vp),
+        ("d_pool_sims", vp),
+        ("pool_capacity", C.c_int64),
+        ("d_pool_off", vp),
+        ("d_part_cnt", vp),
+        ("d_pool_cursor", vp),
+        ("d_work_counter", vp),
+        ("d_status", vp),
+    ]
+
+
 #: every symbol ``include/lkpy_b200.h`` declares: name -> (restype, argtypes)
 SYMBOLS: dict[str, tuple] = {
     "lk_version": (C.c_int, []),
@@ -158,6 +185,10 @@ SYMBOLS: dict[str, tuple] = {
     "lk_knn_build": (C.c_int, [C.POINTER(LkKnnBuildArgs), vp]),
     "lk_knn_merge_topk": (C.c_int, [C.POINTER(LkKnnBuildArgs), vp, vp, vp, vp]),
     "lk_knn_pool_to_csr": (C.c_int, [C.POINTER(LkKnnBuildArgs), vp, vp, vp, vp]),
+    "lk_uknn_geometry": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(LkKnnGeom)]),
+    "lk_uknn_query_cost": (C.c_int, [C.POINTER(LkUknnSearchArgs), vp, vp]),
+    "lk_uknn_search": (C.c_int, [C.POINTER(LkUknnSearchArgs), vp]),
+    "lk_uknn_pool_to_csr": (C.c_int, [C.POINTER(LkUknnSearchArgs), vp, vp, vp, vp]),
     "lk_knn_prep_columns": (C.c_int, [vp, vp, C.c_int32, C.c_int32, vp, vp, vp]),
     "lk_knn_score_warps": (C.c_int64, []),
     "lk_knn_score_dense_ctas": (C.c_int64, []),

@@ -524,17 +524,9 @@ __global__ void pool_to_csr_kernel(lk_knn_build_args a, const int64_t *__restric
     const int warps = (gridDim.x * blockDim.x) >> 5;
     const int lane = threadIdx.x & 31;
     for (int item = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; item < a.geom.n_items; item += warps) {
-        int64_t dst = out_indptr[item];
         // unbounded mode has one unit per (item, half), in column order
-        for (int u = a.d_unit_ptr[item]; u < a.d_unit_ptr[item + 1]; u++) {
-            const int64_t src = a.d_pool_off[u];
-            const int c = a.d_part_cnt[u];
-            for (int t = lane; t < c; t += 32) {
-                out_cols[dst + t] = a.d_pool_cols[src + t];
-                out_vals[dst + t] = a.d_pool_vals[src + t];
-            }
-            dst += c;
-        }
+        warp_copy_pool_segments(a.d_unit_ptr[item], a.d_unit_ptr[item + 1], a.d_pool_off, a.d_part_cnt,
+                                a.d_pool_cols, a.d_pool_vals, out_indptr[item], out_cols, out_vals, lane);
     }
 }
 

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import LkAlsArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnScoreArgs, check, lib, ptr, stream_ptr
+from ._lib import LkAlsArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnScoreArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr
 from .data import InteractionCSR
 
 DEFAULT_CHUNK_NNZ = 4096
@@ -596,6 +596,225 @@ class KnnScorerState:
         if st == 3:
             raise _lib.EngineError("lk_knn_score_batch: contribution pool too small")
         return scores, counts
+
+
+# ---------------------------------------------------------------------------
+# user-kNN neighbour search
+# ---------------------------------------------------------------------------
+
+
+def history_query(item_nums: np.ndarray, ratings: np.ndarray | None) -> tuple[np.ndarray, np.ndarray, float]:
+    """
+    The sparse query vector of a provided history, as ``UserKNNScorer._get_user_data`` builds it densely
+    (``user.py:274-298``): ``item_nums`` are the history's item numbers (negative = unknown item, dropped),
+    ``ratings`` its ratings (explicit feedback: centred by their f32 mean over the whole history, unknown
+    items included) or None (implicit feedback: 1.0).  A repeated item keeps its LAST value, as the
+    reference's ``ratings[idx] = ...`` does.  Returns (items int32 strictly ascending, values f64, mean).
+    """
+    nums = np.asarray(item_nums, dtype=np.int64)
+    if ratings is None:
+        umean = 0.0
+        vals = np.ones(len(nums), dtype=np.float32)
+    else:
+        urv = np.require(ratings, dtype=np.float32)
+        umean = float(urv.mean())
+        vals = urv - umean  # f32 arithmetic, as the reference's f32 rating vector
+    known = nums >= 0
+    nums, vals = nums[known], vals[known]
+    # last occurrence wins: the first occurrence in the reversed history
+    items, first = np.unique(nums[::-1], return_index=True)
+    vals = vals[::-1][first]
+    return items.astype(np.int32), vals.astype(np.float64), umean
+
+
+@dataclass
+class UserQueries:
+    """A batch of neighbour-search queries on the device: query q is entries ``[begin[q], end[q])`` of
+    ``items`` / ``vals`` (rows of ``V`` for known users, or uploaded histories); ``self_`` the user
+    excluded from its neighbours, or -1."""
+
+    begin: torch.Tensor  # int64 [B]
+    end: torch.Tensor  # int64 [B]
+    items: torch.Tensor  # int32
+    vals: torch.Tensor  # float64
+    self_: torch.Tensor  # int32 [B]
+
+    @property
+    def n(self) -> int:
+        return int(self.begin.numel())
+
+
+@dataclass
+class UserNeighbourState:
+    """
+    The unit-normalised f64 user vectors in HBM in both orientations — ``V`` (users x items, the rows of
+    known-user queries) and ``VT`` (items x users, what the search gathers) — with the accumulator
+    geometry and tile pointers of ``lk_uknn_search``.  At the ML-25M shape (25 M ratings) V and VT take
+    12 B per rating each, 600 MB together, and the tile pointers 46 MB.
+    """
+
+    n_users: int
+    n_items: int
+    v_indptr: torch.Tensor  # int32 [n_users + 1]
+    v_items: torch.Tensor  # int32
+    v_vals: torch.Tensor  # float64
+    h_v_indptr: np.ndarray
+    vt_indptr: torch.Tensor  # int32 [n_items + 1]
+    vt_users: torch.Tensor
+    vt_vals: torch.Tensor
+    geom: LkKnnGeom
+    tile_ptr: torch.Tensor
+    work_counter: torch.Tensor
+    status: torch.Tensor
+    cursor: torch.Tensor
+    lock: object = field(default_factory=threading.Lock)
+
+    @classmethod
+    def create(cls, user_vectors, device=None, ctas_per_sm: int = 0) -> "UserNeighbourState":
+        """``user_vectors``: the SciPy CSR (f64) of ``UserKNNScorer.train``."""
+        import scipy.sparse as sps
+
+        device = device or _lib.require_device()
+        v = sps.csr_array(user_vectors, dtype=np.float64)
+        v.sort_indices()
+        vt = sps.csr_array(v.T)
+        vt.sort_indices()
+        if v.nnz >= 2**31:
+            raise _lib.EngineError("user vectors with nnz >= 2**31 are not supported")
+        n_users, n_items = v.shape
+        L = lib()
+        g = LkKnnGeom()
+        check(L.lk_uknn_geometry(n_users, n_items, int(ctas_per_sm), C.byref(g)), "lk_uknn_geometry")
+
+        def up(a, dt):
+            return torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(device)
+
+        vt_indptr, vt_users = up(vt.indptr, np.int32), up(vt.indices, np.int32)
+        tile_ptr = torch.empty(max(1, n_items * (g.n_subtiles + 1)), dtype=torch.int32, device=device)
+        if n_items > 0:
+            check(
+                L.lk_knn_tile_pointers(C.byref(g), ptr(vt_indptr), ptr(vt_users), ptr(tile_ptr), stream_ptr()),
+                "lk_knn_tile_pointers",
+            )
+        z = lambda dt: torch.zeros(1, dtype=dt, device=device)  # noqa: E731
+        return cls(
+            n_users, n_items, up(v.indptr, np.int32), up(v.indices, np.int32), up(v.data, np.float64),
+            np.ascontiguousarray(v.indptr, dtype=np.int64), vt_indptr, vt_users, up(vt.data, np.float64),
+            g, tile_ptr, z(torch.int32), z(torch.int32), z(torch.int64),
+        )  # fmt: skip
+
+    @property
+    def device(self):
+        return self.v_indptr.device
+
+    def known_queries(self, users) -> UserQueries:
+        """Queries that are rows of ``V``: only the user numbers are uploaded; each user is its own self."""
+        u = torch.as_tensor(np.asarray(users, dtype=np.int64)).to(self.device)
+        if u.numel() and (int(u.min()) < 0 or int(u.max()) >= self.n_users):
+            raise IndexError("user number out of range")
+        ip = self.v_indptr.to(torch.int64)
+        return UserQueries(ip[u].contiguous(), ip[u + 1].contiguous(), self.v_items, self.v_vals, u.to(torch.int32))
+
+    def queries(self, specs) -> UserQueries:
+        """
+        A mixed batch.  Each spec is a known user number (its row of ``V``) or a tuple ``(items, vals, self)``
+        from :func:`history_query` (``self`` a user number or None).  Known rows are gathered on the device.
+        """
+        if all(not isinstance(s, tuple) for s in specs):
+            return self.known_queries([int(s) for s in specs])
+        dev = self.device
+        hv = self.h_v_indptr
+        k_at = [i for i, s in enumerate(specs) if not isinstance(s, tuple)]
+        k_users = np.array([int(specs[i]) for i in k_at], dtype=np.int64)
+        k_len = (hv[k_users + 1] - hv[k_users]) if len(k_at) else np.zeros(0, np.int64)
+        k_start = np.concatenate([[0], np.cumsum(k_len)]).astype(np.int64)
+        k_tot = int(k_start[-1])
+        hist = [specs[i] for i in range(len(specs)) if isinstance(specs[i], tuple)]
+        h_len = np.array([len(h[0]) for h in hist], dtype=np.int64)
+        h_start = k_tot + np.concatenate([[0], np.cumsum(h_len)]).astype(np.int64)
+        begin = np.empty(len(specs), np.int64)
+        end = np.empty(len(specs), np.int64)
+        self_ = np.empty(len(specs), np.int32)
+        begin[k_at], end[k_at], self_[k_at] = k_start[:-1], k_start[1:], k_users
+        h_at = [i for i, s in enumerate(specs) if isinstance(s, tuple)]
+        begin[h_at], end[h_at] = h_start[:-1], h_start[1:]
+        self_[h_at] = [-1 if h[2] is None else int(h[2]) for h in hist]
+        items = torch.empty(max(1, int(h_start[-1])), dtype=torch.int32, device=dev)
+        vals = torch.zeros(max(1, int(h_start[-1])), dtype=torch.float64, device=dev)
+        if k_tot:  # V rows, gathered on the device: position p of known query j comes from hv[u_j] + p - k_start[j]
+            shift = torch.from_numpy(hv[k_users] - k_start[:-1]).to(dev)
+            src = torch.repeat_interleave(shift, torch.from_numpy(k_len).to(dev), output_size=k_tot)
+            src += torch.arange(k_tot, device=dev)
+            items[:k_tot] = self.v_items[src]
+            vals[:k_tot] = self.v_vals[src]
+        if len(hist) and h_start[-1] > k_tot:
+            items[k_tot : h_start[-1]] = torch.from_numpy(np.concatenate([h[0] for h in hist]).astype(np.int32)).to(dev)
+            vals[k_tot : h_start[-1]] = torch.from_numpy(np.concatenate([h[1] for h in hist]).astype(np.float64)).to(dev)
+        t = lambda a: torch.from_numpy(a).to(dev)  # noqa: E731
+        return UserQueries(t(begin), t(end), items, vals, t(self_))
+
+    def _args(self, qs: UserQueries, min_sim: float) -> LkUknnSearchArgs:
+        a = LkUknnSearchArgs()
+        a.geom = self.geom
+        a.d_vt_indptr, a.d_vt_users, a.d_vt_vals = ptr(self.vt_indptr), ptr(self.vt_users), ptr(self.vt_vals)
+        a.d_tile_ptr = ptr(self.tile_ptr)
+        a.n_queries = qs.n
+        a.d_q_begin, a.d_q_end, a.d_q_items, a.d_q_vals = ptr(qs.begin), ptr(qs.end), ptr(qs.items), ptr(qs.vals)
+        a.d_q_self = ptr(qs.self_)
+        a.min_sim = float(min_sim)
+        a.d_work_counter, a.d_status, a.d_pool_cursor = ptr(self.work_counter), ptr(self.status), ptr(self.cursor)
+        return a
+
+    def query_cost(self, qs: UserQueries) -> torch.Tensor:
+        """Products of each query's search: the summed ``VT`` row lengths of its items (int64 [B])."""
+        cost = torch.zeros(max(qs.n, 1), dtype=torch.int64, device=self.device)
+        check(lib().lk_uknn_query_cost(C.byref(self._args(qs, 1.0)), ptr(cost), stream_ptr()), "lk_uknn_query_cost")
+        return cost[: qs.n]
+
+    def neighbours(
+        self, qs: UserQueries, min_sim: float, capacity: int | None = None
+    ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """
+        Every query's neighbours ``{v : sim >= min_sim, v != self}`` in ascending ``v``: device CSR (int64
+        indptr [B+1], int32 users, f32 similarities) — the user-mode neighbour lists of
+        ``KnnScorerState.score``.  ``capacity``: survivor pool entries (default: the bound
+        Σ_q min(products_q, n_users)); a pool too small raises :class:`EngineError`.
+        """
+        if not min_sim > 0:
+            raise ValueError("min_sim must be positive")
+        dev, B, H = self.device, qs.n, self.geom.n_halves
+        indptr = torch.zeros(B + 1, dtype=torch.int64, device=dev)
+        if B == 0:
+            return indptr, torch.empty(0, dtype=torch.int32, device=dev), torch.empty(0, dtype=torch.float32, device=dev)
+        if B * H >= 2**31:
+            raise _lib.EngineError(f"{B} queries x {H} user tiles exceed the work-unit numbering; split the batch")
+        L = lib()
+        cost = self.query_cost(qs)
+        order = torch.argsort(cost, descending=True, stable=True)
+        order = order[cost[order] > 0]  # a query without products has no neighbours and needs no unit
+        sched = (order[:, None] * H + torch.arange(H, device=dev)[None, :]).reshape(-1).to(torch.int32)
+        if capacity is None:
+            capacity = int(cost.clamp_max(self.n_users).sum().item())
+        capacity = max(int(capacity), 1)
+        pool_rows = torch.empty(capacity, dtype=torch.int32, device=dev)
+        pool_sims = torch.empty(capacity, dtype=torch.float32, device=dev)
+        pool_off = torch.zeros(B * H, dtype=torch.int64, device=dev)
+        part_cnt = torch.zeros(B * H, dtype=torch.int32, device=dev)
+        with self.lock:  # work counter, cursor and status word are per state
+            a = self._args(qs, min_sim)
+            a.d_sched, a.n_work = ptr(sched), sched.numel()
+            a.d_pool_rows, a.d_pool_sims, a.pool_capacity = ptr(pool_rows), ptr(pool_sims), capacity
+            a.d_pool_off, a.d_part_cnt = ptr(pool_off), ptr(part_cnt)
+            check(L.lk_uknn_search(C.byref(a), stream_ptr()), "lk_uknn_search")
+            st = int(self.status.item())
+        if st == 1:
+            raise _lib.EngineError("lk_uknn_search: neighbour pool overflow; pass a larger capacity")
+        torch.cumsum(part_cnt.view(B, H).sum(dim=1, dtype=torch.int64), 0, out=indptr[1:])
+        nnz = int(indptr[-1].item())
+        rows = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
+        sims = torch.empty(max(nnz, 1), dtype=torch.float32, device=dev)
+        check(L.lk_uknn_pool_to_csr(C.byref(a), ptr(indptr), ptr(rows), ptr(sims), stream_ptr()), "lk_uknn_pool_to_csr")
+        return indptr, rows[:nnz], sims[:nnz]
 
 
 # ---------------------------------------------------------------------------

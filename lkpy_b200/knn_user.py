@@ -3,13 +3,24 @@ User-kNN scorer on the H100 engine (SURVEY.md §8f N3) — the component surface
 ``lenskit.knn.user.UserKNNScorer`` (``src/lenskit/knn/user.py:41-300``).
 
 Training memorises the centred ratings and the unit-normalised user vectors exactly as the reference
-does (``user.py:112-155``, SciPy on the host: it is the model, not a hot path).  Scoring a query is
-(i) the neighbour similarities ``user_vectors @ ratings`` with the ``min_sim`` mask (``user.py:189-214``,
-kept on the host as in the reference) and (ii) the neighbourhood aggregation of
-``_accel.knn.user_score_items_{explicit,implicit}`` (``src/accel/knn/user_score.rs:21-98``), which
-runs on the device: the accumulator kernel of ``knn_score.cu`` in user mode — weights from the
-neighbour list, values from the rating matrix — bit-exact against the oracle's ScoreAccumulator
-emulation (``tests/test_user_knn_gpu.py``).  ``score_batch`` aggregates many queries in one launch.
+does (``user.py:112-155``, SciPy on the host: it is the model, not a hot path).  Scoring a query is two
+device steps:
+
+(i) the neighbour search ``user_vectors @ ratings`` with the self-exclusion and the ``min_sim`` mask
+(``user.py:189-214``): ``lk_uknn_search`` (``knn_user.cu``) gathers, for each of the query's items, the
+item's column of the f64 user vectors and accumulates the similarities in f64 in ascending item order,
+an unfused multiply and add per step — SciPy's own order and rounding, so the neighbour set and the f32
+weights are the reference's bit for bit.  Known users' queries are their rows of the user vectors on the
+device; provided histories are built on the host with the reference's rules (unknown items dropped, a
+repeated item keeps its last value, explicit ratings centred by their f32 mean, implicit 1.0).
+
+(ii) the neighbourhood aggregation of ``_accel.knn.user_score_items_{explicit,implicit}``
+(``src/accel/knn/user_score.rs:21-98``): the accumulator kernel of ``knn_score.cu`` in user mode —
+weights from the neighbour list, values from the rating matrix — bit-exact against the oracle's
+ScoreAccumulator emulation (``tests/test_user_knn_gpu.py``).
+
+``score_batch`` runs each step once for many queries, and the neighbour lists pass from (i) to (ii)
+without leaving the device.  Both device states are built on first use and are not pickled.
 """
 
 from __future__ import annotations
@@ -99,79 +110,72 @@ class UserKNNScorer(Component, Trainable):
             self.__dict__["_state"] = st
         return st
 
+    def _neighbour_state(self) -> engine.UserNeighbourState:
+        ns = self.__dict__.get("_nbr_state")
+        if ns is None:
+            ns = engine.UserNeighbourState.create(self.user_vectors, _lib.require_device())
+            self.__dict__["_nbr_state"] = ns
+        return ns
+
     def __getstate__(self):
         d = dict(self.__dict__)
         d.pop("_state", None)
+        d.pop("_nbr_state", None)
         return d
 
-    def _user_data(self, query: RecQuery):
-        """``_get_user_data`` (user.py:257-300): (user index or None, dense rating vector, user mean) or None."""
+    def _query(self, query: RecQuery):
+        """``_get_user_data`` (user.py:257-300) as a neighbour-search query: (query, user mean) or None, where the
+        query is the user's number (its row of the user vectors) or ``(items, values, self)`` for a history."""
         index = self.users.number(query.user_id, missing=None) if query.user_id is not None else None
         if query.query_items is None:
             if index is None:
                 return None
-            row = self.user_vectors[[int(index)], :].toarray()[0, :]
             umean = float(self.user_means[index]) if self.config.explicit else 0.0
-            return int(index), row, umean
+            return int(index), umean
         if len(query.query_items) == 0:
             return None
-        ratings = np.zeros(len(self.items), dtype=np.float32)
         ui_nos = query.query_items.numbers(vocabulary=self.items, missing="negative")
-        ui_mask = ui_nos >= 0
+        urv = None
         if self.config.explicit:
             urv = query.query_items.field("rating")
             if urv is None:
                 return None
-            urv = np.require(urv, dtype=np.float32)
-            umean = float(urv.mean())
-            ratings[ui_nos[ui_mask]] = urv[ui_mask] - umean
-        else:
-            umean = 0.0
-            ratings[ui_nos[ui_mask]] = 1.0
-        return index, ratings, umean
-
-    def _neighbours(self, query: RecQuery):
-        """The neighbour list of a query (user.py:189-214): (neighbour rows int32, similarities f32, mean) or None."""
-        ud = self._user_data(query)
-        if ud is None:
-            return None
-        uidx, ratings, umean = ud
-        nbr_sims = self.user_vectors @ ratings
-        if uidx is not None:
-            nbr_sims[uidx] = 0  # zero out the self-similarity
-        mask = nbr_sims >= self.config.min_sim
-        if not mask.any():
-            return None
-        return np.flatnonzero(mask).astype(np.int32), nbr_sims[mask].astype(np.float32), umean
+        items, vals, umean = engine.history_query(ui_nos, urv)
+        return (items, vals, None if index is None else int(index)), umean
 
     def score_batch(self, queries: list, targets: list[ItemList]) -> list[ItemList]:
-        """``__call__`` for many queries: the neighbourhood aggregation of all of them in one device launch."""
+        """``__call__`` for many queries: one neighbour search and one neighbourhood aggregation on the device for
+        all of them; the neighbour lists go from the search to the aggregation without leaving the device."""
         st = self._device_state()
         dev = st.sim_cols.device
-        r_ptr, t_ptr = [0], [0]
-        nbrs, sims, tgts, metas = [], [], [], []
-        for q, items in zip(queries, targets):
-            q = RecQuery.create(q)
-            nb = self._neighbours(q) if len(items) > 0 else None
-            iidx = items.numbers(vocabulary=self.items, missing="negative").astype(np.int32)
-            if nb is None:
-                metas.append(None)
-                r_ptr.append(r_ptr[-1])
-                t_ptr.append(t_ptr[-1])
-                continue
-            ki = iidx >= 0
-            nbrs.append(nb[0])
-            sims.append(nb[1])
-            tgts.append(iidx[ki])  # only known items are passed down (user.py:218-221)
-            metas.append((ki, nb[2]))
-            r_ptr.append(r_ptr[-1] + len(nb[0]))
-            t_ptr.append(t_ptr[-1] + int(ki.sum()))
-        cat = lambda xs, dt: torch.from_numpy(np.concatenate(xs).astype(dt) if xs else np.zeros(0, dt)).to(dev)  # noqa: E731
+        specs, at, means = [], [], []
+        for i, (q, items) in enumerate(zip(queries, targets)):
+            qd = self._query(RecQuery.create(q)) if len(items) > 0 else None
+            if qd is not None:
+                specs.append(qd[0])
+                at.append(i)
+                means.append(qd[1])
+        metas = [None] * len(targets)
+        t_ptr, tgts = [0], []
+        nb_indptr = None
+        if specs:
+            ns = self._neighbour_state()
+            nb_indptr, nb_rows, nb_sims = ns.neighbours(ns.queries(specs), self.config.min_sim)
+            n_nbrs = np.diff(nb_indptr.cpu().numpy())
+            for j, i in enumerate(at):
+                if n_nbrs[j] == 0:  # no neighbour: every score is null
+                    t_ptr.append(t_ptr[-1])
+                    continue
+                iidx = targets[i].numbers(vocabulary=self.items, missing="negative").astype(np.int32)
+                ki = iidx >= 0
+                tgts.append(iidx[ki])  # only known items are passed down (user.py:218-221)
+                metas[i] = (ki, means[j], j)
+                t_ptr.append(t_ptr[-1] + int(ki.sum()))
         sc = np.zeros(0, np.float32)
         if t_ptr[-1] > 0:
             scores, _counts = st.score(
-                torch.tensor(r_ptr, dtype=torch.int64, device=dev), cat(nbrs, np.int32), cat(sims, np.float32),
-                torch.tensor(t_ptr, dtype=torch.int64, device=dev), cat(tgts, np.int32),
+                nb_indptr, nb_rows, nb_sims, torch.tensor(t_ptr, dtype=torch.int64, device=dev),
+                torch.from_numpy(np.concatenate(tgts).astype(np.int32)).to(dev),
                 self.config.max_nbrs, self.config.min_nbrs,
             )  # fmt: skip
             sc = scores.cpu().numpy()
@@ -180,9 +184,9 @@ class UserKNNScorer(Component, Trainable):
             if metas[i] is None:
                 out.append(ItemList(items, scores=np.nan))
                 continue
-            ki, umean = metas[i]
+            ki, umean, j = metas[i]
             full = np.full(len(items), np.nan, dtype=np.float32)
-            full[ki] = sc[t_ptr[i] : t_ptr[i + 1]] + np.float32(umean)  # scores += umean (user.py:243-244)
+            full[ki] = sc[t_ptr[j] : t_ptr[j + 1]] + np.float32(umean)  # scores += umean (user.py:243-244)
             out.append(ItemList(items, scores=full))
         return out
 
