@@ -13,6 +13,7 @@
  *   POSV::solve (LAPACK sposv)                    src/accel/als/solve.rs:65-106     in-kernel Cholesky
  *   _accel.knn.compute_similarities               src/accel/knn/item_train.rs:32-93 lk_knn_geometry + lk_knn_build
  *   _accel.knn.score_explicit / score_implicit    src/accel/knn/item_score.rs:22-111 lk_knn_score_batch
+ *   kNN scorer + TopNRanker (topn_pipeline)       src/lenskit/basic/topn.py:32-69   lk_knn_recommend_batch
  *   UserKNNScorer neighbours (SciPy, host)        src/lenskit/knn/user.py:189-214   lk_uknn_search
  *   _accel.data.argtopn (SURVEY.md 8f, "next")    src/accel/data/sorting.rs:131-170 lk_topn_columns
  *
@@ -348,6 +349,35 @@ LK_API int64_t lk_knn_score_warps(void);
 /* number of CTAs of the dense (all-items) scoring grid: one n_items row of d_slotmap each */
 LK_API int64_t lk_knn_score_dense_ctas(void);
 LK_API int lk_knn_score_batch(const lk_knn_score_args *args, void *stream);
+
+/*
+ * Batched top-n recommendation from the kNN scorers (dense mode with ranking, knn_score.cu): for every query,
+ * the reference's composition of TrainingItemsCandidateSelector, the scorer and TopNRanker,
+ *     cands = all items ascending, minus the query's excluded items;  il = scorer(query, cands);
+ *     top   = il[argtopn(il.scores, n)]
+ * with the final score of an item = (accumulator score + d_item_offset[item]) + d_query_offset[q], f32 adds
+ * (NaN stays NaN).  The selection replays argtopn's heap (see lk_topn_columns), so ties are cut and ordered
+ * exactly as there.  `score` is an lk_knn_score_args in dense mode (d_tgt_indptr == d_tgt_items == NULL) with
+ * the same layout rules; its d_scores / d_counts are not used.  Per query q, n entries at q*n:
+ *   d_out_idx   item number of rank t, -1 beyond the count
+ *   d_out_val   its final score, NaN beyond the count
+ *   d_out_nbrs  its accumulator length (the scorer's nbr_counts), 0 beyond the count
+ *   d_out_cnt   [q] = min(n, number of candidates with a non-NaN score)
+ * d_spill: one n_items int32 row per CTA ([lk_knn_score_dense_ctas() * n_items]) for the touched-target list
+ * of a query that touches more targets than the CTA keeps in shared memory; any content on entry.
+ * Statuses as lk_knn_score_batch (2 NaN similarity, 3 pool too small).
+ */
+typedef struct lk_knn_rank_args {
+    int32_t n;                     /* 1..lk_topn_max() */
+    const float *d_item_offset;    /* [n_items] or NULL */
+    const float *d_query_offset;   /* [n_queries] or NULL */
+    const int64_t *d_excl_indptr;  /* [n_queries+1] or NULL: items never recommended to the query */
+    const int32_t *d_excl_items;   /* any order, repeats allowed, negative skipped */
+    int32_t *d_spill;              /* per-CTA touched-target spill rows */
+    int32_t *d_out_idx; float *d_out_val; int32_t *d_out_nbrs; /* [n_queries * n] */
+    int32_t *d_out_cnt;            /* [n_queries] */
+} lk_knn_rank_args;
+LK_API int lk_knn_recommend_batch(const lk_knn_score_args *score, const lk_knn_rank_args *rank, void *stream);
 
 /* ------------------------------------------------------------------------
  * Batched top-N (SURVEY.md §8f N2: the step after the scorer)

@@ -137,6 +137,21 @@ class LkKnnScoreArgs(C.Structure):
     ]
 
 
+class LkKnnRankArgs(C.Structure):
+    _fields_ = [
+        ("n", C.c_int32),
+        ("d_item_offset", vp),
+        ("d_query_offset", vp),
+        ("d_excl_indptr", vp),
+        ("d_excl_items", vp),
+        ("d_spill", vp),
+        ("d_out_idx", vp),
+        ("d_out_val", vp),
+        ("d_out_nbrs", vp),
+        ("d_out_cnt", vp),
+    ]
+
+
 class LkUknnSearchArgs(C.Structure):
     _fields_ = [
         ("geom", LkKnnGeom),
@@ -193,6 +208,7 @@ SYMBOLS: dict[str, tuple] = {
     "lk_knn_score_warps": (C.c_int64, []),
     "lk_knn_score_dense_ctas": (C.c_int64, []),
     "lk_knn_score_batch": (C.c_int, [C.POINTER(LkKnnScoreArgs), vp]),
+    "lk_knn_recommend_batch": (C.c_int, [C.POINTER(LkKnnScoreArgs), C.POINTER(LkKnnRankArgs), vp]),
     "lk_topn_max": (C.c_int, []),
     "lk_topn_columns": (C.c_int, [vp, C.c_int64, C.c_int64, C.c_int64, C.c_int32, vp, vp, vp, vp]),
 }

@@ -24,7 +24,8 @@
 //     per-warp `slotmap` (n_items ints, kept at -1 between queries) maps item ->
 //     position in the query's target list, so cost is proportional to the
 //     contributions and the target list, never to n_items.
-//   * knn_score_dense_kernel (every query against all items): one CTA per query.
+//   * knn_score_dense_kernel (every query against all items): one CTA per query.  Its ranking mode
+//     (lk_knn_recommend_batch) replaces the full output rows by each query's top n, selected in the kernel.
 
 #include <algorithm>
 
@@ -382,6 +383,8 @@ __global__ void __launch_bounds__(256) knn_score_lists_kernel(lk_knn_score_args 
 //      accumulator (replay_list, as in the list kernel);
 //   5. one coalesced pass writes the score and count rows — the result where the slot map has an entry,
 //      NaN / 0 elsewhere — and clears the slot map for the next query.
+// Ranking mode (RANK, lk_knn_recommend_batch) keeps steps 1-4 and replaces step 5 by rank_query below: the
+// query's top n of its final scores, written as n entries instead of two n_items rows.
 // (Round-2 v2 counted on the output row itself and kept [n_queries x n_items] offset / cursor rows: 2.1 MB
 // of DRAM traffic per ML-25M-shaped query, twice its output, L2 hit rate 28 %.)
 // ---------------------------------------------------------------------------------------------
@@ -411,7 +414,193 @@ __device__ __forceinline__ int block_excl_scan(int v, int *s_scan, int *s_carry,
     return carry + woff + incl - v;
 }
 
-__global__ void __launch_bounds__(DENSE_THREADS) knn_score_dense_kernel(lk_knn_score_args a)
+// ---------------------------------------------------------------------------------------------
+// Ranking mode.  For every query the result must be the reference's per-query composition
+//     cands = all items ascending, minus the excluded ones;  il = scorer(query, cands);  il[argtopn(il.scores, n)]
+// argtopn (sorting.rs:131-170, topn.cu) offers the candidates in index order to an indirect min-heap and returns
+// on a NaN offer before it touches the heap.  So offering EVERY item in ascending item order, with the excluded
+// and the untouched items as NaN, replays the reference's heap move for move; its keys are item numbers.
+//   * the offer order is the item order of the slot-map walk, never the touched list (atomic arrival order);
+//   * the only pre-filter is the heap root once the heap is full: the root never decreases after that and a full
+//     heap rejects s <= root.  A filter against a guessed n-th score would change which equal scores survive;
+//   * the offsets are added in f32 before ranking, as the components add them to the scores on the host.
+// The CTA walks the slot-map row in chunks of RANK_CHUNK items (coalesced, clearing the map as step 5 does),
+// compacts the candidates that pass the filter in item order (ballots and a 64-entry scan) and one thread offers
+// them to the heap with topn.cu's sift rules.  The heap and the candidate buffer live in DenseSmem, which steps
+// 1-3 no longer need at that point, so the ranking mode costs no shared memory of its own.
+// ---------------------------------------------------------------------------------------------
+constexpr int RANK_NMAX = 1024;  // lk_topn_max()
+constexpr int RANK_UNITS = 8;    // items per thread and chunk
+constexpr int RANK_CHUNK = DENSE_THREADS * RANK_UNITS;
+constexpr int RANK_WARPS = DENSE_THREADS / 32;
+
+struct RankSmem {
+    float hv[RANK_NMAX];  // heap: score, item number, accumulator length
+    int32_t hk[RANK_NMAX];
+    int32_t hc[RANK_NMAX];
+    float cv[RANK_CHUNK];  // the chunk's candidates, in item order
+    int32_t ck[RANK_CHUNK];
+    int32_t cc[RANK_CHUNK];
+    int32_t wcnt[RANK_UNITS * RANK_WARPS];  // candidates per (unit, warp); then their exclusive offsets
+    int32_t wofs[RANK_UNITS * RANK_WARPS];
+    int32_t n_cand, count;
+    float root;
+};
+static_assert(sizeof(RankSmem) <= sizeof(DenseSmem), "the ranking state must fit in the dense kernel's shared memory");
+
+// heap.rs:67-89 downheap as topn.cu does it (the smaller child, the left one on a tie, while strictly smaller),
+// moving a hole instead of swapping: the same final arrangement
+__device__ void rank_down(RankSmem &r, int pos, const int lim)
+{
+    const float v = r.hv[pos];
+    const int32_t k = r.hk[pos], c = r.hc[pos];
+    for (;;) {
+        int mn = pos;
+        float mv = v;
+        const int left = 2 * pos + 1, right = 2 * pos + 2;
+        if (left < lim && r.hv[left] < mv) {
+            mn = left;
+            mv = r.hv[left];
+        }
+        if (right < lim && r.hv[right] < mv) mn = right;
+        if (mn == pos) break;
+        r.hv[pos] = r.hv[mn], r.hk[pos] = r.hk[mn], r.hc[pos] = r.hc[mn];
+        pos = mn;
+    }
+    r.hv[pos] = v, r.hk[pos] = k, r.hc[pos] = c;
+}
+
+// topn.cu's offer for a non-NaN score: heap.rs:41-45 push + upheap while not full, else heap.rs:46-52 replace the
+// root if strictly greater and downheap
+__device__ __forceinline__ void rank_offer(RankSmem &r, int &count, float &root, const int n, const float s,
+                                           const int32_t k, const int32_t c)
+{
+    if (count < n) {
+        int pos = count++;
+        while (pos > 0) {
+            const int parent = (pos - 1) / 2;
+            if (!(r.hv[parent] > s)) break;
+            r.hv[pos] = r.hv[parent], r.hk[pos] = r.hk[parent], r.hc[pos] = r.hc[parent];
+            pos = parent;
+        }
+        r.hv[pos] = s, r.hk[pos] = k, r.hc[pos] = c;
+        root = r.hv[0];
+    } else if (s > root) {
+        r.hv[0] = s, r.hk[0] = k, r.hc[0] = c;
+        rank_down(r, 0, n);
+        root = r.hv[0];
+    }
+}
+
+// Ranking mode's step 5 for query q (the whole CTA; steps 1-4 done, DenseSmem free): exclusion, the ranking walk,
+// the heap sort and the n output entries.  Leaves the slot map at zero.
+__device__ void rank_query(RankSmem &r, const lk_knn_rank_args &rk, const int q, int32_t *slot, int32_t *offs,
+                           const int32_t *curs, const int64_t NI, const int n_active, const int tid, const int lane,
+                           const int warp)
+{
+    const float qnan = __int_as_float(0x7fc00000);
+    const int n = rk.n;
+    // items never recommended to the query: their touched target's score becomes NaN
+    if (rk.d_excl_indptr != nullptr) {
+        const int64_t e1 = rk.d_excl_indptr[q + 1];
+        for (int64_t p = rk.d_excl_indptr[q] + tid; p < e1; p += DENSE_THREADS) {
+            const int e = rk.d_excl_items[p];
+            if (e >= 0 && e < NI) {
+                const int sl = __ldcg(&slot[e]);
+                if (sl != 0) __stcg(&offs[sl - 1], __float_as_int(qnan));
+            }
+        }
+    }
+    if (tid == 0) r.count = 0;
+    __threadfence_block();
+    __syncthreads();
+    const float qoff = rk.d_query_offset != nullptr ? rk.d_query_offset[q] : 0.0f;
+    const unsigned lanes_below = (1u << lane) - 1u;
+    // no touched target: every score is NaN and the slot map is already clean
+    for (int64_t x0 = 0; n_active > 0 && x0 < NI; x0 += RANK_CHUNK) {
+        const int count0 = r.count;  // the heap as the previous chunk left it
+        const float root0 = r.root;
+        int sl[RANK_UNITS];
+#pragma unroll
+        for (int u = 0; u < RANK_UNITS; u++) {
+            const int64_t x = x0 + u * DENSE_THREADS + tid;
+            sl[u] = x < NI ? __ldcg(&slot[x]) : 0;
+        }
+        float sv[RANK_UNITS];
+        int32_t sc[RANK_UNITS];
+        unsigned pass[RANK_UNITS];
+#pragma unroll
+        for (int u = 0; u < RANK_UNITS; u++) {
+            const int64_t x = x0 + u * DENSE_THREADS + tid;
+            float s = qnan;
+            sc[u] = 0;
+            if (sl[u] != 0) {
+                s = __int_as_float(__ldcg(&offs[sl[u] - 1]));
+                sc[u] = __ldcg(&curs[sl[u] - 1]);
+                __stcg(&slot[x], 0);
+                if (rk.d_item_offset != nullptr) s = __fadd_rn(s, rk.d_item_offset[x]);
+                if (rk.d_query_offset != nullptr) s = __fadd_rn(s, qoff);
+            }
+            sv[u] = s;
+            pass[u] = __ballot_sync(FULL, s == s && (count0 < n || s > root0));
+        }
+        if (lane == 0)
+#pragma unroll
+            for (int u = 0; u < RANK_UNITS; u++) r.wcnt[u * RANK_WARPS + warp] = __popc(pass[u]);
+        __syncthreads();
+        static_assert(RANK_UNITS * RANK_WARPS == 64, "one warp scans the (unit, warp) counts two per lane");
+        if (warp == 0) {
+            const int c0 = r.wcnt[2 * lane], c1 = r.wcnt[2 * lane + 1];
+            const int incl = warp_incl_scan(c0 + c1, lane);
+            r.wofs[2 * lane] = incl - c0 - c1;
+            r.wofs[2 * lane + 1] = incl - c1;
+            if (lane == 31) r.n_cand = incl;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int u = 0; u < RANK_UNITS; u++) {
+            if (pass[u] >> lane & 1u) {
+                const int p = r.wofs[u * RANK_WARPS + warp] + __popc(pass[u] & lanes_below);
+                r.cv[p] = sv[u];
+                r.ck[p] = (int32_t)(x0 + u * DENSE_THREADS + tid);
+                r.cc[p] = sc[u];
+            }
+        }
+        __syncthreads();
+        if (tid == 0 && r.n_cand > 0) {
+            int count = count0;
+            float root = root0;
+            const int nc = r.n_cand;
+            for (int i = 0; i < nc; i++) rank_offer(r, count, root, n, r.cv[i], r.ck[i], r.cc[i]);
+            r.count = count;
+            r.root = root;
+        }
+        __syncthreads();
+    }
+    // heap.rs:56-65 topn_vec: heap sort into descending score order
+    const int count = r.count;
+    if (tid == 0) {
+        for (int m = count - 1; m > 0; m--) {
+            const float tv = r.hv[0];
+            const int32_t tk = r.hk[0], tc = r.hc[0];
+            r.hv[0] = r.hv[m], r.hk[0] = r.hk[m], r.hc[0] = r.hc[m];
+            r.hv[m] = tv, r.hk[m] = tk, r.hc[m] = tc;
+            rank_down(r, 0, m);
+        }
+    }
+    __syncthreads();
+    const int64_t o = (int64_t)q * n;
+    for (int t = tid; t < n; t += DENSE_THREADS) {
+        const bool in = t < count;
+        rk.d_out_idx[o + t] = in ? r.hk[t] : -1;
+        rk.d_out_val[o + t] = in ? r.hv[t] : qnan;
+        rk.d_out_nbrs[o + t] = in ? r.hc[t] : 0;
+    }
+    if (tid == 0) rk.d_out_cnt[q] = count;
+}
+
+template <bool RANK>
+__global__ void __launch_bounds__(DENSE_THREADS) knn_score_dense_kernel(lk_knn_score_args a, lk_knn_rank_args rk)
 {
     extern __shared__ __align__(16) unsigned char dense_raw[];
     DenseSmem &sm = *reinterpret_cast<DenseSmem *>(dense_raw);
@@ -441,10 +630,12 @@ __global__ void __launch_bounds__(DENSE_THREADS) knn_score_dense_kernel(lk_knn_s
         if (s_q >= a.n_queries) break;
         const int q = s_q;
         const int64_t r0 = a.d_ref_indptr[q], r1 = a.d_ref_indptr[q + 1];
-        float *scores = a.d_scores + (int64_t)q * NI;
-        int32_t *counts = a.d_counts + (int64_t)q * NI;
-        // the query's count row is not written before step 5: until then it holds the tail of the touched list
-        auto active_at = [&](int i) { return i < DENSE_ACTIVE_CAP ? sm.active[i] : __ldcg(&counts[i - DENSE_ACTIVE_CAP]); };
+        float *scores = RANK ? nullptr : a.d_scores + (int64_t)q * NI;
+        int32_t *counts = RANK ? nullptr : a.d_counts + (int64_t)q * NI;
+        // the tail of the touched list: the query's count row, not written before step 5; in ranking mode, which
+        // has no such row, the CTA's own spill row
+        int32_t *spill = RANK ? rk.d_spill + (size_t)blockIdx.x * NI : counts;
+        auto active_at = [&](int i) { return i < DENSE_ACTIVE_CAP ? sm.active[i] : __ldcg(&spill[i - DENSE_ACTIVE_CAP]); };
 
         // walk over the contributions of the query, flattened over the block:
         // fn(lo, tcol, mval, pos0) gets four contributions per thread and step — lo[u] = history entry inside
@@ -520,7 +711,7 @@ __global__ void __launch_bounds__(DENSE_THREADS) knn_score_dense_kernel(lk_knn_s
             for (int u = 0; u < CU; u++) {
                 if (old[u] == 0) {  // first touch of this target
                     const int idx = atomicAdd(&s_nactive, 1);
-                    if (idx < DENSE_ACTIVE_CAP) sm.active[idx] = tcol[u]; else __stcg(&counts[idx - DENSE_ACTIVE_CAP], tcol[u]);
+                    if (idx < DENSE_ACTIVE_CAP) sm.active[idx] = tcol[u]; else __stcg(&spill[idx - DENSE_ACTIVE_CAP], tcol[u]);
                 }
             }
         });
@@ -606,6 +797,13 @@ __global__ void __launch_bounds__(DENSE_THREADS) knn_score_dense_kernel(lk_knn_s
         __threadfence_block();
         __syncthreads();
 
+        if constexpr (RANK) {
+            // q and n_active re-read from shared memory: kept in registers across step 4 they cost a spill
+            rank_query(*reinterpret_cast<RankSmem *>(dense_raw), rk, s_q, slot, offs, curs, NI, s_nactive, tid, lane,
+                       warp);
+            __syncthreads();
+            continue;
+        }
         // 5. the output rows, once, coalesced; the slot map goes back to zero
         constexpr int FU = 8;
         for (int64_t x0 = tid; x0 < NI; x0 += DENSE_THREADS * FU) {
@@ -646,52 +844,92 @@ int64_t lk_knn_score_warps(void) { return (int64_t)sm_count() * SCORE_WARPS_PER_
 
 int64_t lk_knn_score_dense_ctas(void) { return (int64_t)sm_count() * 3; }
 
-int lk_knn_score_batch(const lk_knn_score_args *args, void *stream)
+}  // extern "C"
+
+// The checks lk_knn_score_batch and lk_knn_recommend_batch share.  `outputs`: d_scores / d_counts are required.
+static int check_score_args(const lk_knn_score_args &a, const char *who, const bool outputs)
 {
-    LK_REQUIRE(args != nullptr, LK_ERR_INVALID, "lk_knn_score_batch: null args");
-    const lk_knn_score_args &a = *args;
     LK_REQUIRE(a.n_items >= 1 && a.n_queries >= 0, LK_ERR_INVALID, "bad shape");
     LK_REQUIRE(a.max_nbrs >= 1 && a.max_nbrs <= SCORE_MAX_NBRS, LK_ERR_UNSUPPORTED,
                "max_nbrs must be in 1..%d", SCORE_MAX_NBRS);
     const bool dense = a.d_tgt_items == nullptr && a.d_tgt_indptr == nullptr;  // every query against all items
     LK_REQUIRE(a.d_sim_indptr && a.d_sim_cols && a.d_ref_indptr && a.d_ref_items && a.d_list_off && a.d_list_cur &&
-                   a.d_scores && a.d_counts && a.d_work_counter && a.d_status,
-               LK_ERR_INVALID, "lk_knn_score_batch: null pointer");
+                   (!outputs || (a.d_scores && a.d_counts)) && a.d_work_counter && a.d_status,
+               LK_ERR_INVALID, "%s: null pointer", who);
     LK_REQUIRE(a.d_pool && a.d_pool_cursor, LK_ERR_INVALID,
-               "lk_knn_score_batch: the contribution pool (d_pool, d_pool_cursor) is required");
+               "%s: the contribution pool (d_pool, d_pool_cursor) is required", who);
     LK_REQUIRE(reinterpret_cast<uintptr_t>(a.d_pool) % 16 == 0 && a.pool_entries >= 0, LK_ERR_INVALID,
-               "lk_knn_score_batch: bad contribution pool");
+               "%s: bad contribution pool", who);
     LK_REQUIRE(dense || (a.d_tgt_indptr && a.d_tgt_items && a.d_slotmap && a.d_list_cnt), LK_ERR_INVALID,
-               "lk_knn_score_batch: null pointer (target lists)");
+               "%s: null pointer (target lists)", who);
     LK_REQUIRE(!dense || (a.d_slotmap && a.slotmap_warps >= lk_knn_score_dense_ctas()), LK_ERR_INVALID,
-               "lk_knn_score_batch: the dense (all-items) mode needs one n_items row of d_slotmap per CTA "
-               "(lk_knn_score_dense_ctas)");
+               "%s: the dense (all-items) mode needs one n_items row of d_slotmap per CTA "
+               "(lk_knn_score_dense_ctas)", who);
     LK_REQUIRE(a.user_mode ? a.d_ref_vals != nullptr : a.d_sim_vals != nullptr, LK_ERR_INVALID,
-               "lk_knn_score_batch: the weights (similarities) are missing");
+               "%s: the weights (similarities) are missing", who);
     LK_REQUIRE(dense || a.slotmap_warps >= 1, LK_ERR_INVALID, "slotmap too small");
+    return LK_OK;
+}
+
+template <bool RANK>
+static int launch_dense(const lk_knn_score_args &a, const lk_knn_rank_args &rk, cudaStream_t st)
+{
+    // the per-CTA slot maps (n_items ints each) should stay in L2 next to the similarity matrix: two CTAs
+    // per SM instead of three when three rows per SM would take more than half of it
+    const Options &opt = options();
+    int per_sm = ((int64_t)sm_count() * 3 * a.n_items * 4 > (int64_t)(64 << 20)) ? 2 : 3;
+    if (opt.knn_score_ctas > 0) per_sm = std::min(3, opt.knn_score_ctas);
+    const int grid = (int)std::min<int64_t>(a.n_queries, (int64_t)sm_count() * per_sm);
+    const int smem = (int)sizeof(DenseSmem);
+    LK_CUDA_TRY(
+        cudaFuncSetAttribute(knn_score_dense_kernel<RANK>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    knn_score_dense_kernel<RANK><<<grid, DENSE_THREADS, smem, st>>>(a, rk);
+    LK_CUDA_TRY(cudaGetLastError());
+    return LK_OK;
+}
+
+extern "C" {
+
+int lk_knn_score_batch(const lk_knn_score_args *args, void *stream)
+{
+    LK_REQUIRE(args != nullptr, LK_ERR_INVALID, "lk_knn_score_batch: null args");
+    const lk_knn_score_args &a = *args;
+    const int rc = check_score_args(a, "lk_knn_score_batch", true);
+    if (rc != LK_OK) return rc;
+    const bool dense = a.d_tgt_items == nullptr && a.d_tgt_indptr == nullptr;
     if (a.n_queries == 0) return LK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     LK_CUDA_TRY(cudaMemsetAsync(a.d_work_counter, 0, sizeof(int32_t), st));
     LK_CUDA_TRY(cudaMemsetAsync(a.d_pool_cursor, 0, sizeof(unsigned long long), st));
-    if (dense) {
-        // the per-CTA slot maps (n_items ints each) should stay in L2 next to the similarity matrix: two CTAs
-        // per SM instead of three when three rows per SM would take more than half of it
-        const Options &opt = options();
-        int per_sm = ((int64_t)sm_count() * 3 * a.n_items * 4 > (int64_t)(64 << 20)) ? 2 : 3;
-        if (opt.knn_score_ctas > 0) per_sm = std::min(3, opt.knn_score_ctas);
-        const int grid = (int)std::min<int64_t>(a.n_queries, (int64_t)sm_count() * per_sm);
-        const int smem = (int)sizeof(DenseSmem);
-        LK_CUDA_TRY(cudaFuncSetAttribute(knn_score_dense_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        knn_score_dense_kernel<<<grid, DENSE_THREADS, smem, st>>>(a);
-        LK_CUDA_TRY(cudaGetLastError());
-        return LK_OK;
-    }
+    if (dense) return launch_dense<false>(a, lk_knn_rank_args{}, st);
     // as many warps as there are slot-map rows (the caller sizes them to the batch), at most the full grid
     const int64_t warps = std::min<int64_t>(a.slotmap_warps, lk_knn_score_warps());
     const int blocks = (int)((warps + 7) / 8);
     knn_score_lists_kernel<<<blocks, 256, 0, st>>>(a);
     LK_CUDA_TRY(cudaGetLastError());
     return LK_OK;
+}
+
+int lk_knn_recommend_batch(const lk_knn_score_args *score, const lk_knn_rank_args *rank, void *stream)
+{
+    LK_REQUIRE(score != nullptr && rank != nullptr, LK_ERR_INVALID, "lk_knn_recommend_batch: null args");
+    const lk_knn_score_args &a = *score;
+    const lk_knn_rank_args &rk = *rank;
+    const int rc = check_score_args(a, "lk_knn_recommend_batch", false);
+    if (rc != LK_OK) return rc;
+    LK_REQUIRE(a.d_tgt_items == nullptr && a.d_tgt_indptr == nullptr, LK_ERR_INVALID,
+               "lk_knn_recommend_batch: ranks all items (dense mode: d_tgt_indptr and d_tgt_items must be NULL)");
+    LK_REQUIRE(rk.n >= 1 && rk.n <= RANK_NMAX && rk.n <= lk_topn_max(), LK_ERR_UNSUPPORTED,
+               "lk_knn_recommend_batch: n must be in 1..%d", lk_topn_max());
+    LK_REQUIRE(rk.d_spill && rk.d_out_idx && rk.d_out_val && rk.d_out_nbrs && rk.d_out_cnt, LK_ERR_INVALID,
+               "lk_knn_recommend_batch: null pointer (spill rows or outputs)");
+    LK_REQUIRE(rk.d_excl_indptr == nullptr || rk.d_excl_items != nullptr, LK_ERR_INVALID,
+               "lk_knn_recommend_batch: d_excl_items is required with d_excl_indptr");
+    if (a.n_queries == 0) return LK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    LK_CUDA_TRY(cudaMemsetAsync(a.d_work_counter, 0, sizeof(int32_t), st));
+    LK_CUDA_TRY(cudaMemsetAsync(a.d_pool_cursor, 0, sizeof(unsigned long long), st));
+    return launch_dense<true>(a, rk, st);
 }
 
 }  // extern "C"

@@ -16,7 +16,9 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import LkAlsArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnScoreArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr
+from ._lib import (
+    LkAlsArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr,
+)  # fmt: skip
 from .data import InteractionCSR
 
 DEFAULT_CHUNK_NNZ = 4096
@@ -526,6 +528,8 @@ class KnnScorerState:
         total = int(((self.sim_indptr[rr + 1] - self.sim_indptr[rr]) * ok).sum().item())
         pool = self.scratch.get("pool")
         if pool is None or pool.numel() < 4 * max(total, 1):
+            # the old pool goes first: user-mode pools of a few hundred queries take tens of GB
+            pool = self.scratch["pool"] = None
             pool = torch.empty(4 * max(total, 1), dtype=torch.int32, device=dev)
             self.scratch["pool"] = pool
             self.scratch["pool_cursor"] = torch.zeros(1, dtype=torch.int64, device=dev)
@@ -539,36 +543,101 @@ class KnnScorerState:
         with NaN nulls, counts [n_queries, n_items]).  Runs ``knn_score_dense_kernel`` — a CTA per query,
         cost proportional to the contributions plus one streaming fill of the output.
         """
-
-        def per_cta_rows(a: LkKnnScoreArgs) -> None:
-            ctas = int(lib().lk_knn_score_dense_ctas())
-            # per-CTA state of the dense kernel: a slot map (item -> touched-target number; zero between queries
-            # and between launches) and two compact rows indexed by touched-target number
-            rows = self.scratch.get("dense")
-            if rows is None:
-                dev, n = self.sim_cols.device, ctas * self.n_items
-                rows = self.scratch["dense"] = (
-                    torch.empty(n, dtype=torch.int32, device=dev), torch.empty(n, dtype=torch.int32, device=dev),
-                    torch.zeros(n, dtype=torch.int32, device=dev),
-                )  # fmt: skip
-            off, cur, slotmap = rows
-            a.d_list_off, a.d_list_cur = ptr(off), ptr(cur)
-            a.d_slotmap, a.slotmap_warps = ptr(slotmap), ctas
-
         shape = (ref_indptr.numel() - 1, self.n_items)
-        return self._launch(shape, ref_indptr, ref_items, ref_vals, max_nbrs, min_nbrs, per_cta_rows)
+        return self._launch(shape, ref_indptr, ref_items, ref_vals, max_nbrs, min_nbrs, self._per_cta_rows)
+
+    def _per_cta_rows(self, a: LkKnnScoreArgs) -> None:
+        """The dense kernel's per-CTA state: a slot map (item -> touched-target number; zero between queries and
+        between launches) and two compact rows indexed by touched-target number."""
+        ctas = int(lib().lk_knn_score_dense_ctas())
+        rows = self.scratch.get("dense")
+        if rows is None:
+            dev, n = self.sim_cols.device, ctas * self.n_items
+            rows = self.scratch["dense"] = (
+                torch.empty(n, dtype=torch.int32, device=dev), torch.empty(n, dtype=torch.int32, device=dev),
+                torch.zeros(n, dtype=torch.int32, device=dev),
+            )  # fmt: skip
+        off, cur, slotmap = rows
+        a.d_list_off, a.d_list_cur = ptr(off), ptr(cur)
+        a.d_slotmap, a.slotmap_warps = ptr(slotmap), ctas
+
+    def recommend(
+        self,
+        ref_indptr: torch.Tensor,
+        ref_items: torch.Tensor,
+        ref_vals: torch.Tensor | None,
+        max_nbrs: int,
+        min_nbrs: int,
+        n: int,
+        item_offset: torch.Tensor | None = None,
+        query_offset: torch.Tensor | None = None,
+        excl_indptr: torch.Tensor | None = None,
+        excl_items: torch.Tensor | None = None,
+    ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+        """
+        Top-``n`` of every query over ALL items, scored and selected in one launch (``lk_knn_recommend_batch``,
+        the dense kernel's ranking mode): the final score of item i for query q is
+        ``(score + item_offset[i]) + query_offset[q]`` (f32), the items ``excl_items[excl_indptr[q]:excl_indptr[q+1]]``
+        are never recommended to q, and the selection is ``argtopn``'s, ties included.  Returns
+        ``(idx [B, n] int32 item numbers, -1 padding; val [B, n] f32, NaN padding; nbrs [B, n] int32 accumulator
+        lengths, 0 padding; cnt [B] int32)``.
+        """
+        _check_max_nbrs(max_nbrs)
+        n_max = int(lib().lk_topn_max())
+        if not 1 <= int(n) <= n_max:
+            raise ValueError(f"n must be in 1..{n_max}")
+        n = int(n)
+        dev = self.sim_cols.device
+        B = ref_indptr.numel() - 1
+        idx = torch.empty((B, n), dtype=torch.int32, device=dev)
+        val = torch.empty((B, n), dtype=torch.float32, device=dev)
+        nbrs = torch.empty((B, n), dtype=torch.int32, device=dev)
+        cnt = torch.empty(max(B, 1), dtype=torch.int32, device=dev)
+        if excl_items is not None and excl_items.numel() == 0:  # NULL address; never read (bounded by the indptr)
+            excl_items = torch.full((1,), -1, dtype=torch.int32, device=dev)
+
+        def launch(a: LkKnnScoreArgs) -> None:
+            self._per_cta_rows(a)
+            spill = self.scratch.get("spill")
+            if spill is None:  # the touched-target tail of a query past the CTA's shared-memory list
+                spill = torch.empty(int(lib().lk_knn_score_dense_ctas()) * self.n_items, dtype=torch.int32, device=dev)
+                self.scratch["spill"] = spill
+            r = LkKnnRankArgs()
+            r.n = n
+            r.d_item_offset, r.d_query_offset = ptr(item_offset), ptr(query_offset)
+            r.d_excl_indptr, r.d_excl_items = ptr(excl_indptr), ptr(excl_items)
+            r.d_spill = ptr(spill)
+            r.d_out_idx, r.d_out_val, r.d_out_nbrs, r.d_out_cnt = ptr(idx), ptr(val), ptr(nbrs), ptr(cnt)
+            check(lib().lk_knn_recommend_batch(C.byref(a), C.byref(r), stream_ptr()), "lk_knn_recommend_batch")
+
+        if B > 0:
+            self._run(ref_indptr, ref_items, ref_vals, max_nbrs, min_nbrs, launch, "lk_knn_recommend_batch")
+        return idx, val, nbrs, cnt[:B]
 
     def _launch(self, out_shape, ref_indptr, ref_items, ref_vals, max_nbrs, min_nbrs, fill_mode):
-        """What both modes share: the ``max_nbrs`` check, the outputs, the common ``lk_knn_score_args`` fields, the
-        launch, the wait and the status word.  ``fill_mode(args)`` sets the mode's own fields (with the lock held;
-        the scratch they point to must outlive this call)."""
-        if not 1 <= int(max_nbrs) <= KNN_SCORE_MAX_NBRS:
-            raise ValueError(f"max_nbrs must be in 1..{KNN_SCORE_MAX_NBRS}")
+        """``score`` and ``score_all_items``: the outputs and ``lk_knn_score_batch`` around :meth:`_run`.
+        ``fill_mode(args)`` sets the mode's own fields (with the lock held; the scratch they point to must outlive
+        this call)."""
+        _check_max_nbrs(max_nbrs)
         dev = self.sim_cols.device
         scores = torch.empty(out_shape, dtype=torch.float32, device=dev)
         counts = torch.empty(out_shape, dtype=torch.int32, device=dev)
         if scores.numel() == 0:  # no targets (or no queries): nothing to score
             return scores, counts
+
+        def launch(a: LkKnnScoreArgs) -> None:
+            fill_mode(a)
+            a.d_scores, a.d_counts = ptr(scores), ptr(counts)
+            check(lib().lk_knn_score_batch(C.byref(a), stream_ptr()), "lk_knn_score_batch")
+
+        self._run(ref_indptr, ref_items, ref_vals, max_nbrs, min_nbrs, launch, "lk_knn_score_batch")
+        return scores, counts
+
+    def _run(self, ref_indptr, ref_items, ref_vals, max_nbrs, min_nbrs, launch, what: str) -> None:
+        """What every launch shares: the empty-history placeholder, the common ``lk_knn_score_args`` fields, the
+        lock, the wait and the status word.  ``launch(args)`` completes the arguments and calls the entry point
+        ``what`` (with the lock held)."""
+        dev = self.sim_cols.device
         if ref_items.numel() == 0:
             # every history is empty: the address of an empty tensor is NULL, which the library rejects; the
             # kernels never read these placeholders because the indptr bounds every read
@@ -576,26 +645,28 @@ class KnnScorerState:
             ref_vals = None if ref_vals is None else torch.zeros(1, dtype=torch.float32, device=dev)
         with self.lock:  # status word, work counter, pool and slot maps are shared by the callers of one state
             a = LkKnnScoreArgs()
-            fill_mode(a)
             pool, cursor = self._pool_for(ref_items)
             a.n_items = self.n_items
             a.d_sim_indptr, a.d_sim_cols, a.d_sim_vals = ptr(self.sim_indptr), ptr(self.sim_cols), ptr(self.sim_vals)
             a.n_queries = ref_indptr.numel() - 1
             a.d_ref_indptr, a.d_ref_items, a.d_ref_vals = ptr(ref_indptr), ptr(ref_items), ptr(ref_vals)
             a.max_nbrs, a.min_nbrs = int(max_nbrs), int(min_nbrs)
-            a.d_scores, a.d_counts = ptr(scores), ptr(counts)
             a.d_work_counter, a.d_status = ptr(self.work_counter), ptr(self.status)
             a.user_mode, a.n_matrix_rows = (1 if self.user_mode else 0), self.n_rows
             a.d_pool, a.pool_entries, a.d_pool_cursor = ptr(pool), pool.numel() // 4, ptr(cursor)
             self.status.zero_()
-            check(lib().lk_knn_score_batch(C.byref(a), stream_ptr()), "lk_knn_score_batch")
+            launch(a)
             torch.cuda.current_stream().synchronize()
             st = int(self.status.item())
         if st == 2:
             raise ValueError("similarity is null")
         if st == 3:
-            raise _lib.EngineError("lk_knn_score_batch: contribution pool too small")
-        return scores, counts
+            raise _lib.EngineError(f"{what}: contribution pool too small")
+
+
+def _check_max_nbrs(max_nbrs: int) -> None:
+    if not 1 <= int(max_nbrs) <= KNN_SCORE_MAX_NBRS:
+        raise ValueError(f"max_nbrs must be in 1..{KNN_SCORE_MAX_NBRS}")
 
 
 # ---------------------------------------------------------------------------

@@ -7,7 +7,9 @@ Same config fields / aliases (``max_nbrs``/``nnbrs``/``k``, ``min_nbrs``,
 ``block_size``), same trained attributes (``items``, ``item_means``,
 ``item_counts``, ``sim_matrix``), same per-query ``__call__``; plus
 ``score_batch`` which scores many queries in one launch (the reference scores
-one query per call on one thread).
+one query per call on one thread), and ``recommend_batch``, the batched form of
+candidate selector → scorer → ``TopNRanker``, whose scoring and top-n selection
+run together in one kernel (``lk_knn_recommend_batch``).
 """
 
 from __future__ import annotations
@@ -167,3 +169,70 @@ class ItemKNNScorer(Component, Trainable):
         if ratings is None or len(ratings) == 0:
             return ItemList(items, scores=np.nan)  # knn/item.py:238-245
         return self.score_batch([ratings], [items])[0]
+
+    def recommend_batch(self, queries, n: int, *, exclude: Literal["query"] | None = "query") -> list[ItemList]:
+        """
+        Top-``n`` items for every query, scored and selected on the device in one launch: for each query the
+        result of ``TrainingItemsCandidateSelector`` (every item, minus the query's items when
+        ``exclude="query"``), ``__call__`` and ``TopNRanker``, bit for bit, with ``nbr_counts``.  A query without
+        history gets an empty list.
+        """
+        _check_exclude(exclude)
+        st = self._device_state()
+        dev = st.sim_cols.device
+        n_eff = min(int(n), st.n_items)
+        hists = [RecQuery.create(q).query_items for q in queries]
+        if n_eff <= 0:
+            return [_empty_list(self.items) for _ in hists]
+        if n_eff > int(_lib.lib().lk_topn_max()):
+            raise ValueError(f"n={n_eff} exceeds the engine limit of {int(_lib.lib().lk_topn_max())}")
+        at, r_ptr, r_items, r_vals = [], [0], [], []
+        for i, hist in enumerate(hists):
+            if hist is None or len(hist) == 0:  # knn/item.py:238-245: every score is null
+                continue
+            rn = hist.numbers(vocabulary=self.items, missing="negative").astype(np.int32)
+            if self.config.explicit:
+                rv = hist.field("rating")
+                if rv is None:
+                    raise RuntimeError("explicit-feedback scorer must have ratings")
+                rv = rv.astype(np.float32, copy=True)
+                ok = rn >= 0
+                rv[ok] -= self.item_means[rn[ok]]  # knn/item.py:262-271
+                r_vals.append(rv)
+            at.append(i)
+            r_items.append(rn)
+            r_ptr.append(r_ptr[-1] + len(rn))
+        out = [_empty_list(self.items) for _ in hists]
+        if not at:
+            return out
+        ref_ptr = torch.tensor(r_ptr, dtype=torch.int64, device=dev)
+        ref_items = torch.from_numpy(np.concatenate(r_items)).to(dev)
+        idx, val, nbrs, cnt = st.recommend(
+            ref_ptr, ref_items,
+            torch.from_numpy(np.concatenate(r_vals)).to(dev) if self.config.explicit else None,
+            self.config.max_nbrs, self.config.min_nbrs, n_eff,
+            item_offset=torch.from_numpy(self.item_means).to(dev) if self.config.explicit else None,
+            # the candidates leave out the query's own items: its history, already on the device
+            excl_indptr=ref_ptr if exclude == "query" else None,
+            excl_items=ref_items if exclude == "query" else None,
+        )  # fmt: skip
+        idx, val, nbrs, cnt = idx.cpu().numpy(), val.cpu().numpy(), nbrs.cpu().numpy(), cnt.cpu().numpy()
+        for j, i in enumerate(at):
+            c = int(cnt[j])
+            out[i] = ItemList(
+                item_ids=self.items.ids(idx[j, :c]), item_nums=idx[j, :c].copy(), vocabulary=self.items,
+                scores=val[j, :c].copy(), nbr_counts=nbrs[j, :c].copy(),
+            )  # fmt: skip
+        return out
+
+
+def _check_exclude(exclude) -> None:
+    if exclude not in ("query", None):
+        raise ValueError(f'exclude must be "query" or None, not {exclude!r}')
+
+
+def _empty_list(vocabulary) -> ItemList:
+    return ItemList(
+        item_ids=vocabulary.ids(np.zeros(0, np.int32)), item_nums=np.zeros(0, np.int32), vocabulary=vocabulary,
+        scores=np.zeros(0, np.float32),
+    )  # fmt: skip

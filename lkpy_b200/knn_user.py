@@ -20,7 +20,9 @@ weights from the neighbour list, values from the rating matrix — bit-exact aga
 ScoreAccumulator emulation (``tests/test_user_knn_gpu.py``).
 
 ``score_batch`` runs each step once for many queries, and the neighbour lists pass from (i) to (ii)
-without leaving the device.  Both device states are built on first use and are not pickled.
+without leaving the device.  ``recommend_batch`` does the same over all items and selects each query's top n
+in the aggregation kernel (its ranking mode, ``lk_knn_recommend_batch``), the batched form of scorer →
+``TopNRanker``.  Both device states are built on first use and are not pickled.
 """
 
 from __future__ import annotations
@@ -37,6 +39,7 @@ from . import _lib, engine
 from .als import _as_dataset
 from .components import Component, ItemList, RecQuery, Trainable, TrainingOptions
 from .data import InteractionCSR
+from .knn import _check_exclude, _empty_list
 
 
 class UserKNNConfig(BaseModel, extra="forbid"):
@@ -192,3 +195,52 @@ class UserKNNScorer(Component, Trainable):
 
     def __call__(self, query, items: ItemList) -> ItemList:
         return self.score_batch([query], [items])[0]
+
+    def recommend_batch(self, queries, n: int, *, exclude: Literal["query"] | None = "query") -> list[ItemList]:
+        """
+        Top-``n`` items for every query: one neighbour search, then scoring and selection over all items in one
+        launch (``KnnScorerState.recommend`` in user mode).  For each query the result of
+        ``TrainingItemsCandidateSelector`` (every item, minus the known items of ``query.query_items`` when
+        ``exclude="query"``; a query given only a user id excludes nothing), ``__call__`` and ``TopNRanker``, bit
+        for bit.  A query without neighbours or usable data gets an empty list.
+        """
+        _check_exclude(exclude)
+        st = self._device_state()
+        dev = st.sim_cols.device
+        n_eff = min(int(n), st.n_items)
+        rqs = [RecQuery.create(q) for q in queries]
+        if n_eff <= 0:
+            return [_empty_list(self.items) for _ in rqs]
+        if n_eff > int(_lib.lib().lk_topn_max()):
+            raise ValueError(f"n={n_eff} exceeds the engine limit of {int(_lib.lib().lk_topn_max())}")
+        specs, at, means, excl = [], [], [], []
+        for i, rq in enumerate(rqs):
+            qd = self._query(rq)
+            if qd is not None:
+                specs.append(qd[0])
+                at.append(i)
+                means.append(qd[1])
+                ex = np.zeros(0, np.int32)
+                if exclude == "query" and rq.query_items is not None:
+                    ex = rq.query_items.numbers(vocabulary=self.items, missing="negative").astype(np.int32)
+                excl.append(ex)
+        out = [_empty_list(self.items) for _ in rqs]
+        if not specs:
+            return out
+        ns = self._neighbour_state()
+        nb_indptr, nb_rows, nb_sims = ns.neighbours(ns.queries(specs), self.config.min_sim)
+        e_ptr = np.concatenate([[0], np.cumsum([len(e) for e in excl])]).astype(np.int64)
+        idx, val, _nbrs, cnt = st.recommend(
+            nb_indptr, nb_rows, nb_sims, self.config.max_nbrs, self.config.min_nbrs, n_eff,
+            query_offset=torch.tensor(means, dtype=torch.float32, device=dev),  # scores += umean (user.py:243-244)
+            excl_indptr=torch.from_numpy(e_ptr).to(dev) if exclude == "query" else None,
+            excl_items=torch.from_numpy(np.concatenate(excl)).to(dev) if exclude == "query" else None,
+        )  # fmt: skip
+        idx, val, cnt = idx.cpu().numpy(), val.cpu().numpy(), cnt.cpu().numpy()
+        for j, i in enumerate(at):
+            c = int(cnt[j])  # 0 for a query without neighbours: every score is null
+            out[i] = ItemList(
+                item_ids=self.items.ids(idx[j, :c]), item_nums=idx[j, :c].copy(), vocabulary=self.items,
+                scores=val[j, :c].copy(),
+            )  # fmt: skip
+        return out
