@@ -37,7 +37,7 @@ class AccelTask(Generic[R]):
 
     Both are live: the kernels hand out work from a device counter and re-read a device cancel flag
     every time a CTA fetches work (``fetch_work``, common.cuh).  ``cancel()`` raises the flag from a
-    side stream — rows / similarity rows already started finish, nothing new starts, ``invoke`` raises
+    side stream — rows / similarity rows already handed out finish, nothing new starts, ``invoke`` raises
     — and ``current_progress()`` copies the counter out on that side stream without disturbing the
     compute stream (the role of ``CancelAdapter``, ``implicit.rs:72-73``).
     """

@@ -13,7 +13,9 @@
 //      explicit: A = G + reg * n * I                           y = sum_j v_j o_j
 //
 // Each warp owns a 64 x 64 quadrant of G as 4 x 8 m16n8 accumulator tiles (128 floats per lane, the
-// SIMT kernel's register footprint).  A = Z^T and B = Z are the same staged tile:
+// SIMT kernel's register footprint); at k = 64 the one warp keeps only the 20 tiles the Cholesky reads (the
+// lower triangle and the diagonal 16 x 16 blocks, 80 floats per lane), which lets 12 CTAs share an SM.
+// A = Z^T and B = Z are the same staged tile:
 //   * bf16 rows with unweighted / uniformly weighted Gram: mma.m16n8k16 bf16, operands loaded with
 //     ldmatrix.trans (the tile is feature-contiguous, the MMA wants pairs along the gathered rows).
 //     The products are exact; parity is against the oracle that rounds the gathered rows to bf16.
@@ -38,15 +40,25 @@ struct TcCfg {
     static constexpr bool BF16MMA = sizeof(ET) == 2 && !WEIGHTED;
     static constexpr int SROW = KP + 8;  // staged row stride (elements)
     static constexpr int STAGE_ELTS = C::STAGE_ROWS * SROW;
-    static constexpr int STAGES_BYTES = C::NSTAGE * STAGE_ELTS * (int)sizeof(ET);
     static constexpr int CHOL_BYTES = KP * C::LDA * 4;
+    // k = 64 bf16: a third stage still fits in the Cholesky buffer the stages share, and gives the gather two
+    // stages of look-ahead
+    static constexpr int NSTAGE = KP == 64 && 3 * STAGE_ELTS * (int)sizeof(ET) <= CHOL_BYTES ? 3 : C::NSTAGE;
+    static constexpr int STAGES_BYTES = NSTAGE * STAGE_ELTS * (int)sizeof(ET);
     static constexpr int UNI = STAGES_BYTES > CHOL_BYTES ? STAGES_BYTES : CHOL_BYTES;
     static constexpr int ZERO_BYTES = KP * 2;  // one zero bf16 row (ldmatrix target for rows past the end)
-    // union | y[KP] | dinv[KP] | mbarriers | misc | zero row
-    static constexpr int SMEM_BYTES = UNI + KP * 4 + KP * 4 + C::NSTAGE * 8 + 64 + ZERO_BYTES;
-    // operand fragments sit next to the 128 accumulators: fewer resident warps than the SIMT kernel, up to
-    // 255 registers each (8 one-warp CTAs per SM at k = 64, 2 four-warp CTAs at k = 128)
-    static constexpr int OCC = KP >= 128 ? 2 : 8;
+    // union | y[KP] | dinv[KP] | zero row | mbarriers | misc
+    static constexpr int ZERO_OFF = UNI + KP * 4 + KP * 4;
+    static_assert(UNI % 16 == 0 && ZERO_OFF % 16 == 0, "bulk-copy destinations and ldmatrix rows are 16-byte aligned");
+    static constexpr int SMEM_BYTES = ZERO_OFF + ZERO_BYTES + NSTAGE * 8 + 64;
+    // k = 64: chol_solve reads only the lower triangle and the diagonal 16 x 16 blocks of the system, so the
+    // one warp accumulates only the 20 m16n8 tiles (mi, nj) with nj <= 2 mi + 1 (80 floats per lane instead
+    // of 128).  k = 128 keeps full 64 x 64 quadrants (a warp's quadrant may lie wholly in either triangle).
+    static constexpr bool LOWER = KP == 64;
+    __device__ static constexpr bool tile(int mi, int nj) { return !LOWER || nj <= 2 * mi + 1; }
+    // operand fragments sit next to the accumulators: fewer resident warps than the SIMT kernel (12 one-warp
+    // CTAs per SM at k = 64, up to 168 registers each; 2 four-warp CTAs at k = 128, up to 255)
+    static constexpr int OCC = KP >= 128 ? 2 : 12;
 };
 
 __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], uint32_t addr)
@@ -92,16 +104,16 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
 {
     using C = AlsCfg<KP>;
     using T = TcCfg<KP, ET, WEIGHTED>;
-    constexpr int NW = C::NW, NT = C::NT, LDA = C::LDA, SROW = T::SROW;
+    constexpr int NW = C::NW, NT = C::NT, LDA = C::LDA, SROW = T::SROW, NS = T::NSTAGE;
     constexpr bool IMPLICIT = MODE == LK_ALS_IMPLICIT;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     ET *stage0 = reinterpret_cast<ET *>(smem_raw);
     float *As = reinterpret_cast<float *>(smem_raw);
     float *ys = reinterpret_cast<float *>(smem_raw + T::UNI);
     float *dinv = ys + KP;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(dinv + KP);
-    int *s_misc = reinterpret_cast<int *>(bars + C::NSTAGE);
-    unsigned char *zero_row = reinterpret_cast<unsigned char *>(s_misc + 16);
+    unsigned char *zero_row = smem_raw + T::ZERO_OFF;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(zero_row + T::ZERO_BYTES);
+    int *s_misc = reinterpret_cast<int *>(bars + NS);
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = lane >> 2, t = lane & 3;
@@ -113,15 +125,28 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
     const float scale = (IMPLICIT && !WEIGHTED) ? a.uniform_val : 1.0f;
 
     if (tid == 0) {
-        for (int s = 0; s < C::NSTAGE; s++) mbar_init(&bars[s], 1);
+        for (int s = 0; s < NS; s++) mbar_init(&bars[s], 1);
         mbar_fence_init();
     }
     for (int i = tid; i < T::ZERO_BYTES / 16; i += NT) reinterpret_cast<uint4 *>(zero_row)[i] = make_uint4(0, 0, 0, 0);
     __syncthreads();
     uint32_t phases = 0;
 
+    // k = 64: thread 0 claims the next chunk when it starts the current one, so the atomic's round trip
+    // overlaps a whole chunk of work instead of leading the next one.  A claimed chunk is always finished:
+    // after the cancel flag is raised, a CTA still completes the one chunk it has claimed ahead.
+    constexpr bool CLAIM_AHEAD = KP == 64;
+    int next = 0;
+    if (CLAIM_AHEAD && tid == 0) next = fetch_work(a.d_work_counter, a.d_cancel);
     for (;;) {
-        if (tid == 0) s_misc[0] = fetch_work(a.d_work_counter, a.d_cancel);
+        if (tid == 0) {
+            if constexpr (CLAIM_AHEAD) {
+                s_misc[0] = next;
+                if (next < a.n_chunks) next = fetch_work(a.d_work_counter, a.d_cancel);
+            } else {
+                s_misc[0] = fetch_work(a.d_work_counter, a.d_cancel);
+            }
+        }
         __syncthreads();
         const int64_t ci = s_misc[0];
         __syncthreads();
@@ -142,13 +167,14 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
             continue;
         }
 
-        float acc[4][8][4];
+        float acc[4][8][4];  // tiles outside T::tile are never touched
 #pragma unroll
         for (int mi = 0; mi < 4; mi++)
 #pragma unroll
             for (int nj = 0; nj < 8; nj++)
 #pragma unroll
-                for (int r = 0; r < 4; r++) acc[mi][nj][r] = 0.0f;
+                for (int r = 0; r < 4; r++)
+                    if (T::tile(mi, nj)) acc[mi][nj][r] = 0.0f;
         float yacc[C::YPT];
 #pragma unroll
         for (int q = 0; q < C::YPT; q++) yacc[q] = 0.0f;
@@ -156,19 +182,16 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
         const int n_it = (len + 31) >> 5;
         const int32_t *cols = a.d_cols + begin;
         const float *vals = a.d_vals + begin;
-        int cA = -1, cB = -1, cC = -1;
-        float vA = 0.f, vB = 0.f, vC = 0.f;
-        if (lane < len) {
-            cA = __ldg(cols + lane);
-            vA = __ldg(vals + lane);
-        }
-        if (32 + lane < len) {
-            cB = __ldg(cols + 32 + lane);
-            vB = __ldg(vals + 32 + lane);
-        }
+        // column index of this lane's row in stages it .. it + NS (cq[0]: stage it), value in stages it, it + 1
+        int cq[NS + 1];
+        float vq[2];
+#pragma unroll
+        for (int j = 0; j < NS; j++) cq[j] = j * 32 + lane < len ? __ldg(cols + j * 32 + lane) : -1;
+#pragma unroll
+        for (int j = 0; j < 2; j++) vq[j] = j * 32 + lane < len ? __ldg(vals + j * 32 + lane) : 0.f;
 
         auto issue = [&](int it, int c) {
-            const int s = it & 1;
+            const int s = it % NS;
             const int nrows = min(32, len - it * 32);
             ET *dst = stage0 + s * T::STAGE_ELTS;
             if (warp == 0) {
@@ -177,18 +200,17 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
             }
         };
 
-        issue(0, cA);
+#pragma unroll
+        for (int j = 0; j < NS - 1; j++)
+            if (j < n_it) issue(j, cq[j]);
         for (int it = 0; it < n_it; it++) {
-            const int s = it & 1;
-            // column indices two stages ahead
-            if ((it + 2) * 32 + lane < len) {
-                cC = __ldg(cols + (it + 2) * 32 + lane);
-                vC = __ldg(vals + (it + 2) * 32 + lane);
-            } else {
-                cC = -1;
-                vC = 0.f;
-            }
-            if (it + 1 < n_it) issue(it + 1, cB);
+            const int s = it % NS;
+            // column indices NS stages ahead
+            const int nxt = (it + NS) * 32 + lane;
+            cq[NS] = nxt < len ? __ldg(cols + nxt) : -1;
+            const int vnxt = (it + 2) * 32 + lane;
+            const float vn = vnxt < len ? __ldg(vals + vnxt) : 0.f;
+            if (it + NS - 1 < n_it) issue(it + NS - 1, cq[NS - 1]);
             mbar_wait(&bars[s], (phases >> s) & 1u);
             phases ^= (1u << s);
             const int nrows = min(32, len - it * 32);
@@ -196,7 +218,7 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
 
             // right-hand side, as the SIMT kernel computes it
             for (int r = 0; r < nrows; r++) {
-                const float v = __shfl_sync(FULL, vA, r);
+                const float v = __shfl_sync(FULL, vq[0], r);
                 const float w = IMPLICIT ? v + 1.0f : v;
 #pragma unroll
                 for (int q = 0; q < C::YPT; q++) yacc[q] = fmaf(tc_elt(st[r * SROW + tid + q * NT]), w, yacc[q]);
@@ -225,10 +247,12 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
                     for (int mi = 0; mi < 4; mi++)
 #pragma unroll
                         for (int nj = 0; nj < 8; nj++)
-                            mma_bf16_16816(acc[mi][nj], af[mi], bfr[nj >> 1][2 * (nj & 1)], bfr[nj >> 1][2 * (nj & 1) + 1]);
+                            if (T::tile(mi, nj))
+                                mma_bf16_16816(acc[mi][nj], af[mi], bfr[nj >> 1][2 * (nj & 1)],
+                                               bfr[nj >> 1][2 * (nj & 1) + 1]);
                 }
             } else {
-                const float sq = WEIGHTED ? sqrtf(vA) : 1.0f;  // rows past the end carry v = 0
+                const float sq = WEIGHTED ? sqrtf(vq[0]) : 1.0f;  // rows past the end carry v = 0
                 for (int k0 = 0; k0 < nrows; k0 += 8) {
                     const int r0 = k0 + t, r1 = k0 + t + 4;
                     const bool ok0 = r0 < nrows, ok1 = r1 < nrows;
@@ -252,6 +276,7 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
                         split_tf32(z(ok1, p1, s1, m0 + 8), ah[3], al[3]);
 #pragma unroll
                         for (int nj = 0; nj < 8; nj++) {
+                            if (!T::tile(mi, nj)) continue;
                             mma_tf32_1688(acc[mi][nj], ah, bh[nj][0], bh[nj][1]);
                             mma_tf32_1688(acc[mi][nj], ah, bl[nj][0], bl[nj][1]);
                             mma_tf32_1688(acc[mi][nj], al, bh[nj][0], bh[nj][1]);
@@ -260,10 +285,10 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
                 }
             }
             cta_sync<NW>();  // everyone is done with stage s before it is re-armed
-            cA = cB;
-            vA = vB;
-            cB = cC;
-            vB = vC;
+#pragma unroll
+            for (int j = 0; j < NS; j++) cq[j] = cq[j + 1];
+            vq[0] = vq[1];
+            vq[1] = vn;
         }
 
         // accumulator (mi, nj, r) holds G[qi + 16 mi + g + 8 (r / 2)][qj + 8 nj + 2 t + r % 2]
@@ -273,7 +298,8 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
 #pragma unroll
                 for (int nj = 0; nj < 8; nj++)
 #pragma unroll
-                    for (int r = 0; r < 4; r++) acc[mi][nj][r] *= scale;
+                    for (int r = 0; r < 4; r++)
+                        if (T::tile(mi, nj)) acc[mi][nj][r] *= scale;
         }
 
         // ---- rows split over several chunks: park the partial, last part reduces
@@ -285,7 +311,8 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
                 for (int nj = 0; nj < 8; nj++)
 #pragma unroll
                     for (int h = 0; h < 2; h++)
-                        __stcg(reinterpret_cast<float2 *>(slot + (qi + 16 * mi + g + 8 * h) * KP + qj + 8 * nj + 2 * t),
+                        if (T::tile(mi, nj))
+                            __stcg(reinterpret_cast<float2 *>(slot + (qi + 16 * mi + g + 8 * h) * KP + qj + 8 * nj + 2 * t),
                                make_float2(acc[mi][nj][2 * h], acc[mi][nj][2 * h + 1]));
 #pragma unroll
             for (int q = 0; q < C::YPT; q++) __stcg(slot + KP * KP + tid + q * NT, yacc[q]);
@@ -305,7 +332,8 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
 #pragma unroll
                 for (int nj = 0; nj < 8; nj++)
 #pragma unroll
-                    for (int r = 0; r < 4; r++) acc[mi][nj][r] = 0.0f;
+                    for (int r = 0; r < 4; r++)
+                        if (T::tile(mi, nj)) acc[mi][nj][r] = 0.0f;
 #pragma unroll
             for (int q = 0; q < C::YPT; q++) yacc[q] = 0.0f;
             for (int p = 0; p < nparts; p++) {
@@ -316,6 +344,7 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
                     for (int nj = 0; nj < 8; nj++)
 #pragma unroll
                         for (int h = 0; h < 2; h++) {
+                            if (!T::tile(mi, nj)) continue;
                             const float2 v = __ldcg(
                                 reinterpret_cast<const float2 *>(sp + (qi + 16 * mi + g + 8 * h) * KP + qj + 8 * nj + 2 * t));
                             acc[mi][nj][2 * h] += v.x;
@@ -335,6 +364,7 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
             for (int nj = 0; nj < 8; nj++)
 #pragma unroll
                 for (int h = 0; h < 2; h++) {
+                    if (!T::tile(mi, nj)) continue;
                     const int gi = qi + 16 * mi + g + 8 * h, gc = qj + 8 * nj + 2 * t;
                     float v0 = acc[mi][nj][2 * h], v1 = acc[mi][nj][2 * h + 1];
                     if constexpr (IMPLICIT) {
@@ -366,6 +396,8 @@ static int launch_tc(const lk_als_args &a, cudaStream_t st)
     using T = TcCfg<KP, ET, WEIGHTED>;
     auto kern = als_tc_kernel<KP, ET, MODE, WEIGHTED>;
     LK_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SMEM_BYTES));
+    // k = 64 needs the whole 228 KB carve-out for 12 resident CTAs
+    LK_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     int occ = 0;
     LK_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, AlsCfg<KP>::NT, T::SMEM_BYTES));
     const int64_t grid = std::max<int64_t>(1, std::min<int64_t>((int64_t)sm_count() * std::max(occ, 1), a.n_chunks));

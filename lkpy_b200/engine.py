@@ -213,7 +213,9 @@ def als_half_epoch(
     a.d_status = ptr(plan.status)
     a.vals_uniform = 1 if plan.vals_uniform else 0
     a.uniform_val = plan.uniform_val
-    a.d_cancel = ptr(cancel)  # optional device flag: non-zero stops the hand-out of rows (cooperative cancel)
+    # optional device flag: non-zero stops the hand-out of rows (cooperative cancel); rows already handed out
+    # finish, which for the k = 64 tensor-core kernel includes the one chunk each CTA claims ahead
+    a.d_cancel = ptr(cancel)
     check(lib().lk_als_half_epoch(C.byref(a), stream_ptr()), "lk_als_half_epoch")
 
 
