@@ -16,6 +16,7 @@
  *   kNN scorer + TopNRanker (topn_pipeline)       src/lenskit/basic/topn.py:32-69   lk_knn_recommend_batch
  *   UserKNNScorer neighbours (SciPy, host)        src/lenskit/knn/user.py:189-214   lk_uknn_search
  *   _accel.data.argtopn (SURVEY.md 8f, "next")    src/accel/data/sorting.rs:131-170 lk_topn_columns
+ *   ALS scorer + TopNRanker (score_matrix/recommend_batch) src/lenskit/als/_common.py:133-175 lk_als_recommend_batch
  *
  * Conventions
  *   - plain C: pointers and sizes only; no C++/torch types cross this boundary;
@@ -378,6 +379,43 @@ typedef struct lk_knn_rank_args {
     int32_t *d_out_cnt;            /* [n_queries] */
 } lk_knn_rank_args;
 LK_API int lk_knn_recommend_batch(const lk_knn_score_args *score, const lk_knn_rank_args *rank, void *stream);
+
+/* ------------------------------------------------------------------------
+ * Batched ALS scoring and top-n recommendation (als_recommend.cu).  For query b with embedding x_b
+ * (d_queries row b) and item i (d_items row i), the score is one fp32 FMA chain in ascending d,
+ *     s = +0.0f;  for d = 0 .. k-1:  s = fmaf(Q[i,d], x_b[d], s)
+ * then s = s + d_item_offset[i] and s = s + d_query_offset[b] (f32 adds, each only when the pointer is set).
+ *   n == 0   score mode: d_scores[i * n_queries + b] = s (item-major, the layout of Q . X^T);
+ *   n >= 1   rank mode (n <= lk_topn_max()): for every query, argtopn over its candidates (all items ascending,
+ *            minus d_excl_items[d_excl_indptr[b] .. d_excl_indptr[b+1]]), ties included, written like
+ *            lk_topn_columns' outputs but query-major:
+ *              d_out_idx[b*n + t]  item number of rank t, -1 beyond the count
+ *              d_out_val[b*n + t]  its score, NaN beyond the count
+ *              d_out_cnt[b]        the number of candidates with a non-NaN score, at most n
+ *            The excluded items must be ASCENDING within each query; repeats and negative numbers are allowed
+ *            (and skipped).  d_excl_indptr may be NULL (nothing excluded).  n > 128 keeps the heaps in
+ *            d_workspace, lk_als_recommend_workspace_bytes(n_queries, n) bytes (NULL when that is 0).
+ * k in 1..128; n_items < 2^31.  Both modes share the dot products, so argtopn over a score-mode column gives
+ * the rank-mode list bit for bit.  The grid is one CTA per 64 queries sweeping every item: batch widely.
+ * ---------------------------------------------------------------------- */
+typedef struct lk_als_rec_args {
+    int64_t n_items;
+    int32_t k;                      /* 1..128 */
+    int32_t n_queries;
+    const float *d_items;           /* Q [n_items][k], row-major */
+    const float *d_queries;         /* X [n_queries][k], row-major */
+    const float *d_item_offset;     /* [n_items] or NULL */
+    const float *d_query_offset;    /* [n_queries] or NULL */
+    int32_t n;                      /* 0: score mode; 1..lk_topn_max(): rank mode */
+    float *d_scores;                /* score mode: [n_items][n_queries] */
+    const int64_t *d_excl_indptr;   /* rank mode: [n_queries+1] or NULL */
+    const int32_t *d_excl_items;    /* ascending within a query, repeats allowed, negative skipped */
+    void *d_workspace;              /* lk_als_recommend_workspace_bytes(n_queries, n) bytes */
+    int32_t *d_out_idx; float *d_out_val; /* [n_queries * n] */
+    int32_t *d_out_cnt;             /* [n_queries] */
+} lk_als_rec_args;
+LK_API int64_t lk_als_recommend_workspace_bytes(int32_t n_queries, int32_t n);
+LK_API int lk_als_recommend_batch(const lk_als_rec_args *args, void *stream);
 
 /* ------------------------------------------------------------------------
  * Batched top-N (SURVEY.md §8f N2: the step after the scorer)

@@ -179,6 +179,26 @@ class LkUknnSearchArgs(C.Structure):
     ]
 
 
+class LkAlsRecArgs(C.Structure):
+    _fields_ = [
+        ("n_items", C.c_int64),
+        ("k", C.c_int32),
+        ("n_queries", C.c_int32),
+        ("d_items", vp),
+        ("d_queries", vp),
+        ("d_item_offset", vp),
+        ("d_query_offset", vp),
+        ("n", C.c_int32),
+        ("d_scores", vp),
+        ("d_excl_indptr", vp),
+        ("d_excl_items", vp),
+        ("d_workspace", vp),
+        ("d_out_idx", vp),
+        ("d_out_val", vp),
+        ("d_out_cnt", vp),
+    ]
+
+
 #: every symbol ``include/lkpy_b200.h`` declares: name -> (restype, argtypes)
 SYMBOLS: dict[str, tuple] = {
     "lk_version": (C.c_int, []),
@@ -211,6 +231,8 @@ SYMBOLS: dict[str, tuple] = {
     "lk_knn_recommend_batch": (C.c_int, [C.POINTER(LkKnnScoreArgs), C.POINTER(LkKnnRankArgs), vp]),
     "lk_topn_max": (C.c_int, []),
     "lk_topn_columns": (C.c_int, [vp, C.c_int64, C.c_int64, C.c_int64, C.c_int32, vp, vp, vp, vp]),
+    "lk_als_recommend_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
+    "lk_als_recommend_batch": (C.c_int, [C.POINTER(LkAlsRecArgs), vp]),
 }
 
 _lib = None

@@ -174,35 +174,85 @@ class ALSBase(UsesTrainer, Component):
             scorable |= known
         return X, scorable, user_nums, fold_bias
 
-    def score_matrix(self, queries) -> torch.Tensor:
-        """Scores of every item for every query, item-major: [n_items, B] f32, NaN columns for unscorable queries."""
-        X, scorable, user_nums, fold_bias = self.embed_batch(queries)
-        S = self._device_items() @ X.T  # [n_items, B]; fp32 GEMM (allow_tf32 is off by default)
+    def _offsets(self, user_nums, fold_bias, dev):
         item_off, query_off = self.batch_offsets(user_nums, fold_bias)
         if item_off is not None:
-            S += torch.from_numpy(item_off.astype(np.float32)).to(S.device)[:, None]
+            item_off = torch.from_numpy(np.ascontiguousarray(item_off, dtype=np.float32)).to(dev)
         if query_off is not None:
-            S += torch.from_numpy(query_off.astype(np.float32)).to(S.device)[None, :]
+            query_off = torch.from_numpy(np.ascontiguousarray(query_off, dtype=np.float32)).to(dev)
+        return item_off, query_off
+
+    def score_matrix(self, queries) -> torch.Tensor:
+        """
+        Scores of every item for every query, item-major: [n_items, B] f32, NaN columns for unscorable queries.
+        Each score is one fp32 FMA chain over ascending d, then the item offset and the query offset (f32 adds):
+        ``engine.als_recommend``'s score mode.
+        """
+        X, scorable, user_nums, fold_bias = self.embed_batch(queries)
+        item_off, query_off = self._offsets(user_nums, fold_bias, X.device)
+        S = engine.als_recommend(self._device_items(), X, None, item_off, query_off)
         if not scorable.all():
             S[:, torch.from_numpy(np.flatnonzero(~scorable)).to(S.device)] = float("nan")
         return S
 
-    def recommend_batch(self, queries, n: int) -> list[ItemList]:
-        """Top-``n`` items for every query: the batched form of scorer → ``TopNRanker``."""
-        S = self.score_matrix(queries)
-        n_eff = min(int(n), S.shape[0])
+    def recommend_batch(self, queries, n: int, *, exclude: Literal["query"] | None = None) -> list[ItemList]:
+        """
+        Top-``n`` items for every query, scored and selected on the device in one launch (``engine.als_recommend``'s
+        rank mode; memory O(B·n), no score matrix): for each query the result of the candidate selector, the
+        scores of :meth:`score_matrix` and ``TopNRanker``, bit for bit.  ``exclude="query"`` leaves the query's
+        own items (``query.query_items`` known to the model) out of the candidates, as
+        ``TrainingItemsCandidateSelector`` does; the default ``None`` ranks every item.  (The kNN scorers'
+        ``recommend_batch`` defaults to ``"query"``.)  An unscorable query gets an empty list.  The kernel sweeps
+        every item once per 64 queries, so batch widely.
+        """
+        from .knn import _check_exclude
+
+        _check_exclude(exclude)
+        queries = [RecQuery.create(q) for q in queries]
+        n_items = self.item_embeddings.shape[0]
+        n_eff = min(int(n), n_items)
         if n_eff <= 0:
-            return [ItemList([], scores=np.empty(0, dtype=np.float32)) for _ in range(S.shape[1])]
-        idx, val, cnt = engine.topn_columns(S, n_eff)
+            return [ItemList([], scores=np.empty(0, dtype=np.float32)) for _ in queries]
+        n_max = int(_lib.lib().lk_topn_max())
+        if n_eff > n_max:
+            raise ValueError(f"n={n_eff} exceeds the engine limit of {n_max}")
+        X, scorable, user_nums, fold_bias = self.embed_batch(queries)
+        out = [_empty_list(self.items) for _ in queries]
+        at = np.flatnonzero(scorable)
+        if len(at) == 0:
+            return out
+        dev = X.device
+        item_off, query_off = self._offsets(user_nums, fold_bias, dev)
+        excl_ptr = excl_items = None
+        if exclude == "query":
+            ptr_, nums = [0], []
+            for b in at:
+                qi = queries[b].query_items
+                e = qi.numbers(vocabulary=self.items, missing="negative") if qi is not None else np.zeros(0)
+                nums.append(np.asarray(e, dtype=np.int32))
+                ptr_.append(ptr_[-1] + len(e))
+            excl_ptr = torch.tensor(ptr_, dtype=torch.int64, device=dev)
+            excl_items = torch.from_numpy(np.concatenate(nums)).to(dev)
+        sel = torch.from_numpy(at).to(dev)
+        idx, val, cnt = engine.als_recommend(
+            self._device_items(), X[sel].contiguous(), n_eff, item_off,
+            query_off[sel] if query_off is not None else None, excl_ptr, excl_items,
+        )  # fmt: skip
         idx, val, cnt = idx.cpu().numpy(), val.cpu().numpy(), cnt.cpu().numpy()
-        out = []
-        for b in range(S.shape[1]):
-            c = int(cnt[b])
-            out.append(
-                ItemList(item_ids=self.items.ids(idx[b, :c]), item_nums=idx[b, :c].copy(), vocabulary=self.items,
-                         scores=val[b, :c].copy())
+        for j, b in enumerate(at):
+            c = int(cnt[j])
+            out[b] = ItemList(
+                item_ids=self.items.ids(idx[j, :c]), item_nums=idx[j, :c].copy(), vocabulary=self.items,
+                scores=val[j, :c].copy(),
             )  # fmt: skip
         return out
+
+
+def _empty_list(vocabulary) -> ItemList:
+    return ItemList(
+        item_ids=vocabulary.ids(np.zeros(0, np.int32)), item_nums=np.zeros(0, np.int32), vocabulary=vocabulary,
+        scores=np.zeros(0, np.float32),
+    )  # fmt: skip
 
 
 def _solve_cholesky(A: np.ndarray, y: np.ndarray) -> np.ndarray:

@@ -30,6 +30,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "topn_heap.cuh"
 
 namespace lk {
 
@@ -426,8 +427,8 @@ __device__ __forceinline__ int block_excl_scan(int v, int *s_scan, int *s_carry,
 //   * the offsets are added in f32 before ranking, as the components add them to the scores on the host.
 // The CTA walks the slot-map row in chunks of RANK_CHUNK items (coalesced, clearing the map as step 5 does),
 // compacts the candidates that pass the filter in item order (ballots and a 64-entry scan) and one thread offers
-// them to the heap with topn.cu's sift rules.  The heap and the candidate buffer live in DenseSmem, which steps
-// 1-3 no longer need at that point, so the ranking mode costs no shared memory of its own.
+// them to the heap of topn_heap.cuh.  The heap and the candidate buffer live in DenseSmem, which steps 1-3 no
+// longer need at that point, so the ranking mode costs no shared memory of its own.
 // ---------------------------------------------------------------------------------------------
 constexpr int RANK_NMAX = 1024;  // lk_topn_max()
 constexpr int RANK_UNITS = 8;    // items per thread and chunk
@@ -448,49 +449,17 @@ struct RankSmem {
 };
 static_assert(sizeof(RankSmem) <= sizeof(DenseSmem), "the ranking state must fit in the dense kernel's shared memory");
 
-// heap.rs:67-89 downheap as topn.cu does it (the smaller child, the left one on a tie, while strictly smaller),
-// moving a hole instead of swapping: the same final arrangement
-__device__ void rank_down(RankSmem &r, int pos, const int lim)
-{
-    const float v = r.hv[pos];
-    const int32_t k = r.hk[pos], c = r.hc[pos];
-    for (;;) {
-        int mn = pos;
-        float mv = v;
-        const int left = 2 * pos + 1, right = 2 * pos + 2;
-        if (left < lim && r.hv[left] < mv) {
-            mn = left;
-            mv = r.hv[left];
-        }
-        if (right < lim && r.hv[right] < mv) mn = right;
-        if (mn == pos) break;
-        r.hv[pos] = r.hv[mn], r.hk[pos] = r.hk[mn], r.hc[pos] = r.hc[mn];
-        pos = mn;
-    }
-    r.hv[pos] = v, r.hk[pos] = k, r.hc[pos] = c;
-}
-
-// topn.cu's offer for a non-NaN score: heap.rs:41-45 push + upheap while not full, else heap.rs:46-52 replace the
-// root if strictly greater and downheap
-__device__ __forceinline__ void rank_offer(RankSmem &r, int &count, float &root, const int n, const float s,
-                                           const int32_t k, const int32_t c)
-{
-    if (count < n) {
-        int pos = count++;
-        while (pos > 0) {
-            const int parent = (pos - 1) / 2;
-            if (!(r.hv[parent] > s)) break;
-            r.hv[pos] = r.hv[parent], r.hk[pos] = r.hk[parent], r.hc[pos] = r.hc[parent];
-            pos = parent;
-        }
-        r.hv[pos] = s, r.hk[pos] = k, r.hc[pos] = c;
-        root = r.hv[0];
-    } else if (s > root) {
-        r.hv[0] = s, r.hk[0] = k, r.hc[0] = c;
-        rank_down(r, 0, n);
-        root = r.hv[0];
-    }
-}
+// the ranking heap in RankSmem; its entries carry the accumulator length beside the item number
+struct RankHeap {
+    struct Ent {
+        float v;
+        int32_t k, c;
+    };
+    RankSmem &r;
+    __device__ __forceinline__ float val(const int p) const { return r.hv[p]; }
+    __device__ __forceinline__ Ent get(const int p) const { return {r.hv[p], r.hk[p], r.hc[p]}; }
+    __device__ __forceinline__ void put(const int p, const Ent e) { r.hv[p] = e.v, r.hk[p] = e.k, r.hc[p] = e.c; }
+};
 
 // Ranking mode's step 5 for query q (the whole CTA; steps 1-4 done, DenseSmem free): exclusion, the ranking walk,
 // the heap sort and the n output entries.  Leaves the slot map at zero.
@@ -571,7 +540,8 @@ __device__ void rank_query(RankSmem &r, const lk_knn_rank_args &rk, const int q,
             int count = count0;
             float root = root0;
             const int nc = r.n_cand;
-            for (int i = 0; i < nc; i++) rank_offer(r, count, root, n, r.cv[i], r.ck[i], r.cc[i]);
+            RankHeap h{r};
+            for (int i = 0; i < nc; i++) topn_heap_offer(h, count, root, n, RankHeap::Ent{r.cv[i], r.ck[i], r.cc[i]});
             r.count = count;
             r.root = root;
         }
@@ -580,13 +550,8 @@ __device__ void rank_query(RankSmem &r, const lk_knn_rank_args &rk, const int q,
     // heap.rs:56-65 topn_vec: heap sort into descending score order
     const int count = r.count;
     if (tid == 0) {
-        for (int m = count - 1; m > 0; m--) {
-            const float tv = r.hv[0];
-            const int32_t tk = r.hk[0], tc = r.hc[0];
-            r.hv[0] = r.hv[m], r.hk[0] = r.hk[m], r.hc[0] = r.hc[m];
-            r.hv[m] = tv, r.hk[m] = tk, r.hc[m] = tc;
-            rank_down(r, 0, m);
-        }
+        RankHeap h{r};
+        topn_heap_sort(h, count);
     }
     __syncthreads();
     const int64_t o = (int64_t)q * n;

@@ -20,8 +20,22 @@
 // kept in a register.  Heap storage is per-thread local memory.
 
 #include "common.cuh"
+#include "topn_heap.cuh"
 
 namespace lk {
+
+// the heap in the thread's own arrays (local memory)
+struct TopnLocalHeap {
+    struct Ent {
+        float v;
+        int32_t k;
+    };
+    float *hv;
+    int32_t *hk;
+    __device__ __forceinline__ float val(const int p) const { return hv[p]; }
+    __device__ __forceinline__ Ent get(const int p) const { return {hv[p], hk[p]}; }
+    __device__ __forceinline__ void put(const int p, const Ent e) { hv[p] = e.v, hk[p] = e.k; }
+};
 
 template <int NMAX>
 __global__ void __launch_bounds__(128)
@@ -33,57 +47,13 @@ topn_columns_kernel(const float *__restrict__ scores, const int64_t n_rows, cons
     if (u >= n_cols) return;
     float hv[NMAX];
     int32_t hk[NMAX];
+    TopnLocalHeap h{hv, hk};
     int count = 0;
     float root = 0.0f;  // hv[0] once the heap is full
 
-    // heap.rs:67-89 downheap, iterative
-    auto down = [&](int pos, const int lim) {
-        for (;;) {
-            int mn = pos;
-            float mv = hv[pos];
-            const int left = 2 * pos + 1, right = 2 * pos + 2;
-            if (left < lim) {
-                const float lv = hv[left];
-                if (lv < mv) {
-                    mn = left;
-                    mv = lv;
-                }
-            }
-            if (right < lim) {
-                const float rv = hv[right];
-                if (rv < mv) mn = right;
-            }
-            if (mn == pos) return;
-            const float tv = hv[pos];
-            const int32_t tk = hk[pos];
-            hv[pos] = hv[mn], hk[pos] = hk[mn];
-            hv[mn] = tv, hk[mn] = tk;
-            pos = mn;
-        }
-    };
     auto offer = [&](const float s, const int32_t i) {
         if (s != s) return;  // sorting.rs:142 accept = !is_nan
-        if (count < n) {     // heap.rs:41-45 push + upheap
-            int pos = count++;
-            hv[pos] = s, hk[pos] = i;
-            while (pos > 0) {
-                const int parent = (pos - 1) / 2;
-                if (hv[parent] > hv[pos]) {
-                    const float tv = hv[pos];
-                    const int32_t tk = hk[pos];
-                    hv[pos] = hv[parent], hk[pos] = hk[parent];
-                    hv[parent] = tv, hk[parent] = tk;
-                    pos = parent;
-                } else {
-                    break;
-                }
-            }
-            root = hv[0];
-        } else if (s > root) {  // heap.rs:46-52 replace the root, downheap
-            hv[0] = s, hk[0] = i;
-            down(0, n);
-            root = hv[0];
-        }
+        topn_heap_offer(h, count, root, n, TopnLocalHeap::Ent{s, i});
     };
 
     const float *col = scores + u;
@@ -98,16 +68,7 @@ topn_columns_kernel(const float *__restrict__ scores, const int64_t n_rows, cons
     }
     for (; i < n_rows; i++) offer(__ldcs(col + i * ld), (int32_t)i);
 
-    // heap.rs:56-65 topn_vec: heap sort, the arrays end up in descending score order
-    int m = count;
-    while (m > 0) {
-        m--;
-        const float tv = hv[0];
-        const int32_t tk = hk[0];
-        hv[0] = hv[m], hk[0] = hk[m];
-        hv[m] = tv, hk[m] = tk;
-        down(0, m);
-    }
+    topn_heap_sort(h, count);  // heap.rs:56-65 topn_vec: descending score order
     for (int t = 0; t < n; t++) {
         out_idx[u * n + t] = t < count ? hk[t] : -1;
         if (out_val != nullptr) out_val[u * n + t] = t < count ? hv[t] : __int_as_float(0x7fc00000);

@@ -1,0 +1,76 @@
+// topn_heap.cuh — the one device copy of argtopn's indirect min-heap (src/accel/indirect/heap.rs,
+// src/accel/data/sorting.rs:131-170), shared by topn.cu, the ranking mode of knn_score.cu and
+// als_recommend.cu.
+//
+// The heap is reached through a storage policy H so that each kernel keeps its own layout (per-thread local
+// arrays, shared memory, a strided workspace) and its own payload:
+//     typename H::Ent         the entry: a float score `v` and whatever rides along with it
+//     float H::val(int pos)   the score at pos
+//     Ent   H::get(int pos)   the entry at pos
+//     void  H::put(int pos, Ent e)
+// Both sifts move a hole instead of swapping, which leaves exactly the arrangement the reference's swaps leave.
+#pragma once
+
+namespace lk {
+
+// heap.rs:67-89 downheap: the smaller child, the left one on a tie, while strictly smaller than the moving entry
+template <class H>
+__device__ __forceinline__ void topn_heap_down(H &h, int pos, const int lim)
+{
+    const typename H::Ent e = h.get(pos);
+    for (;;) {
+        int mn = pos;
+        float mv = e.v;
+        const int left = 2 * pos + 1, right = 2 * pos + 2;
+        if (left < lim) {
+            const float lv = h.val(left);
+            if (lv < mv) {
+                mn = left;
+                mv = lv;
+            }
+        }
+        if (right < lim && h.val(right) < mv) mn = right;
+        if (mn == pos) break;
+        h.put(pos, h.get(mn));
+        pos = mn;
+    }
+    h.put(pos, e);
+}
+
+// argtopn's offer of a non-NaN entry (the caller drops NaN, sorting.rs:142): heap.rs:41-45 push + upheap while
+// the heap has room, else heap.rs:46-52 replace the root if strictly greater and downheap.  `root` mirrors the
+// root's score once the heap holds an entry.
+template <class H>
+__device__ __forceinline__ void topn_heap_offer(H &h, int &count, float &root, const int n,
+                                                const typename H::Ent e)
+{
+    if (count < n) {
+        int pos = count++;
+        while (pos > 0) {
+            const int parent = (pos - 1) / 2;
+            if (!(h.val(parent) > e.v)) break;
+            h.put(pos, h.get(parent));
+            pos = parent;
+        }
+        h.put(pos, e);
+        root = h.val(0);
+    } else if (e.v > root) {
+        h.put(0, e);
+        topn_heap_down(h, 0, n);
+        root = h.val(0);
+    }
+}
+
+// heap.rs:56-65 topn_vec: heap sort; positions 0..count-1 end up in descending score order
+template <class H>
+__device__ __forceinline__ void topn_heap_sort(H &h, const int count)
+{
+    for (int m = count - 1; m > 0; m--) {
+        const typename H::Ent t = h.get(0);
+        h.put(0, h.get(m));
+        h.put(m, t);
+        topn_heap_down(h, 0, m);
+    }
+}
+
+}  // namespace lk

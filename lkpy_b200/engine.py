@@ -17,7 +17,8 @@ import torch
 
 from . import _lib
 from ._lib import (
-    LkAlsArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr,
+    LkAlsArgs, LkAlsRecArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkUknnSearchArgs, check, lib,
+    ptr, stream_ptr,
 )  # fmt: skip
 from .data import InteractionCSR
 
@@ -920,3 +921,82 @@ def topn_columns(scores: torch.Tensor, n: int, with_values: bool = True):
         "lk_topn_columns",
     )  # fmt: skip
     return idx, val, cnt[:n_cols]
+
+
+def als_recommend(
+    items: torch.Tensor,
+    queries: torch.Tensor,
+    n: int | None = None,
+    item_offset: torch.Tensor | None = None,
+    query_offset: torch.Tensor | None = None,
+    excl_indptr: torch.Tensor | None = None,
+    excl_items: torch.Tensor | None = None,
+):
+    """
+    ALS scores of every item for every query (``lk_als_recommend_batch``): one fp32 FMA chain per score over
+    ascending d, ``s = fmaf(items[i, d], queries[b, d], s)`` from +0, then ``+ item_offset[i]`` and
+    ``+ query_offset[b]`` (f32).  ``items`` is [n_items, k], ``queries`` [B, k], both f32 with k in 1..128.
+
+    ``n=None`` (score mode) returns the item-major matrix ``S [n_items, B]`` f32.  An integer ``n`` (rank mode,
+    1..``lk_topn_max()``) returns ``(idx [B, n] int32 item numbers, -1 padding; val [B, n] f32, NaN padding;
+    cnt [B] int32)``: for every query, ``argtopn`` over all items minus
+    ``excl_items[excl_indptr[b]:excl_indptr[b+1]]`` (any order; repeats, negative and unknown numbers are
+    ignored), ties included, without storing the score matrix.  The grid has one CTA per 64 queries, each
+    sweeping every item, so small batches leave the GPU idle: batch widely.
+    """
+    _lib.require_device()
+    if items.dtype != torch.float32 or queries.dtype != torch.float32 or items.dim() != 2 or queries.dim() != 2:
+        raise TypeError("items and queries must be 2-D float32 tensors")
+    n_items, k = items.shape
+    B = queries.shape[0]
+    if queries.shape[1] != k:
+        raise ValueError(f"queries have {queries.shape[1]} columns, items {k}")
+    dev = queries.device
+    items, queries = items.contiguous(), queries.contiguous()
+    a = LkAlsRecArgs()
+    a.n_items, a.k, a.n_queries = n_items, k, B
+    a.d_items, a.d_queries = ptr(items), ptr(queries)
+    if item_offset is not None:
+        item_offset = item_offset.to(device=dev, dtype=torch.float32).contiguous()
+    if query_offset is not None:
+        query_offset = query_offset.to(device=dev, dtype=torch.float32).contiguous()
+    a.d_item_offset, a.d_query_offset = ptr(item_offset), ptr(query_offset)
+    if n is None:
+        S = torch.empty((n_items, B), dtype=torch.float32, device=dev)
+        a.n, a.d_scores = 0, ptr(S)
+        check(lib().lk_als_recommend_batch(C.byref(a), stream_ptr()), "lk_als_recommend_batch")
+        return S
+    n_max = int(lib().lk_topn_max())
+    if not 1 <= int(n) <= n_max:
+        raise ValueError(f"n must be in 1..{n_max}")
+    n = int(n)
+    if excl_indptr is not None:
+        excl_indptr, excl_items = _sorted_exclusions(excl_indptr, excl_items, n_items, B, dev)
+    idx = torch.empty((B, n), dtype=torch.int32, device=dev)
+    val = torch.empty((B, n), dtype=torch.float32, device=dev)
+    cnt = torch.empty(max(B, 1), dtype=torch.int32, device=dev)
+    ws_bytes = int(lib().lk_als_recommend_workspace_bytes(B, n))
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes > 0 else None
+    a.n = n
+    a.d_excl_indptr, a.d_excl_items, a.d_workspace = ptr(excl_indptr), ptr(excl_items), ptr(ws)
+    a.d_out_idx, a.d_out_val, a.d_out_cnt = ptr(idx), ptr(val), ptr(cnt)
+    check(lib().lk_als_recommend_batch(C.byref(a), stream_ptr()), "lk_als_recommend_batch")
+    return idx, val, cnt[:B]
+
+
+def _sorted_exclusions(indptr: torch.Tensor, items: torch.Tensor, n_items: int, B: int, dev):
+    """The exclusion lists as the kernel takes them: item numbers in 0..n_items-1, ascending within each query."""
+    indptr = indptr.to(device=dev, dtype=torch.int64)
+    items = items.to(device=dev, dtype=torch.int64)
+    if indptr.numel() != B + 1:
+        raise ValueError(f"excl_indptr must have {B + 1} entries")
+    seg = torch.repeat_interleave(torch.arange(B, device=dev), indptr[1:] - indptr[:-1])
+    ok = (items >= 0) & (items < n_items)
+    seg, items = seg[ok], items[ok]
+    keys = torch.sort(seg * n_items + items).values
+    out_ptr = torch.zeros(B + 1, dtype=torch.int64, device=dev)
+    out_ptr[1:] = torch.cumsum(torch.bincount(seg, minlength=B), 0)
+    out_items = (keys - (keys // max(n_items, 1)) * n_items).to(torch.int32)
+    if out_items.numel() == 0:  # a non-NULL address the kernel never reads (bounded by the indptr)
+        out_items = torch.full((1,), -1, dtype=torch.int32, device=dev)
+    return out_ptr, out_items
