@@ -17,6 +17,8 @@
  *   UserKNNScorer neighbours (SciPy, host)        src/lenskit/knn/user.py:189-214   lk_uknn_search
  *   _accel.data.argtopn (SURVEY.md 8f, "next")    src/accel/data/sorting.rs:131-170 lk_topn_columns
  *   ALS scorer + TopNRanker (score_matrix/recommend_batch) src/lenskit/als/_common.py:133-175 lk_als_recommend_batch
+ *   _accel.data.count_cooc / dense_cooc           src/accel/data/cooc.rs:49-214     lk_cooc_count (+ _diagonal, _dense)
+ *   AssociationScorer.train / __call__            src/lenskit/knn/association.py    lk_cooc_count (LK_ASSOC_*), lk_assoc_score_batch
  *
  * Conventions
  *   - plain C: pointers and sizes only; no C++/torch types cross this boundary;
@@ -435,6 +437,114 @@ LK_API int lk_als_recommend_batch(const lk_als_rec_args *args, void *stream);
 LK_API int lk_topn_max(void);
 LK_API int lk_topn_columns(const float *d_scores, int64_t n_rows, int64_t n_cols, int64_t ld, int32_t n,
                            int32_t *d_out_idx, float *d_out_val, int32_t *d_out_cnt, void *stream);
+
+/* ------------------------------------------------------------------------
+ * Co-occurrence counting (cooc.cu): the counts of `_accel.data.count_cooc` / `dense_cooc`
+ * (src/accel/data/cooc.rs:185-214, pairs/symmetric.rs, pairs/dense.rs) and the association matrix of
+ * AssociationScorer.train (src/lenskit/knn/association.py:91-130).
+ *
+ * The groups play the users of the item-kNN build: GI is the groups x items CSR (a group's items ascending,
+ * repeated items kept), IG its transpose with one entry per occurrence.  Row i of the result is
+ *     C[i][j] = sum over the occurrences of i in a group g of the occurrences of j in g  (= sum_g #i * #j)
+ * over the columns j > i (full_rows == 0, the strict upper triangle) or j != i (full_rows == 1).  The diagonal
+ * sum_g #i (#i + 1) / 2 comes from lk_cooc_diagonal.  Work units are (item, column tile):
+ * unit = item * geom.n_halves + h; units not listed in d_sched produce nothing (their d_part_cnt stays as
+ * given, so the caller zeroes it).  Survivors (non-zero counts) go to a bump-allocated pool in column order per
+ * unit; lk_cooc_pool_to_csr gathers them into a row-sorted CSR with int64 offsets.
+ *   method LK_COOC_COUNT: pool values are the int32 counts;
+ *   LK_ASSOC_PROBABILITY / LK_ASSOC_LIFT (full_rows == 1): the f32 association value of entry (r, c),
+ *     v = f32(f64(f32(count)) / (f64(cnt[r]) + damping));  lift: v = f32(v * f32(n_groups)),
+ *     v = f32(f64(v) / (f64(cnt[c]) + damping))          (cnt = d_item_count, n_groups = geom.n_users)
+ * Every count of a row is at most the row's cost (lk_cooc_row_cost); the caller passes the largest cost in
+ * max_row_cost and a value of 2^31 or more returns LK_ERR_UNSUPPORTED instead of wrapping.
+ * Statuses: 1 = pool too small (nothing is usable; never a truncated result).
+ * ---------------------------------------------------------------------- */
+#define LK_COOC_COUNT 0
+#define LK_ASSOC_PROBABILITY 1
+#define LK_ASSOC_LIFT 2
+
+/* Accumulator tiling for n_cols columns over the rows of an n_rows-row CSR whose tile pointers are taken
+ * (groups for counting, items for association scoring). */
+LK_API int lk_cooc_geometry(int32_t n_rows, int32_t n_cols, lk_knn_geom *geom);
+
+typedef struct lk_cooc_args {
+    lk_knn_geom geom;                  /* lk_cooc_geometry(n_groups, n_items) */
+    const int32_t *d_gi_indptr;        /* [n_groups+1] */
+    const int32_t *d_gi_items;         /* ascending within a group, repeats kept */
+    const int32_t *d_ig_indptr;        /* [n_items+1] */
+    const int32_t *d_ig_groups;        /* one entry per occurrence */
+    const int32_t *d_tile_ptr;         /* lk_knn_tile_pointers(geom, d_gi_indptr, d_gi_items) */
+    int32_t full_rows;                 /* 0: columns > row; 1: every column but the row */
+    int32_t method;                    /* LK_COOC_COUNT or LK_ASSOC_* */
+    const int32_t *d_item_count;       /* [n_items] per-item interaction counts (LK_ASSOC_*) */
+    double damping;                    /* >= 0 */
+    int64_t max_row_cost;              /* largest lk_cooc_row_cost of a scheduled row */
+    const int32_t *d_sched;            /* [n_work] unit ids, most expensive first */
+    int64_t n_work;
+    int32_t *d_pool_cols;              /* [pool_capacity] */
+    void *d_pool_vals;                 /* [pool_capacity] 32-bit: int32 counts or f32 values */
+    int64_t pool_capacity;
+    int64_t *d_pool_off;               /* [n_items * n_halves] */
+    int32_t *d_part_cnt;               /* [n_items * n_halves] */
+    unsigned long long *d_pool_cursor; /* [1] zeroed by the call */
+    int32_t *d_work_counter;           /* [1] zeroed by the call; = units handed out so far (progress) */
+    int32_t *d_status;                 /* [1] zeroed by the call */
+    const int32_t *d_cancel;           /* optional device flag (see lk_als_args.d_cancel) */
+} lk_cooc_args;
+
+/* d_cost [n_items] (int64): the pair updates of each row, sum over its occurrences of the group's columns
+ * that the row counts (columns > item, or the whole group with full_rows). */
+LK_API int lk_cooc_row_cost(const lk_cooc_args *args, int64_t *d_cost, void *stream);
+LK_API int lk_cooc_count(const lk_cooc_args *args, void *stream);
+/* d_out_indptr [n_items+1]: exclusive scan of the per-item sums of d_part_cnt; d_out_vals 32-bit words */
+LK_API int lk_cooc_pool_to_csr(const lk_cooc_args *args, const int64_t *d_out_indptr, int32_t *d_out_cols,
+                               void *d_out_vals, void *stream);
+/* d_diag [n_items] (int64, zeroed by the caller) += sum over groups of #i (#i + 1) / 2 */
+LK_API int lk_cooc_diagonal(const lk_cooc_args *args, int64_t *d_diag, void *stream);
+/* Dense sink of dense_cooc: d_out [n_items][n_items] f32 (zeroed by the caller) gets f32(count) of every entry
+ * of the strict-upper-triangle CSR at (i, j) and (j, i), and f32(d_diag[i]) at (i, i) when d_diag is set. */
+LK_API int lk_cooc_dense(int32_t n_items, const int64_t *d_indptr, const int32_t *d_cols, const int32_t *d_counts,
+                         const int64_t *d_diag, float *d_out, void *stream);
+
+/* ------------------------------------------------------------------------
+ * Association scoring (cooc.cu): AssociationScorer.__call__ (association.py:132-163) batched, and its
+ * composition with TrainingItemsCandidateSelector and TopNRanker.  For query q with reference rows
+ * r_0 .. r_{R-1} (d_ref_items in query order, repeats kept, all in [0, n_items)) and item c:
+ *   agg 0 (mean, max_nbrs = None):  s = +0.0f;  for t = 0 .. R-1: s = s + A[r_t, c]  (f32 adds in query order,
+ *                                   absent entries add nothing);  score = f32(f64(s) / f64(R))
+ *   agg 1 (max, max_nbrs = 1):      score = max over t of A[r_t, c], absent entries 0
+ *   R == 0: every score is NaN.
+ * A is the association CSR (int64 offsets, rows sorted by column); d_tile_ptr [n_items * (n_subtiles+1)] holds,
+ * for each row and s = 0..n_subtiles, the position of its first column >= s * tile_cols RELATIVE to the row
+ * start (lk_assoc_tile_pointers).
+ *   n == 0  score mode: d_scores [n_queries][n_items].
+ *   n >= 1  rank mode (n <= lk_topn_max()): argtopn over every item ascending minus the query's excluded items
+ *           (ascending within a query, repeats and negative numbers skipped), ties included; outputs as
+ *           lk_als_recommend_batch's rank mode.
+ * n_queries * geom.n_halves < 2^31.
+ * ---------------------------------------------------------------------- */
+LK_API int lk_assoc_tile_pointers(const lk_knn_geom *geom, const int64_t *d_indptr, const int32_t *d_cols,
+                                  int32_t *d_tile_ptr, void *stream);
+
+typedef struct lk_assoc_score_args {
+    lk_knn_geom geom;                  /* lk_cooc_geometry(n_items, n_items) */
+    const int64_t *d_indptr;           /* [n_items+1] */
+    const int32_t *d_cols;
+    const float *d_vals;
+    const int32_t *d_tile_ptr;
+    int32_t n_queries;
+    int32_t agg;                       /* 0 mean, 1 max */
+    const int64_t *d_ref_indptr;       /* [n_queries+1] */
+    const int32_t *d_ref_items;
+    int32_t n;                         /* 0: score mode; 1..lk_topn_max(): rank mode */
+    float *d_scores;                   /* score mode: [n_queries][n_items] */
+    const int64_t *d_excl_indptr;      /* rank mode: [n_queries+1] or NULL */
+    const int32_t *d_excl_items;
+    int32_t *d_out_idx; float *d_out_val; /* rank mode: [n_queries * n] */
+    int32_t *d_out_cnt;                /* rank mode: [n_queries] */
+} lk_assoc_score_args;
+
+LK_API int lk_assoc_score_batch(const lk_assoc_score_args *args, void *stream);
 
 #ifdef __cplusplus
 }

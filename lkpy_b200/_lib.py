@@ -17,6 +17,7 @@ LK_OK = 0
 LK_DTYPE_F32, LK_DTYPE_BF16 = 0, 1
 LK_ALS_IMPLICIT, LK_ALS_EXPLICIT = 0, 1
 LK_MAX_REPLICAS = 8
+LK_COOC_COUNT, LK_ASSOC_PROBABILITY, LK_ASSOC_LIFT = 0, 1, 2
 
 i32p = C.POINTER(C.c_int32)
 i64p = C.POINTER(C.c_int64)
@@ -199,6 +200,54 @@ class LkAlsRecArgs(C.Structure):
     ]
 
 
+class LkCoocArgs(C.Structure):
+    _fields_ = [
+        ("geom", LkKnnGeom),
+        ("d_gi_indptr", vp),
+        ("d_gi_items", vp),
+        ("d_ig_indptr", vp),
+        ("d_ig_groups", vp),
+        ("d_tile_ptr", vp),
+        ("full_rows", C.c_int32),
+        ("method", C.c_int32),
+        ("d_item_count", vp),
+        ("damping", C.c_double),
+        ("max_row_cost", C.c_int64),
+        ("d_sched", vp),
+        ("n_work", C.c_int64),
+        ("d_pool_cols", vp),
+        ("d_pool_vals", vp),
+        ("pool_capacity", C.c_int64),
+        ("d_pool_off", vp),
+        ("d_part_cnt", vp),
+        ("d_pool_cursor", vp),
+        ("d_work_counter", vp),
+        ("d_status", vp),
+        ("d_cancel", vp),
+    ]
+
+
+class LkAssocScoreArgs(C.Structure):
+    _fields_ = [
+        ("geom", LkKnnGeom),
+        ("d_indptr", vp),
+        ("d_cols", vp),
+        ("d_vals", vp),
+        ("d_tile_ptr", vp),
+        ("n_queries", C.c_int32),
+        ("agg", C.c_int32),
+        ("d_ref_indptr", vp),
+        ("d_ref_items", vp),
+        ("n", C.c_int32),
+        ("d_scores", vp),
+        ("d_excl_indptr", vp),
+        ("d_excl_items", vp),
+        ("d_out_idx", vp),
+        ("d_out_val", vp),
+        ("d_out_cnt", vp),
+    ]
+
+
 #: every symbol ``include/lkpy_b200.h`` declares: name -> (restype, argtypes)
 SYMBOLS: dict[str, tuple] = {
     "lk_version": (C.c_int, []),
@@ -233,6 +282,14 @@ SYMBOLS: dict[str, tuple] = {
     "lk_topn_columns": (C.c_int, [vp, C.c_int64, C.c_int64, C.c_int64, C.c_int32, vp, vp, vp, vp]),
     "lk_als_recommend_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
     "lk_als_recommend_batch": (C.c_int, [C.POINTER(LkAlsRecArgs), vp]),
+    "lk_cooc_geometry": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(LkKnnGeom)]),
+    "lk_cooc_row_cost": (C.c_int, [C.POINTER(LkCoocArgs), vp, vp]),
+    "lk_cooc_count": (C.c_int, [C.POINTER(LkCoocArgs), vp]),
+    "lk_cooc_pool_to_csr": (C.c_int, [C.POINTER(LkCoocArgs), vp, vp, vp, vp]),
+    "lk_cooc_diagonal": (C.c_int, [C.POINTER(LkCoocArgs), vp, vp]),
+    "lk_cooc_dense": (C.c_int, [C.c_int32, vp, vp, vp, vp, vp, vp]),
+    "lk_assoc_tile_pointers": (C.c_int, [C.POINTER(LkKnnGeom), vp, vp, vp, vp]),
+    "lk_assoc_score_batch": (C.c_int, [C.POINTER(LkAssocScoreArgs), vp]),
 }
 
 _lib = None

@@ -544,8 +544,105 @@ def argtopn_batch(scores: Any, n: int) -> list[np.ndarray]:
     return [idx[b, : cnt[b]].copy() for b in range(s.shape[0])]
 
 
+def _int32_column(name: str, a: Any) -> np.ndarray:
+    """A non-null int32 array from Arrow or NumPy input (the reference's ``checked_array::<Int32Type>``)."""
+    if hasattr(a, "null_count") and hasattr(a, "to_numpy"):
+        import pyarrow as pa
+
+        if isinstance(a, pa.ChunkedArray):
+            a = a.combine_chunks()
+        if a.null_count:
+            raise ValueError(f"{name} contains nulls")
+        if not pa.types.is_int32(a.type):
+            raise TypeError(f"{name} must be int32, got {a.type}")
+        return a.to_numpy(zero_copy_only=False)
+    arr = np.asarray(a)
+    if arr.ndim != 1 or arr.dtype != np.int32:
+        raise TypeError(f"{name} must be a 1-D int32 array")
+    return arr
+
+
+def _cooc_input(n_groups: int, n_items: int, groups: Any, cols: Any) -> tuple[np.ndarray, np.ndarray]:
+    """Validate the inputs of ``count_cooc`` / ``dense_cooc``: what the reference asserts (and panics on) is a
+    ``ValueError`` here."""
+    if len(groups) != len(cols):
+        raise ValueError("array length mismatch")  # cooc.rs:62-64
+    g, i = _int32_column("groups", groups), _int32_column("cols", cols)
+    if int(n_groups) < 0 or int(n_items) < 0:
+        raise ValueError("n_groups and n_items must be non-negative")
+    if len(g):
+        if np.any(g[1:] < g[:-1]):
+            raise ValueError("groups must be ascending")  # cooc.rs:221-224
+        if g[0] < 0 or g[-1] >= n_groups:
+            raise ValueError(f"group number out of range 0..{n_groups}")
+        if i.min() < 0 or i.max() >= n_items:
+            raise ValueError(f"item number out of range 0..{n_items}")
+    return np.array(g, dtype=np.int32), np.array(i, dtype=np.int32)  # writable copies: torch wraps them
+
+
+def _cooc_upper(n_groups: int, n_items: int, g: np.ndarray, i: np.ndarray, task: AccelTask, diagonal: bool):
+    """Device CoocPlan, the upper-triangle CSR and (optionally) the diagonal, after a cancel check."""
+    dev = _lib.require_device()
+    plan = engine.CoocPlan.create(n_groups, n_items, torch.from_numpy(g).to(dev), torch.from_numpy(i).to(dev))
+    indptr, cols, counts = plan.count(full_rows=False, attach=task._attach)
+    task._check_cancelled()
+    return plan, indptr, cols, counts, plan.diagonal() if diagonal else None
+
+
+def count_cooc(n_groups: int, n_items: int, groups: Any, cols: Any, *, ordered: bool = False, diagonal: bool = True):
+    """
+    ``_accel.data.count_cooc`` (src/accel/data/cooc.rs:49-113): a list of ``pa.RecordBatch`` with non-null int32
+    columns ``row``, ``col``, ``count`` — the diagonal (every item, zeros included) when ``diagonal``, the strict
+    upper triangle row-major with columns ascending, and the same entries with ``row`` and ``col`` swapped.
+    ``ordered=True`` is not supported.  Parameter names follow the stub (``_accel/data.pyi``): ``cols`` are the items.
+    """
+    if ordered:
+        raise NotImplementedError("ordered co-occurrences are not supported on the GPU engine")
+    g, i = _cooc_input(n_groups, n_items, groups, cols)
+    n_groups, n_items = int(n_groups), int(n_items)
+
+    def run(task: AccelTask) -> list:
+        import pyarrow as pa
+
+        with _engine_lock:
+            if n_items == 0:
+                e = np.zeros(0, np.int32)
+                upper, diag = (np.zeros(1, np.int64), e, e), (e if diagonal else None)
+            else:
+                _plan, ip, c, v, d = _cooc_upper(n_groups, n_items, g, i, task, diagonal)
+                upper, diag = (ip.cpu().numpy(), c.cpu().numpy(), v.cpu().numpy()), (None if d is None else d.cpu().numpy())
+        ip, cols, counts = upper
+        rows = np.repeat(np.arange(n_items, dtype=np.int32), np.diff(ip))
+        schema = pa.schema([pa.field(k, pa.int32(), nullable=False) for k in ("row", "col", "count")])
+
+        def batch(r, c, v):
+            return pa.RecordBatch.from_arrays([pa.array(r, pa.int32()), pa.array(c, pa.int32()), pa.array(v, pa.int32())],
+                                              schema=schema)  # fmt: skip
+
+        out = [] if diag is None else [batch(np.arange(n_items, dtype=np.int32), np.arange(n_items, dtype=np.int32), diag)]
+        return out + [batch(rows, cols, counts), batch(cols, rows, counts)]
+
+    return AccelTask(run, total=n_items)
+
+
+def dense_cooc(n_groups: int, n_items: int, groups: Any, cols: Any, *, diagonal: bool = True):
+    """``_accel.data.dense_cooc`` (src/accel/data/cooc.rs:116-160): an ``n_items x n_items`` float32 ndarray with the
+    counts in both triangles and, when ``diagonal``, the diagonal counts (0 otherwise)."""
+    g, i = _cooc_input(n_groups, n_items, groups, cols)
+    n_groups, n_items = int(n_groups), int(n_items)
+
+    def run(task: AccelTask) -> np.ndarray:
+        if n_items == 0:
+            return np.zeros((0, 0), dtype=np.float32)
+        with _engine_lock:
+            plan, ip, c, v, d = _cooc_upper(n_groups, n_items, g, i, task, diagonal)
+            return plan.dense(ip, c, v, d).cpu().numpy()
+
+    return AccelTask(run, total=n_items)
+
+
 #: ``from lkpy_b200.accel import als, knn`` mirrors ``from lenskit._accel import als, knn``
-data = SimpleNamespace(argtopn=argtopn, argtopn_batch=argtopn_batch)
+data = SimpleNamespace(argtopn=argtopn, argtopn_batch=argtopn_batch, count_cooc=count_cooc, dense_cooc=dense_cooc)
 als = SimpleNamespace(
     train_implicit_matrix=train_implicit_matrix, train_explicit_matrix=train_explicit_matrix
 )

@@ -17,8 +17,8 @@ import torch
 
 from . import _lib
 from ._lib import (
-    LkAlsArgs, LkAlsRecArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkUknnSearchArgs, check, lib,
-    ptr, stream_ptr,
+    LkAlsArgs, LkAlsRecArgs, LkAssocScoreArgs, LkCoocArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs,
+    LkUknnSearchArgs, check, lib, ptr, stream_ptr,
 )  # fmt: skip
 from .data import InteractionCSR
 
@@ -1000,3 +1000,240 @@ def _sorted_exclusions(indptr: torch.Tensor, items: torch.Tensor, n_items: int, 
     if out_items.numel() == 0:  # a non-NULL address the kernel never reads (bounded by the indptr)
         out_items = torch.full((1,), -1, dtype=torch.int32, device=dev)
     return out_ptr, out_items
+
+
+# ---------------------------------------------------------------------------
+# co-occurrence counting and association scoring
+# ---------------------------------------------------------------------------
+
+
+@dataclass
+class CoocPlan:
+    """
+    The inputs of ``lk_cooc_count`` for one (groups, items) interaction list: the groups x items CSR (GI, a
+    group's items ascending, repeats kept), its transpose IG (one entry per occurrence), the column tiling and
+    GI's tile pointers.  At the ML-25M shape (25 M interactions) GI and IG take 100 MB each and the tile
+    pointers 32 MB.
+    """
+
+    n_groups: int
+    n_items: int
+    gi_indptr: torch.Tensor  # int32 [n_groups + 1]
+    gi_items: torch.Tensor
+    ig_indptr: torch.Tensor  # int32 [n_items + 1]
+    ig_groups: torch.Tensor
+    geom: LkKnnGeom
+    tile_ptr: torch.Tensor
+    work_counter: torch.Tensor
+    status: torch.Tensor
+    cursor: torch.Tensor
+    #: optional device int32 flag checked by the count kernel whenever a CTA fetches a work unit
+    cancel: torch.Tensor | None = None
+
+    @classmethod
+    def create(cls, n_groups: int, n_items: int, groups: torch.Tensor, items: torch.Tensor) -> "CoocPlan":
+        """``groups`` / ``items``: int32 device tensors of equal length, ``groups`` ascending, every number in range
+        (the caller validates)."""
+        if n_items < 1:
+            raise ValueError("n_items must be positive")
+        if groups.numel() >= 2**31:
+            raise _lib.EngineError("co-occurrence input with 2**31 or more entries is not supported")
+        dev = groups.device
+        g, i = groups.to(torch.int64), items.to(torch.int64)
+
+        def offsets(keys: torch.Tensor, n: int) -> torch.Tensor:
+            ip = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+            torch.cumsum(torch.bincount(keys, minlength=n), 0, out=ip[1:])
+            return ip.to(torch.int32)
+
+        gi_items = (torch.sort(g * n_items + i).values % n_items).to(torch.int32)
+        ig_groups = (torch.sort(i * max(n_groups, 1) + g).values % max(n_groups, 1)).to(torch.int32)
+        gi_indptr, ig_indptr = offsets(g, n_groups), offsets(i, n_items)
+        L = lib()
+        geom = LkKnnGeom()
+        check(L.lk_cooc_geometry(n_groups, n_items, C.byref(geom)), "lk_cooc_geometry")
+        tile_ptr = torch.empty(max(1, n_groups * (geom.n_subtiles + 1)), dtype=torch.int32, device=dev)
+        if gi_items.numel() == 0:
+            gi_items = torch.zeros(1, dtype=torch.int32, device=dev)  # a non-NULL address, never read
+            ig_groups = torch.zeros(1, dtype=torch.int32, device=dev)
+        check(
+            L.lk_knn_tile_pointers(C.byref(geom), ptr(gi_indptr), ptr(gi_items), ptr(tile_ptr), stream_ptr()),
+            "lk_knn_tile_pointers",
+        )
+        z = lambda dt: torch.zeros(1, dtype=dt, device=dev)  # noqa: E731
+        return cls(
+            n_groups, n_items, gi_indptr, gi_items, ig_indptr, ig_groups, geom, tile_ptr,
+            z(torch.int32), z(torch.int32), z(torch.int64),
+        )  # fmt: skip
+
+    def _args(self, full_rows: bool) -> LkCoocArgs:
+        a = LkCoocArgs()
+        a.geom = self.geom
+        a.d_gi_indptr, a.d_gi_items = ptr(self.gi_indptr), ptr(self.gi_items)
+        a.d_ig_indptr, a.d_ig_groups = ptr(self.ig_indptr), ptr(self.ig_groups)
+        a.d_tile_ptr = ptr(self.tile_ptr)
+        a.full_rows = 1 if full_rows else 0
+        a.d_work_counter, a.d_status, a.d_pool_cursor = ptr(self.work_counter), ptr(self.status), ptr(self.cursor)
+        a.d_cancel = ptr(self.cancel)
+        return a
+
+    def row_cost(self, full_rows: bool) -> torch.Tensor:
+        """Pair updates of every row (int64 [n_items]): its columns > item, or all of them with ``full_rows``."""
+        cost = torch.empty(self.n_items, dtype=torch.int64, device=self.gi_indptr.device)
+        check(lib().lk_cooc_row_cost(C.byref(self._args(full_rows)), ptr(cost), stream_ptr()), "lk_cooc_row_cost")
+        return cost
+
+    def count(
+        self,
+        full_rows: bool = False,
+        method: int = _lib.LK_COOC_COUNT,
+        item_count: torch.Tensor | None = None,
+        damping: float = 0.0,
+        attach=None,
+    ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """
+        The co-occurrence rows as a device CSR (int64 indptr [n_items+1], int32 columns ascending, values): the
+        strict upper triangle, or every off-diagonal entry with ``full_rows``.  Values are the int32 counts, or with
+        ``method`` ``LK_ASSOC_PROBABILITY`` / ``LK_ASSOC_LIFT`` (full rows only) the f32 association values of
+        ``AssociationScorer.train`` from ``item_count`` (int32 [n_items]) and ``damping``.  ``attach(counter,
+        units)``, if given, is called before the launch and returns the device cancel flag.
+        """
+        dev = self.gi_indptr.device
+        n, H, CW = self.n_items, self.geom.n_halves, self.geom.warps * self.geom.tile_cols
+        cost = self.row_cost(full_rows)
+        order = torch.argsort(cost, descending=True, stable=True)
+        order = order[cost[order] > 0]  # a row without pair updates has no entries and needs no unit
+        h = torch.arange(H, device=dev)
+        units = order[:, None] * H + h[None, :]
+        if not full_rows:  # tiles left of the diagonal hold no column > item
+            units = units[(h[None, :] + 1) * CW > order[:, None] + 1]
+        sched = units.reshape(-1).to(torch.int32).contiguous()
+        width = (n - 1 - torch.arange(n, device=dev)) if not full_rows else torch.full((n,), n - 1, device=dev)
+        capacity = max(int(torch.minimum(cost, width).sum().item()), 1)  # a row has at most min(cost, width) entries
+        max_cost = int(cost.max().item()) if n else 0
+        pool_cols = torch.empty(capacity, dtype=torch.int32, device=dev)
+        pool_vals = torch.empty(capacity, dtype=torch.int32, device=dev)
+        pool_off = torch.zeros(n * H, dtype=torch.int64, device=dev)
+        part_cnt = torch.zeros(n * H, dtype=torch.int32, device=dev)
+        a = self._args(full_rows)
+        if attach is not None:
+            self.cancel = attach(self.work_counter, sched.numel())
+            a.d_cancel = ptr(self.cancel)
+        a.method, a.d_item_count, a.damping = int(method), ptr(item_count), float(damping)
+        a.max_row_cost = max_cost
+        a.d_sched, a.n_work = ptr(sched), sched.numel()
+        a.d_pool_cols, a.d_pool_vals, a.pool_capacity = ptr(pool_cols), ptr(pool_vals), capacity
+        a.d_pool_off, a.d_part_cnt = ptr(pool_off), ptr(part_cnt)
+        check(lib().lk_cooc_count(C.byref(a), stream_ptr()), "lk_cooc_count")
+        if int(self.status.item()) == 1:
+            raise _lib.EngineError("lk_cooc_count: pool overflow")
+        indptr = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+        torch.cumsum(part_cnt.view(n, H).sum(dim=1, dtype=torch.int64), 0, out=indptr[1:])
+        nnz = int(indptr[-1].item())
+        cols = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
+        vals = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
+        check(lib().lk_cooc_pool_to_csr(C.byref(a), ptr(indptr), ptr(cols), ptr(vals), stream_ptr()), "lk_cooc_pool_to_csr")
+        torch.cuda.current_stream().synchronize()
+        if method != _lib.LK_COOC_COUNT:
+            vals = vals.view(torch.float32)
+        return indptr, cols[:nnz], vals[:nnz]
+
+    def diagonal(self) -> torch.Tensor:
+        """``sum_g #i (#i + 1) / 2`` for every item (int32 [n_items]); a count of 2**31 or more raises."""
+        d = torch.zeros(self.n_items, dtype=torch.int64, device=self.gi_indptr.device)
+        check(lib().lk_cooc_diagonal(C.byref(self._args(False)), ptr(d), stream_ptr()), "lk_cooc_diagonal")
+        if self.n_items and int(d.max().item()) >= 2**31:
+            raise _lib.EngineError("a diagonal co-occurrence count exceeds int32")
+        return d.to(torch.int32)
+
+    def dense(self, indptr: torch.Tensor, cols: torch.Tensor, counts: torch.Tensor, diag: torch.Tensor | None):
+        """``dense_cooc``'s matrix from the upper-triangle CSR of :meth:`count` and, optionally, :meth:`diagonal`."""
+        n = self.n_items
+        out = torch.zeros((n, n), dtype=torch.float32, device=indptr.device)
+        d64 = None if diag is None else diag.to(torch.int64)
+        check(
+            lib().lk_cooc_dense(n, ptr(indptr), ptr(_nonempty(cols)), ptr(_nonempty(counts)), ptr(d64), ptr(out),
+                                stream_ptr()),
+            "lk_cooc_dense",
+        )  # fmt: skip
+        return out
+
+
+def _nonempty(t: torch.Tensor) -> torch.Tensor:
+    """A tensor with a non-NULL address: the library rejects NULL, and bounded reads never touch the placeholder."""
+    return t if t.numel() else torch.zeros(1, dtype=t.dtype, device=t.device)
+
+
+@dataclass
+class AssocState:
+    """The association matrix in HBM (int64 offsets, rows sorted by column) with the tiling and row-relative tile
+    pointers of ``lk_assoc_score_batch``.  Read-only once built: every call allocates its own outputs, so concurrent
+    callers need no lock."""
+
+    n_items: int
+    indptr: torch.Tensor  # int64 [n_items + 1]
+    cols: torch.Tensor  # int32
+    vals: torch.Tensor  # float32
+    geom: LkKnnGeom
+    tile_ptr: torch.Tensor
+
+    @classmethod
+    def create(cls, n_items: int, indptr, cols, vals, device=None) -> "AssocState":
+        device = device or _lib.require_device()
+        dev = lambda t, dt: _nonempty(torch.as_tensor(t).to(device=device, dtype=dt).contiguous())  # noqa: E731
+        ip, c, v = dev(indptr, torch.int64), dev(cols, torch.int32), dev(vals, torch.float32)
+        g = LkKnnGeom()
+        check(lib().lk_cooc_geometry(n_items, n_items, C.byref(g)), "lk_cooc_geometry")
+        tp = torch.empty(max(1, n_items * (g.n_subtiles + 1)), dtype=torch.int32, device=device)
+        check(lib().lk_assoc_tile_pointers(C.byref(g), ptr(ip), ptr(c), ptr(tp), stream_ptr()), "lk_assoc_tile_pointers")
+        return cls(n_items, ip, c, v, g, tp)
+
+    def _args(self, ref_indptr: torch.Tensor, ref_items: torch.Tensor, agg: int) -> LkAssocScoreArgs:
+        a = LkAssocScoreArgs()
+        a.geom = self.geom
+        a.d_indptr, a.d_cols, a.d_vals, a.d_tile_ptr = ptr(self.indptr), ptr(self.cols), ptr(self.vals), ptr(self.tile_ptr)
+        a.n_queries = ref_indptr.numel() - 1
+        a.agg = int(agg)
+        a.d_ref_indptr, a.d_ref_items = ptr(ref_indptr), ptr(_nonempty(ref_items))
+        return a
+
+    def score(self, ref_indptr: torch.Tensor, ref_items: torch.Tensor, agg: int) -> torch.Tensor:
+        """
+        Scores of every item for every query (f32 [B, n_items]): query q's reference rows are
+        ``ref_items[ref_indptr[q]:ref_indptr[q+1]]`` in query order (all in range); ``agg`` 0 is the mean over them
+        (``max_nbrs=None``), 1 the maximum (``max_nbrs=1``); a query without rows scores NaN everywhere.
+        """
+        B = ref_indptr.numel() - 1
+        out = torch.empty((B, self.n_items), dtype=torch.float32, device=self.indptr.device)
+        if B == 0:
+            return out
+        a = self._args(ref_indptr, ref_items, agg)
+        a.n, a.d_scores = 0, ptr(out)
+        check(lib().lk_assoc_score_batch(C.byref(a), stream_ptr()), "lk_assoc_score_batch")
+        return out
+
+    def recommend(
+        self, ref_indptr: torch.Tensor, ref_items: torch.Tensor, agg: int, n: int,
+        excl_indptr: torch.Tensor | None = None, excl_items: torch.Tensor | None = None,
+    ):  # fmt: skip
+        """
+        Top-``n`` of every query over all items minus ``excl_items[excl_indptr[q]:excl_indptr[q+1]]`` (any order),
+        with ``argtopn``'s order and ties: ``(idx [B, n] int32, -1 padding; val [B, n] f32, NaN padding; cnt [B])``.
+        """
+        n_max = int(lib().lk_topn_max())
+        if not 1 <= int(n) <= n_max:
+            raise ValueError(f"n must be in 1..{n_max}")
+        n, dev, B = int(n), self.indptr.device, ref_indptr.numel() - 1
+        idx = torch.empty((B, n), dtype=torch.int32, device=dev)
+        val = torch.empty((B, n), dtype=torch.float32, device=dev)
+        cnt = torch.empty(max(B, 1), dtype=torch.int32, device=dev)
+        if B == 0:
+            return idx, val, cnt[:0]
+        if excl_indptr is not None:
+            excl_indptr, excl_items = _sorted_exclusions(excl_indptr, excl_items, self.n_items, B, dev)
+        a = self._args(ref_indptr, ref_items, agg)
+        a.n = n
+        a.d_excl_indptr, a.d_excl_items = ptr(excl_indptr), ptr(excl_items)
+        a.d_out_idx, a.d_out_val, a.d_out_cnt = ptr(idx), ptr(val), ptr(cnt)
+        check(lib().lk_assoc_score_batch(C.byref(a), stream_ptr()), "lk_assoc_score_batch")
+        return idx, val, cnt[:B]
