@@ -37,7 +37,7 @@ def _stale() -> bool:
         return True
     t = LIB.stat().st_mtime
     deps = [CSRC / s for s in SOURCES] + [
-        CSRC / "common.cuh", CSRC / "als_common.cuh", CSRC / "topn_heap.cuh",
+        CSRC / "common.cuh", CSRC / "als_common.cuh", CSRC / "topn_heap.cuh", CSRC / "tiles.cuh",
     ]  # fmt: skip
     deps.append(CSRC.parent.parent / "include" / "lkpy_b200.h")
     return any(d.stat().st_mtime > t for d in deps)

@@ -155,29 +155,6 @@ __device__ __forceinline__ int warp_incl_scan(int v, int lane)
     return v;
 }
 
-// One warp copies the bump-allocated pool segments of units [u0, u1), in that order, to one CSR row
-// starting at `dst`: the pool -> CSR pass of the unbounded item-kNN build, of the user-kNN neighbour search and of
-// the co-occurrence count.
-// V is the 32-bit value type of the pool (f32 similarities, int32 co-occurrence counts).
-template <typename V>
-__device__ __forceinline__ void warp_copy_pool_segments(int64_t u0, int64_t u1, const int64_t *__restrict__ pool_off,
-                                                        const int32_t *__restrict__ part_cnt,
-                                                        const int32_t *__restrict__ pool_cols,
-                                                        const V *__restrict__ pool_vals, int64_t dst,
-                                                        int32_t *__restrict__ out_cols, V *__restrict__ out_vals,
-                                                        int lane)
-{
-    for (int64_t u = u0; u < u1; u++) {
-        const int64_t src = pool_off[u];
-        const int c = part_cnt[u];
-        for (int t = lane; t < c; t += 32) {
-            out_cols[dst + t] = pool_cols[src + t];
-            out_vals[dst + t] = pool_vals[src + t];
-        }
-        dst += c;
-    }
-}
-
 __device__ __forceinline__ float bf16_bits_to_f32(uint32_t hi16)
 {
     return __uint_as_float(hi16 << 16);

@@ -1,11 +1,11 @@
 // cooc.cu — co-occurrence counting and association scoring for sm_90a.
 //
 // Counting replaces count_cooc_parallel (src/accel/data/cooc.rs:185-214), which walks the groups serially and
-// makes one atomic increment per position pair into an n(n+1)/2 int32 triangle.  Here the groups play the users
-// of the item-kNN build (knn_build.cu): row i is built by walking i's group occurrences (IG) and, for each, the
-// group's items (GI) inside the warp's column sub-tile, found through lk_knn_tile_pointers.  A warp owns a
-// contiguous sub-tile of uint32 counters in shared memory; integer addition commutes, so the lanes add with
-// shared-memory atomics in any order.  Keeping repeated items in both GI and IG makes the reference's duplicate
+// makes one atomic increment per position pair into an n(n+1)/2 int32 triangle.  Here the shared tile core
+// (tiles.cuh) builds row i from i's group occurrences (IG) as the input rows and, for each, the group's items (GI)
+// inside the warp's column sub-tile, found through lk_knn_tile_pointers.  A warp owns a contiguous sub-tile of
+// uint32 counters in shared memory; integer addition commutes, so the lanes add with shared-memory atomics in any
+// order.  Keeping repeated items in both GI and IG makes the reference's duplicate
 // semantics (sum_g #i * #j off the diagonal) fall out of the enumeration.  Work units are (item, column tile),
 // handed out most-expensive-first by a persistent grid; the strict upper triangle skips the tiles left of the
 // diagonal.  After a unit the warps compact their non-zero counters (ballot + popcount keep column order) into
@@ -14,13 +14,13 @@
 //
 // Scoring replaces AssociationScorer.__call__: one CTA per (query, column tile) in score mode, one CTA per
 // query sweeping the column tiles in ascending order in rank mode.  Each warp owns a sub-tile of f32
-// accumulators and walks the query's reference rows in query order (32 rows flattened over the lanes for the
-// loads, applied one row per round, as in knn_build.cu), so every accumulator sees the same sequence of f32
+// accumulators and walks the query's reference rows in query order (the input rows of the tile core, applied one
+// row per round), so every accumulator sees the same sequence of f32
 // adds as NumPy's np.mean(axis=0) over the dense rows (absent entries add +0.0, which changes nothing).  In rank
 // mode warp 0 then offers the tile's scores in ascending item order to argtopn's heap (topn_heap.cuh), keeping
 // only count < n || s > root (exact: a full heap's root never decreases and a full heap rejects s <= root) and
 // skipping excluded items (argtopn's NaN offer).
-#include "common.cuh"
+#include "tiles.cuh"
 #include "topn_heap.cuh"
 
 namespace lk {
@@ -30,10 +30,9 @@ constexpr int CO_NT = CO_WARPS * 32;
 constexpr int CO_HEAP_MAX = 1024;  // lk_topn_max()
 constexpr int CO_CTAS = 2;
 
-static int co_smem_bytes(const lk_knn_geom &g)
-{
-    return g.warps * g.tile_cols * 4 + CO_HEAP_MAX * 8 + g.warps * 4 + 16;
-}
+constexpr int CO_FIXED_SMEM = CO_HEAP_MAX * 8 + CO_WARPS * 4 + 16;  // argtopn heap, per-warp counts
+
+static int co_smem_bytes(const lk_knn_geom &g) { return g.warps * g.tile_cols * 4 + CO_FIXED_SMEM; }
 
 __global__ void cooc_row_cost_kernel(const lk_cooc_args a, int64_t *__restrict__ cost)
 {
@@ -75,13 +74,11 @@ __global__ void __launch_bounds__(CO_NT, CO_CTAS) cooc_count_kernel(const lk_coo
 {
     constexpr int W = CO_WARPS;
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    __shared__ int64_t s_work;
-    __shared__ unsigned long long s_off;
+    __shared__ int s_work;
     const lk_knn_geom &g = a.geom;
     const int TW = g.tile_cols, S1 = g.n_subtiles + 1, H = g.n_halves;
     uint32_t *acc = reinterpret_cast<uint32_t *>(smem_raw);  // [W * TW]
     int *wcnt = reinterpret_cast<int *>(acc + W * TW);         // [W]
-    uint32_t *pool_vals = static_cast<uint32_t *>(a.d_pool_vals);
     const float n_groups = (float)g.n_users;  // NumPy's f32 array * Python int
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -89,10 +86,7 @@ __global__ void __launch_bounds__(CO_NT, CO_CTAS) cooc_count_kernel(const lk_coo
     __syncthreads();
 
     for (;;) {
-        if (tid == 0) s_work = fetch_work(a.d_work_counter, a.d_cancel);
-        __syncthreads();
-        const int64_t wi = s_work;
-        __syncthreads();
+        const int64_t wi = cta_next_work(a.d_work_counter, a.d_cancel, &s_work);
         if (wi >= a.n_work) break;
         const int unit = a.d_sched[wi];
         const int item = unit / H, h = unit - item * H;
@@ -113,25 +107,12 @@ __global__ void __launch_bounds__(CO_NT, CO_CTAS) cooc_count_kernel(const lk_coo
                     base = __ldg(tp);
                     len = __ldg(tp + 1) - base;
                 }
-                const int incl = warp_incl_scan(len, lane);
-                const int total = __shfl_sync(FULL, incl, 31);
-                any |= total > 0;
-                const int adj = base - (incl - len);  // source index = adj[owner] + e
-                for (int e0 = 0; e0 < total; e0 += 32) {
-                    const int e = e0 + lane;
-                    int own = 0;  // owner: smallest lane with incl > e
-#pragma unroll
-                    for (int step = 16; step > 0; step >>= 1) {
-                        const int t = __shfl_sync(FULL, incl, own + step - 1);
-                        if (t <= e) own += step;
-                    }
-                    own = min(own, 31);
-                    const int src = __shfl_sync(FULL, adj, own) + e;
-                    if (e < total) {
+                any |= warp_walk_segments(base, len, lane, [&](bool valid, int, int src) {
+                    if (valid) {
                         const int col = __ldg(a.d_gi_items + src);
                         if (col >= lo_col && col != item) atomicAdd(&my[col - col0], 1u);
                     }
-                }
+                });
             }
         }
         if (!__syncthreads_or(any)) {  // no group of the item reaches this tile: every counter is still 0
@@ -142,53 +123,13 @@ __global__ void __launch_bounds__(CO_NT, CO_CTAS) cooc_count_kernel(const lk_coo
             continue;
         }
 
-        int cnt = 0;
-        for (int c0 = 0; c0 < TW; c0 += 32) cnt += __popc(__ballot_sync(FULL, my[c0 + lane] != 0u));
-        if (lane == 0) wcnt[warp] = cnt;
-        __syncthreads();
-        if (tid == 0) {
-            int n = 0;
-            for (int w = 0; w < W; w++) n += wcnt[w];
-            unsigned long long off = atomicAdd(a.d_pool_cursor, (unsigned long long)n);
-            if (off + (unsigned long long)n > (unsigned long long)a.pool_capacity) {
-                atomicCAS(a.d_status, 0, 1);
-                off = ~0ull;
-            }
-            s_off = off;
-            a.d_pool_off[unit] = (int64_t)off;
-            a.d_part_cnt[unit] = n;
-        }
-        __syncthreads();
-        const unsigned long long off = s_off;
-        int pos = 0;
-        for (int w = 0; w < warp; w++) pos += wcnt[w];
         const double row_den = a.method != LK_COOC_COUNT ? __dadd_rn((double)a.d_item_count[item], a.damping) : 1.0;
-        for (int c0 = 0; c0 < TW; c0 += 32) {
-            const int c = col0 + c0 + lane;
-            const uint32_t v = my[c0 + lane];
-            const bool keep = v != 0u;
-            const unsigned b = __ballot_sync(FULL, keep);
-            if (keep && off != ~0ull) {
-                const unsigned long long k = off + pos + __popc(b & ((1u << lane) - 1u));
-                a.d_pool_cols[k] = c;
-                pool_vals[k] = a.method == LK_COOC_COUNT ? v : assoc_bits(v, row_den, a, c, n_groups);
-            }
-            pos += __popc(b);
-            my[c0 + lane] = 0u;
-        }
-        __syncthreads();  // wcnt and s_off are rewritten by the next unit
+        cta_emit_pool_segment<W>(
+            my, TW, col0, unit, [](uint32_t v, int) { return v != 0u; },
+            [&](uint32_t v, int c) { return a.method == LK_COOC_COUNT ? v : assoc_bits(v, row_den, a, c, n_groups); },
+            0u, wcnt, a.d_pool_cursor, a.pool_capacity, a.d_status, a.d_pool_off, a.d_part_cnt, a.d_pool_cols,
+            static_cast<uint32_t *>(a.d_pool_vals));
     }
-}
-
-__global__ void cooc_pool_to_csr_kernel(const lk_cooc_args a, const int64_t *__restrict__ out_indptr,
-                                        int32_t *__restrict__ out_cols, uint32_t *__restrict__ out_vals)
-{
-    const int warps = (gridDim.x * blockDim.x) >> 5;
-    const int lane = threadIdx.x & 31;
-    const int64_t H = a.geom.n_halves;
-    for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < a.geom.n_items; i += warps)
-        warp_copy_pool_segments(i * H, (i + 1) * H, a.d_pool_off, a.d_part_cnt, a.d_pool_cols,
-                                static_cast<const uint32_t *>(a.d_pool_vals), out_indptr[i], out_cols, out_vals, lane);
 }
 
 // one thread per group: runs of an item inside the group's ascending list give #i (#i + 1) / 2
@@ -313,37 +254,18 @@ __global__ void __launch_bounds__(CO_NT, CO_CTAS) assoc_score_kernel(const lk_as
                 base = __ldg(a.d_indptr + r) + b0;
                 len = __ldg(tp + 1) - b0;
             }
-            const int incl = warp_incl_scan(len, lane);
-            const int total = __shfl_sync(FULL, incl, 31);
-            const int64_t adj = base - (incl - len);  // source index = adj[owner] + e
-            for (int e0 = 0; e0 < total; e0 += 32) {
-                const int e = e0 + lane;
-                const bool valid = e < total;
-                int own = 0;  // owner: smallest lane with incl > e
-#pragma unroll
-                for (int step = 16; step > 0; step >>= 1) {
-                    const int t = __shfl_sync(FULL, incl, own + step - 1);
-                    if (t <= e) own += step;
-                }
-                own = min(own, 31);
-                const int64_t src = __shfl_sync(FULL, adj, own) + e;
+            warp_walk_segments(base, len, lane, [&](bool valid, int own, int64_t src) {
                 int j = 0;
                 float v = 0.0f;
                 if (valid) {
                     j = __ldg(a.d_cols + src) - col0;
                     v = __ldg(a.d_vals + src);
                 }
-                // reference rows in query order, one row per round: the lanes of one row hit distinct columns
-                unsigned pend = __ballot_sync(FULL, valid);
-                while (pend) {
-                    const int leader = __ffs(pend) - 1;
-                    const int oo = __shfl_sync(FULL, own, leader);
-                    const bool mine = valid && own == oo;
-                    if (mine) my[j] = a.agg == 0 ? __fadd_rn(my[j], v) : fmaxf(my[j], v);
-                    __syncwarp();
-                    pend &= ~__ballot_sync(FULL, mine);
-                }
-            }
+                // reference rows in query order
+                warp_apply_in_owner_order(valid, own, [&] {
+                    my[j] = a.agg == 0 ? __fadd_rn(my[j], v) : fmaxf(my[j], v);
+                });
+            });
         }
         // final scores of the warp's sub-tile: np.mean divides the f32 sum by the row count in f64
         if (a.agg == 0) {
@@ -419,26 +341,8 @@ extern "C" {
 int lk_cooc_geometry(int32_t n_rows, int32_t n_cols, lk_knn_geom *geom)
 {
     LK_REQUIRE(geom != nullptr && n_rows >= 0 && n_cols >= 1, LK_ERR_INVALID, "lk_cooc_geometry: bad arguments");
-    const int warps = CO_WARPS;
-    // shared memory budget per CTA (227 KB usable per SM, 1 KB reserved per CTA), 4-byte accumulators; the
-    // argtopn heap of the scoring kernel's rank mode is reserved in every geometry
-    const int budget = (227 * 1024) / CO_CTAS - 1024 - (CO_HEAP_MAX * 8 + warps * 4 + 16) - 64;
-    const int max_cols = budget / 4;
-    int halves = (n_cols + max_cols - 1) / max_cols;
-    if (halves < 1) halves = 1;
-    const int cw = (n_cols + halves - 1) / halves;
-    int tw = (cw + warps - 1) / warps;
-    tw = (tw + 31) & ~31;
-    while ((int64_t)tw * warps > max_cols && tw > 32) tw -= 32;
-    halves = (int)(((int64_t)n_cols + tw * warps - 1) / (tw * warps));
-    geom->n_users = n_rows;
-    geom->n_items = n_cols;
-    geom->warps = warps;
-    geom->tile_cols = tw;
-    geom->n_halves = halves;
-    geom->n_subtiles = halves * warps;
-    geom->smem_bytes = co_smem_bytes(*geom);
-    geom->ctas_per_sm = CO_CTAS;
+    // 4-byte accumulators; the argtopn heap of the scoring kernel's rank mode is reserved in every geometry
+    tile_geometry(n_rows, n_cols, CO_WARPS, CO_CTAS, 4, CO_FIXED_SMEM, 64, geom);
     return LK_OK;
 }
 
@@ -499,10 +403,10 @@ int lk_cooc_pool_to_csr(const lk_cooc_args *args, const int64_t *d_out_indptr, i
     if (int rc = cooc_check(args, "lk_cooc_pool_to_csr")) return rc;
     LK_REQUIRE(d_out_indptr && d_out_cols && d_out_vals && args->d_pool_off && args->d_part_cnt, LK_ERR_INVALID,
                "lk_cooc_pool_to_csr: null pointer");
-    cooc_pool_to_csr_kernel<<<sm_count() * 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        *args, d_out_indptr, d_out_cols, static_cast<uint32_t *>(d_out_vals));
-    LK_CUDA_TRY(cudaGetLastError());
-    return LK_OK;
+    const lk_cooc_args &a = *args;
+    return launch_pool_to_csr(a.geom.n_items, a.geom.n_halves, a.d_pool_off, a.d_part_cnt, a.d_pool_cols,
+                              static_cast<const uint32_t *>(a.d_pool_vals), d_out_indptr, d_out_cols,
+                              static_cast<uint32_t *>(d_out_vals), stream);
 }
 
 int lk_cooc_diagonal(const lk_cooc_args *args, int64_t *d_diag, void *stream)

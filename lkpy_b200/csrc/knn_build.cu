@@ -28,16 +28,13 @@
 // slices (piece p of P: the p-th P-th of every warp's sub-tile) so that one hot
 // item cannot keep a single CTA busy longer than a GPU's fair share of the whole
 // build — a column split leaves every dots[j] with its full ascending-user sum
-// (a user split would change the rounding).
-//
-// Ordering inside a warp: the products of up to 32 users are flattened over the
-// lanes in (user, column) order and applied one user per round (the lanes of one
-// user hit distinct columns).
+// (a user split would change the rounding).  The users play the input rows of the
+// shared tile core (tiles.cuh).
 
 #include <algorithm>
 #include <cstdlib>
 
-#include "common.cuh"
+#include "tiles.cuh"
 
 namespace lk {
 
@@ -191,13 +188,9 @@ __global__ void __launch_bounds__(W * 32, 1024 / (W * 32)) knn_build_kernel(lk_k
     for (int idx = tid; idx < CW; idx += NT) acc[idx] = SENT;
     __syncthreads();
 
-    const int64_t n_work = a.n_work;
     for (;;) {
-        if (tid == 0) bc[8] = fetch_work(a.d_work_counter, a.d_cancel);
-        __syncthreads();
-        const int64_t wi = bc[8];
-        __syncthreads();
-        if (wi >= n_work) break;
+        const int64_t wi = cta_next_work(a.d_work_counter, a.d_cancel, bc + 8);
+        if (wi >= a.n_work) break;
         const int uid = a.d_sched[wi];
         const int4 un = __ldg(reinterpret_cast<const int4 *>(a.d_units) + uid);
         const int item = un.x, h = un.y;
@@ -206,11 +199,11 @@ __global__ void __launch_bounds__(W * 32, 1024 / (W * 32)) knn_build_kernel(lk_k
         // ------------------------------------------------------------------
         // accumulate: warp `warp` owns columns [col0, col0 + TW), of which this unit covers [jlo, jhi)
         // ------------------------------------------------------------------
+        const int s = h * W + warp;
+        const int col0 = s * TW;
+        uint32_t *my = acc + warp * TW;
         {
-            const int s = h * W + warp;
-            const int col0 = s * TW;
             const int jlo = un.z * pw, jhi = jlo + pw;
-            uint32_t *my = acc + warp * TW;
             const int iu0 = a.d_iu_indptr[item];
             const int m = a.d_iu_indptr[item + 1] - iu0;
             for (int t0 = 0; t0 < m; t0 += 32) {
@@ -223,49 +216,23 @@ __global__ void __launch_bounds__(W * 32, 1024 / (W * 32)) knn_build_kernel(lk_k
                     base = __ldg(tp);
                     len = __ldg(tp + 1) - base;
                 }
-                const int incl = warp_incl_scan(len, lane);
-                const int total = __shfl_sync(FULL, incl, 31);
-                const int adj = base - (incl - len);  // source index = adj[owner] + e
-                for (int e0 = 0; e0 < total; e0 += 32) {
-                    const int e = e0 + lane;
-                    bool valid = e < total;
-                    int q = 0;  // owner: smallest lane with incl > e
-#pragma unroll
-                    for (int step = 16; step > 0; step >>= 1) {
-                        const int t = __shfl_sync(FULL, incl, q + step - 1);
-                        if (t <= e) q += step;
-                    }
-                    q = min(q, 31);
-                    const int src = __shfl_sync(FULL, adj, q) + e;
-                    const float rq = __shfl_sync(FULL, r, q);
+                warp_walk_segments(base, len, lane, [&](bool valid, int own, int src) {
+                    const float rq = __shfl_sync(FULL, r, own);
                     int j = 0;
                     float prod = 0.0f;
                     if (valid) {
                         const int col = __ldg(a.d_ui_cols + src);
-                        const float val = __ldg(a.d_ui_vals + src);
-                        prod = __fmul_rn(rq, val);  // never contracted (item_train.rs:128)
+                        prod = __fmul_rn(rq, __ldg(a.d_ui_vals + src));  // never contracted (item_train.rs:128)
                         j = col - col0;
                         // diagonal excluded by index (item_train.rs:120-122); columns of other pieces are not ours
                         valid = col != item && j >= jlo && j < jhi;
                     }
-                    // users in ascending order, one user per round: the lanes of one user hit distinct columns.
-                    // (Grouping lanes by column instead — __match_any_sync, or one ballot per column bit — was
-                    // measured slower on ML-25M-shaped data: a popular column is present in most users'
-                    // segments, so the rounds per batch stay near the number of users.)
-                    unsigned pend = __ballot_sync(FULL, valid);
-                    while (pend) {
-                        const int leader = __ffs(pend) - 1;
-                        const int qq = __shfl_sync(FULL, q, leader);
-                        const bool mine = valid && q == qq;
-                        if (mine) {
-                            const uint32_t old = my[j];
-                            const float b = old == SENT ? 0.0f : __uint_as_float(old);
-                            my[j] = __float_as_uint(__fadd_rn(b, prod));
-                        }
-                        __syncwarp();
-                        pend &= ~__ballot_sync(FULL, mine);
-                    }
-                }
+                    warp_apply_in_owner_order(valid, own, [&] {
+                        const uint32_t old = my[j];
+                        const float b = old == SENT ? 0.0f : __uint_as_float(old);
+                        my[j] = __float_as_uint(__fadd_rn(b, prod));
+                    });
+                });
             }
         }
         __syncthreads();
@@ -273,8 +240,16 @@ __global__ void __launch_bounds__(W * 32, 1024 / (W * 32)) knn_build_kernel(lk_k
         // ------------------------------------------------------------------
         // epilogue: threshold, (top-K | all), emit, reset accumulators
         // ------------------------------------------------------------------
-        const int half_col0 = h * CW;
         const int64_t pidx = uid;  // partial lists / pool segments are indexed by unit
+        if (K <= 0) {  // unbounded: all candidates, in column order, into the pool
+            cta_emit_pool_segment<W>(
+                my, TW, col0, pidx, [&](uint32_t bits, int) { return is_cand(bits, min_sim); },
+                [](uint32_t bits, int) { return bits; }, SENT, wsum, a.d_pool_cursor, a.pool_capacity, a.d_status,
+                a.d_pool_off, a.d_part_cnt, a.d_pool_cols, reinterpret_cast<uint32_t *>(a.d_pool_vals));
+            continue;
+        }
+
+        const int half_col0 = h * CW;
         // candidate count
         int local = 0;
         for (int idx = tid; idx < CW; idx += NT) local += is_cand(acc[idx], min_sim) ? 1 : 0;
@@ -289,47 +264,6 @@ __global__ void __launch_bounds__(W * 32, 1024 / (W * 32)) knn_build_kernel(lk_k
         int n_cand = 0;
         for (int w = 0; w < W; w++) n_cand += wsum[w];
         __syncthreads();
-
-        if (K <= 0) {
-            // unbounded: all candidates, in column order, into the pool
-            if (tid == 0) {
-                unsigned long long off = atomicAdd(a.d_pool_cursor, (unsigned long long)n_cand);
-                if (off + (unsigned long long)n_cand > (unsigned long long)a.pool_capacity) {
-                    atomicCAS(a.d_status, 0, 1);
-                    off = ~0ull;
-                }
-                reinterpret_cast<unsigned long long *>(bc)[0] = off;
-                a.d_pool_off[pidx] = (int64_t)off;
-                a.d_part_cnt[pidx] = n_cand;
-            }
-            __syncthreads();
-            const unsigned long long off = reinterpret_cast<unsigned long long *>(bc)[0];
-            // contiguous column range per thread keeps column order
-            const int per = (CW + NT - 1) / NT;
-            const int c_lo = min(CW, tid * per), c_hi = min(CW, c_lo + per);
-            int cnt = 0;
-            for (int c = c_lo; c < c_hi; c++) cnt += is_cand(acc[c], min_sim) ? 1 : 0;
-            const int incl = warp_incl_scan(cnt, lane);
-            if (lane == 31) wsum[warp] = incl;
-            __syncthreads();
-            int woff = 0;
-            for (int w = 0; w < warp; w++) woff += wsum[w];
-            int pos = woff + incl - cnt;
-            if (off != ~0ull) {
-                for (int c = c_lo; c < c_hi; c++) {
-                    const uint32_t bits = acc[c];
-                    if (is_cand(bits, min_sim)) {
-                        a.d_pool_cols[off + pos] = half_col0 + c;
-                        a.d_pool_vals[off + pos] = __uint_as_float(bits);
-                        pos++;
-                    }
-                }
-            }
-            __syncthreads();
-            for (int idx = tid; idx < CW; idx += NT) acc[idx] = SENT;
-            __syncthreads();
-            continue;
-        }
 
         int32_t *pc = a.d_part_cols + pidx * K;
         float *pv = a.d_part_vals + pidx * K;
@@ -518,22 +452,9 @@ __global__ void __launch_bounds__(128) knn_merge_kernel(lk_knn_build_args a, int
     }
 }
 
-__global__ void pool_to_csr_kernel(lk_knn_build_args a, const int64_t *__restrict__ out_indptr,
-                                   int32_t *__restrict__ out_cols, float *__restrict__ out_vals)
-{
-    const int warps = (gridDim.x * blockDim.x) >> 5;
-    const int lane = threadIdx.x & 31;
-    for (int item = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; item < a.geom.n_items; item += warps) {
-        // unbounded mode has one unit per (item, half), in column order
-        warp_copy_pool_segments(a.d_unit_ptr[item], a.d_unit_ptr[item + 1], a.d_pool_off, a.d_part_cnt,
-                                a.d_pool_cols, a.d_pool_vals, out_indptr[item], out_cols, out_vals, lane);
-    }
-}
-
-static int knn_smem_bytes(const lk_knn_geom &g)
-{
-    return g.warps * g.tile_cols * 4 + HIST_BINS * 4 + 16 * 4 + g.warps * 4 + 16;
-}
+// shared memory besides the accumulators: radix histogram, broadcast slots, per-warp sums
+static int knn_fixed_smem(int warps) { return HIST_BINS * 4 + 16 * 4 + warps * 4 + 16; }
+static int knn_smem_bytes(const lk_knn_geom &g) { return g.warps * g.tile_cols * 4 + knn_fixed_smem(g.warps); }
 
 }  // namespace lk
 
@@ -550,24 +471,7 @@ int lk_knn_geometry(int32_t n_users, int32_t n_items, lk_knn_geom *geom)
     if (options().knn_ctas > 0) ctas = options().knn_ctas;
     LK_REQUIRE(warps == 8 || warps == 16 || warps == 32, LK_ERR_INVALID, "LK_KNN_WARPS must be 8, 16 or 32");
     LK_REQUIRE(ctas >= 1 && ctas <= 8, LK_ERR_INVALID, "LK_KNN_CTAS must be 1..8");
-    // shared memory budget per CTA (227 KB usable per SM, 1 KB reserved per CTA)
-    const int budget = (227 * 1024) / ctas - 1024 - (HIST_BINS * 4 + 16 * 4 + warps * 4 + 16);
-    const int max_cols = budget / 4;
-    int halves = (n_items + max_cols - 1) / max_cols;
-    if (halves < 1) halves = 1;
-    int cw = (n_items + halves - 1) / halves;
-    int tw = (cw + warps - 1) / warps;
-    tw = (tw + 31) & ~31;
-    while ((int64_t)tw * warps > max_cols && tw > 32) tw -= 32;
-    halves = (n_items + tw * warps - 1) / (tw * warps);
-    geom->n_users = n_users;
-    geom->n_items = n_items;
-    geom->warps = warps;
-    geom->tile_cols = tw;
-    geom->n_halves = halves;
-    geom->n_subtiles = halves * warps;
-    geom->smem_bytes = knn_smem_bytes(*geom);
-    geom->ctas_per_sm = ctas;
+    tile_geometry(n_users, n_items, warps, ctas, 4, knn_fixed_smem(warps), 0, geom);
     return LK_OK;
 }
 
@@ -666,10 +570,10 @@ int lk_knn_pool_to_csr(const lk_knn_build_args *args, const int64_t *d_out_indpt
                        float *d_out_vals, void *stream)
 {
     LK_REQUIRE(args && d_out_indptr && d_out_cols && d_out_vals, LK_ERR_INVALID, "lk_knn_pool_to_csr: null");
-    pool_to_csr_kernel<<<sm_count() * 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(*args, d_out_indptr,
-                                                                                   d_out_cols, d_out_vals);
-    LK_CUDA_TRY(cudaGetLastError());
-    return LK_OK;
+    // the unbounded build has one unit per (item, half), item-major and in column order
+    const lk_knn_build_args &a = *args;
+    return launch_pool_to_csr(a.geom.n_items, a.geom.n_halves, a.d_pool_off, a.d_part_cnt, a.d_pool_cols,
+                              a.d_pool_vals, d_out_indptr, d_out_cols, d_out_vals, stream);
 }
 
 }  // extern "C"

@@ -8,29 +8,27 @@
 // f64 multiply, then an add, no FMA, from +0.0.  Items outside the query only add +-0.0, which cannot
 // change a nonzero sum, so sim(q, v) is exactly the sequence
 //   acc[v] = acc[v] + VT[i, v] * x[i]      for the query's items i ascending,
-// each step rounded on its own (__dmul_rn / __dadd_rn; nvcc would otherwise contract to DFMA).  The
-// structure is the item-kNN build's (knn_build.cu) with the roles swapped: the query's items play the
-// build's users, VT rows play UI rows, and one warp owns a contiguous user sub-tile of f64 accumulators
-// in shared memory, so every accumulator receives all its additions from one warp in ascending item
-// order.  The threshold is compared in f64 (a sim just above min_sim whose f32 cast falls below it is
-// kept, as in the reference).
+// each step rounded on its own (__dmul_rn / __dadd_rn; nvcc would otherwise contract to DFMA).  This is the
+// shared tile core (tiles.cuh) over f64 accumulators: the query's items, ascending, are the input rows and
+// their VT rows the segments, so every accumulator receives all its additions in ascending item order.  The
+// threshold is compared in f64 (a sim just above min_sim whose f32 cast falls below it is kept, as in the
+// reference).
 //
 // Work units are (query, user tile), handed out most-expensive-first from an atomic counter by a
-// persistent grid.  After a unit's products, each warp scans its own sub-tile 32 accumulators at a time
-// (ballot + popcount keep user order), the CTA bump-allocates one pool segment for the unit, the warps
-// write their survivors into it and reset the accumulators.  The scan visits every accumulator of the
-// tile: at the ML-25M shape a median query makes ~4x more products per tile than the tile has users and
-// ~40 % of all users are neighbours, so tracking touched words would skip little; a unit with no
-// products at all (no item of the query reaches the tile) skips the scan.
+// persistent grid.  The pool epilogue visits every accumulator of the tile: at the ML-25M shape a median
+// query makes ~4x more products per tile than the tile has users and ~40 % of all users are neighbours, so
+// tracking touched words would skip little; a unit with no products at all (no item of the query reaches
+// the tile) skips it.
 
 #include <algorithm>
 
-#include "common.cuh"
+#include "tiles.cuh"
 
 namespace lk {
 
 constexpr int UKNN_WARPS = 16;
 constexpr int UKNN_NT = UKNN_WARPS * 32;
+constexpr int UKNN_FIXED_SMEM = UKNN_WARPS * 4 + 16;  // per-warp counts
 
 __global__ void uknn_query_cost_kernel(lk_uknn_search_args a, int64_t *__restrict__ cost)
 {
@@ -52,8 +50,7 @@ __global__ void __launch_bounds__(UKNN_NT, 2) uknn_search_kernel(lk_uknn_search_
 {
     constexpr int W = UKNN_WARPS;
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    __shared__ int64_t s_work;
-    __shared__ unsigned long long s_off;
+    __shared__ int s_work;
     const lk_knn_geom &g = a.geom;
     const int TW = g.tile_cols, S1 = g.n_subtiles + 1, H = g.n_halves;
     const int CW = W * TW;
@@ -67,10 +64,7 @@ __global__ void __launch_bounds__(UKNN_NT, 2) uknn_search_kernel(lk_uknn_search_
     __syncthreads();
 
     for (;;) {
-        if (tid == 0) s_work = fetch_work(a.d_work_counter, nullptr);
-        __syncthreads();
-        const int64_t wi = s_work;
-        __syncthreads();
+        const int64_t wi = cta_next_work(a.d_work_counter, nullptr, &s_work);
         if (wi >= a.n_work) break;
         const int unit = a.d_sched[wi];
         const int q = unit / H, h = unit - q * H;
@@ -78,10 +72,7 @@ __global__ void __launch_bounds__(UKNN_NT, 2) uknn_search_kernel(lk_uknn_search_
         const int col0 = s * TW;
         double *my = acc + warp * TW;
 
-        // ------------------------------------------------------------------
-        // products: the query's items in ascending order, 32 at a time flattened over the lanes for the
-        // loads, applied one item per round (the lanes of one item hit distinct users)
-        // ------------------------------------------------------------------
+        // products: the query's items in ascending order play the input rows
         const int64_t q0 = a.d_q_begin[q];
         const int m = (int)(a.d_q_end[q] - q0);
         bool any = false;
@@ -95,21 +86,7 @@ __global__ void __launch_bounds__(UKNN_NT, 2) uknn_search_kernel(lk_uknn_search_
                 base = __ldg(tp);
                 len = __ldg(tp + 1) - base;
             }
-            const int incl = warp_incl_scan(len, lane);
-            const int total = __shfl_sync(FULL, incl, 31);
-            any |= total > 0;
-            const int adj = base - (incl - len);  // source index = adj[owner] + e
-            for (int e0 = 0; e0 < total; e0 += 32) {
-                const int e = e0 + lane;
-                const bool valid = e < total;
-                int own = 0;  // owner: smallest lane with incl > e
-#pragma unroll
-                for (int step = 16; step > 0; step >>= 1) {
-                    const int t = __shfl_sync(FULL, incl, own + step - 1);
-                    if (t <= e) own += step;
-                }
-                own = min(own, 31);
-                const int src = __shfl_sync(FULL, adj, own) + e;
+            any |= warp_walk_segments(base, len, lane, [&](bool valid, int own, int src) {
                 const double xq = __shfl_sync(FULL, x, own);
                 int j = 0;
                 double prod = 0.0;
@@ -117,16 +94,8 @@ __global__ void __launch_bounds__(UKNN_NT, 2) uknn_search_kernel(lk_uknn_search_
                     j = __ldg(a.d_vt_users + src) - col0;
                     prod = __dmul_rn(__ldg(a.d_vt_vals + src), xq);  // VT[i,v] * x[i], never contracted
                 }
-                unsigned pend = __ballot_sync(FULL, valid);
-                while (pend) {
-                    const int leader = __ffs(pend) - 1;
-                    const int oo = __shfl_sync(FULL, own, leader);
-                    const bool mine = valid && own == oo;
-                    if (mine) my[j] = __dadd_rn(my[j], prod);
-                    __syncwarp();
-                    pend &= ~__ballot_sync(FULL, mine);
-                }
-            }
+                warp_apply_in_owner_order(valid, own, [&] { my[j] = __dadd_rn(my[j], prod); });
+            });
         }
         if (!__syncthreads_or(any)) {  // no item of the query reaches this tile: every accumulator is still +0.0
             if (tid == 0) {
@@ -136,63 +105,17 @@ __global__ void __launch_bounds__(UKNN_NT, 2) uknn_search_kernel(lk_uknn_search_
             continue;
         }
 
-        // ------------------------------------------------------------------
-        // epilogue: count, one pool segment per unit, write in user order, reset
-        // ------------------------------------------------------------------
+        // epilogue: one pool segment per unit in user order; the threshold is compared in f64, and the kept sims
+        // are rounded to nearest, as NumPy's astype(float32)
         const int self = a.d_q_self != nullptr ? a.d_q_self[q] : -1;
-        int cnt = 0;
-        for (int c0 = 0; c0 < TW; c0 += 32) {
-            const int v = col0 + c0 + lane;
-            const bool keep = my[c0 + lane] >= min_sim && v != self;
-            cnt += __popc(__ballot_sync(FULL, keep));
-        }
-        if (lane == 0) wcnt[warp] = cnt;
-        __syncthreads();
-        if (tid == 0) {
-            int n = 0;
-            for (int w = 0; w < W; w++) n += wcnt[w];
-            unsigned long long off = atomicAdd(a.d_pool_cursor, (unsigned long long)n);
-            if (off + (unsigned long long)n > (unsigned long long)a.pool_capacity) {
-                atomicCAS(a.d_status, 0, 1);
-                off = ~0ull;
-            }
-            s_off = off;
-            a.d_pool_off[unit] = (int64_t)off;
-            a.d_part_cnt[unit] = n;
-        }
-        __syncthreads();
-        const unsigned long long off = s_off;
-        int pos = 0;
-        for (int w = 0; w < warp; w++) pos += wcnt[w];
-        for (int c0 = 0; c0 < TW; c0 += 32) {
-            const int v = col0 + c0 + lane;
-            const double sim = my[c0 + lane];
-            const bool keep = sim >= min_sim && v != self;
-            const unsigned b = __ballot_sync(FULL, keep);
-            if (keep && off != ~0ull) {
-                const unsigned long long k = off + pos + __popc(b & ((1u << lane) - 1u));
-                a.d_pool_rows[k] = v;
-                a.d_pool_sims[k] = (float)sim;  // round to nearest, as NumPy's astype(float32)
-            }
-            pos += __popc(b);
-            my[c0 + lane] = 0.0;
-        }
-        __syncthreads();  // wcnt and s_off are rewritten by the next unit
+        cta_emit_pool_segment<W>(
+            my, TW, col0, unit, [&](double sim, int v) { return sim >= min_sim && v != self; },
+            [](double sim, int) { return __float_as_uint((float)sim); }, 0.0, wcnt, a.d_pool_cursor, a.pool_capacity,
+            a.d_status, a.d_pool_off, a.d_part_cnt, a.d_pool_rows, reinterpret_cast<uint32_t *>(a.d_pool_sims));
     }
 }
 
-__global__ void uknn_pool_to_csr_kernel(lk_uknn_search_args a, const int64_t *__restrict__ out_indptr,
-                                        int32_t *__restrict__ out_rows, float *__restrict__ out_sims)
-{
-    const int warps = (gridDim.x * blockDim.x) >> 5;
-    const int lane = threadIdx.x & 31;
-    const int64_t H = a.geom.n_halves;
-    for (int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; q < a.n_queries; q += warps)
-        warp_copy_pool_segments(q * H, (q + 1) * H, a.d_pool_off, a.d_part_cnt, a.d_pool_rows, a.d_pool_sims,
-                                out_indptr[q], out_rows, out_sims, lane);
-}
-
-static int uknn_smem_bytes(const lk_knn_geom &g) { return g.warps * g.tile_cols * 8 + g.warps * 4 + 16; }
+static int uknn_smem_bytes(const lk_knn_geom &g) { return g.warps * g.tile_cols * 8 + UKNN_FIXED_SMEM; }
 
 }  // namespace lk
 
@@ -203,27 +126,10 @@ extern "C" {
 int lk_uknn_geometry(int32_t n_users, int32_t n_items, int32_t ctas_per_sm, lk_knn_geom *geom)
 {
     LK_REQUIRE(geom != nullptr && n_users >= 1 && n_items >= 0, LK_ERR_INVALID, "lk_uknn_geometry: bad arguments");
-    const int warps = UKNN_WARPS;
     const int ctas = ctas_per_sm > 0 ? ctas_per_sm : 2;
     LK_REQUIRE(ctas <= 2, LK_ERR_INVALID, "lk_uknn_geometry: ctas_per_sm must be 0, 1 or 2");
-    // shared memory budget per CTA (227 KB usable per SM, 1 KB reserved per CTA), 8-byte accumulators
-    const int budget = (227 * 1024) / ctas - 1024 - (warps * 4 + 16) - 64;
-    const int max_cols = budget / 8;
-    int halves = (n_users + max_cols - 1) / max_cols;
-    if (halves < 1) halves = 1;
-    const int cw = (n_users + halves - 1) / halves;
-    int tw = (cw + warps - 1) / warps;
-    tw = (tw + 31) & ~31;
-    while ((int64_t)tw * warps > max_cols && tw > 32) tw -= 32;
-    halves = (n_users + tw * warps - 1) / (tw * warps);
-    geom->n_users = n_items;  // VT rows
-    geom->n_items = n_users;  // accumulator columns
-    geom->warps = warps;
-    geom->tile_cols = tw;
-    geom->n_halves = halves;
-    geom->n_subtiles = halves * warps;
-    geom->smem_bytes = uknn_smem_bytes(*geom);
-    geom->ctas_per_sm = ctas;
+    // 8-byte accumulators over the users; VT's rows (items) are the input rows
+    tile_geometry(n_items, n_users, UKNN_WARPS, ctas, 8, UKNN_FIXED_SMEM, 64, geom);
     return LK_OK;
 }
 
@@ -280,10 +186,9 @@ int lk_uknn_pool_to_csr(const lk_uknn_search_args *args, const int64_t *d_out_in
     if (args->n_queries == 0) return LK_OK;
     LK_REQUIRE(d_out_indptr && d_out_rows && d_out_sims && args->d_pool_off && args->d_part_cnt, LK_ERR_INVALID,
                "lk_uknn_pool_to_csr: null pointer");
-    uknn_pool_to_csr_kernel<<<sm_count() * 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(*args, d_out_indptr,
-                                                                                        d_out_rows, d_out_sims);
-    LK_CUDA_TRY(cudaGetLastError());
-    return LK_OK;
+    const lk_uknn_search_args &a = *args;
+    return launch_pool_to_csr(a.n_queries, a.geom.n_halves, a.d_pool_off, a.d_part_cnt, a.d_pool_rows, a.d_pool_sims,
+                              d_out_indptr, d_out_rows, d_out_sims, stream);
 }
 
 }  // extern "C"

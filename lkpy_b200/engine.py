@@ -404,32 +404,48 @@ class KnnBuildPlan:
         if capacity is None:
             # every kept pair shares a user: at most sum of the processed rows' product counts
             capacity = int(min(int(self.cost[rows.long()].sum().item()), rows.numel() * max(n_items - 1, 1)))
-        capacity = max(capacity, 1)
-        pool_cols = torch.empty(capacity, dtype=torch.int32, device=dev)
-        pool_vals = torch.empty(capacity, dtype=torch.float32, device=dev)
-        pool_off = torch.zeros(n_items * H, dtype=torch.int64, device=dev)
-        part_cnt = torch.zeros(n_items * H, dtype=torch.int32, device=dev)
         cursor = torch.zeros(1, dtype=torch.int64, device=dev)
         self.status.zero_()
         a = self._args(u, sched, min_sim, 0)
-        a.d_part_cnt = ptr(part_cnt)
-        a.d_pool_cols, a.d_pool_vals, a.pool_capacity = ptr(pool_cols), ptr(pool_vals), capacity
-        a.d_pool_off, a.d_pool_cursor = ptr(pool_off), ptr(cursor)
-        check(L.lk_knn_build(C.byref(a), stream_ptr()), "lk_knn_build")
-        if int(self.status.item()) == 1:
-            raise _lib.EngineError("similarity pool overflow; pass a larger capacity")
-        counts = part_cnt.view(n_items, H).sum(dim=1, dtype=torch.int64)
-        indptr = torch.zeros(n_items + 1, dtype=torch.int64, device=dev)
-        torch.cumsum(counts, 0, out=indptr[1:])
-        nnz = int(indptr[-1].item())
-        out_cols = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
-        out_vals = torch.empty(max(nnz, 1), dtype=torch.float32, device=dev)
-        check(
-            L.lk_knn_pool_to_csr(C.byref(a), ptr(indptr), ptr(out_cols), ptr(out_vals), stream_ptr()),
-            "lk_knn_pool_to_csr",
+
+        def launch(pool_cols, pool_vals, pool_off, part_cnt):
+            a.d_part_cnt = ptr(part_cnt)
+            a.d_pool_cols, a.d_pool_vals, a.pool_capacity = ptr(pool_cols), ptr(pool_vals), pool_cols.numel()
+            a.d_pool_off, a.d_pool_cursor = ptr(pool_off), ptr(cursor)
+            check(L.lk_knn_build(C.byref(a), stream_ptr()), "lk_knn_build")
+            return int(self.status.item())
+
+        def gather(indptr, cols, vals):
+            rc = L.lk_knn_pool_to_csr(C.byref(a), ptr(indptr), ptr(cols), ptr(vals), stream_ptr())
+            check(rc, "lk_knn_pool_to_csr")
+
+        return pool_to_csr(
+            dev, n_items, H, capacity, torch.float32, launch, gather, "similarity pool overflow; pass a larger capacity"
         )
-        torch.cuda.current_stream().synchronize()
-        return indptr, out_cols[:nnz], out_vals[:nnz]
+
+
+def pool_to_csr(dev, n_rows: int, units_per_row: int, capacity: int, vals_dtype, launch, gather, overflow: str):
+    """
+    The host side of a tiled kernel's bump pool (``tiles.cuh``): allocates a pool of ``capacity`` (at least 1)
+    entries and the per-unit segment offsets and counts of ``n_rows * units_per_row`` units, row-major;
+    ``launch(pool_cols, pool_vals, pool_off, part_cnt)`` runs the kernel and returns the status word, 1 raising
+    :class:`EngineError` with ``overflow``; ``gather(indptr, cols, vals)`` copies the segments, in unit order, into
+    the CSR.  Returns the device CSR (int64 indptr [n_rows + 1], int32 columns, values of ``vals_dtype``).
+    """
+    capacity = max(int(capacity), 1)
+    pool_cols = torch.empty(capacity, dtype=torch.int32, device=dev)
+    pool_vals = torch.empty(capacity, dtype=vals_dtype, device=dev)
+    pool_off = torch.zeros(n_rows * units_per_row, dtype=torch.int64, device=dev)
+    part_cnt = torch.zeros(n_rows * units_per_row, dtype=torch.int32, device=dev)
+    if launch(pool_cols, pool_vals, pool_off, part_cnt) == 1:
+        raise _lib.EngineError(overflow)
+    indptr = torch.zeros(n_rows + 1, dtype=torch.int64, device=dev)
+    torch.cumsum(part_cnt.view(n_rows, units_per_row).sum(dim=1, dtype=torch.int64), 0, out=indptr[1:])
+    nnz = int(indptr[-1].item())
+    cols = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
+    vals = torch.empty(max(nnz, 1), dtype=vals_dtype, device=dev)
+    gather(indptr, cols, vals)
+    return indptr, cols[:nnz], vals[:nnz]
 
 
 def topk_rows_to_csr(
@@ -857,8 +873,8 @@ class UserNeighbourState:
         if not min_sim > 0:
             raise ValueError("min_sim must be positive")
         dev, B, H = self.device, qs.n, self.geom.n_halves
-        indptr = torch.zeros(B + 1, dtype=torch.int64, device=dev)
         if B == 0:
+            indptr = torch.zeros(1, dtype=torch.int64, device=dev)
             return indptr, torch.empty(0, dtype=torch.int32, device=dev), torch.empty(0, dtype=torch.float32, device=dev)
         if B * H >= 2**31:
             raise _lib.EngineError(f"{B} queries x {H} user tiles exceed the work-unit numbering; split the batch")
@@ -869,26 +885,24 @@ class UserNeighbourState:
         sched = (order[:, None] * H + torch.arange(H, device=dev)[None, :]).reshape(-1).to(torch.int32)
         if capacity is None:
             capacity = int(cost.clamp_max(self.n_users).sum().item())
-        capacity = max(int(capacity), 1)
-        pool_rows = torch.empty(capacity, dtype=torch.int32, device=dev)
-        pool_sims = torch.empty(capacity, dtype=torch.float32, device=dev)
-        pool_off = torch.zeros(B * H, dtype=torch.int64, device=dev)
-        part_cnt = torch.zeros(B * H, dtype=torch.int32, device=dev)
-        with self.lock:  # work counter, cursor and status word are per state
-            a = self._args(qs, min_sim)
-            a.d_sched, a.n_work = ptr(sched), sched.numel()
-            a.d_pool_rows, a.d_pool_sims, a.pool_capacity = ptr(pool_rows), ptr(pool_sims), capacity
-            a.d_pool_off, a.d_part_cnt = ptr(pool_off), ptr(part_cnt)
-            check(L.lk_uknn_search(C.byref(a), stream_ptr()), "lk_uknn_search")
-            st = int(self.status.item())
-        if st == 1:
-            raise _lib.EngineError("lk_uknn_search: neighbour pool overflow; pass a larger capacity")
-        torch.cumsum(part_cnt.view(B, H).sum(dim=1, dtype=torch.int64), 0, out=indptr[1:])
-        nnz = int(indptr[-1].item())
-        rows = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
-        sims = torch.empty(max(nnz, 1), dtype=torch.float32, device=dev)
-        check(L.lk_uknn_pool_to_csr(C.byref(a), ptr(indptr), ptr(rows), ptr(sims), stream_ptr()), "lk_uknn_pool_to_csr")
-        return indptr, rows[:nnz], sims[:nnz]
+        a = self._args(qs, min_sim)
+        a.d_sched, a.n_work = ptr(sched), sched.numel()
+
+        def launch(pool_rows, pool_sims, pool_off, part_cnt):
+            with self.lock:  # work counter, cursor and status word are per state
+                a.d_pool_rows, a.d_pool_sims, a.pool_capacity = ptr(pool_rows), ptr(pool_sims), pool_rows.numel()
+                a.d_pool_off, a.d_part_cnt = ptr(pool_off), ptr(part_cnt)
+                check(L.lk_uknn_search(C.byref(a), stream_ptr()), "lk_uknn_search")
+                return int(self.status.item())
+
+        def gather(indptr, rows, sims):
+            rc = L.lk_uknn_pool_to_csr(C.byref(a), ptr(indptr), ptr(rows), ptr(sims), stream_ptr())
+            check(rc, "lk_uknn_pool_to_csr")
+
+        return pool_to_csr(
+            dev, B, H, capacity, torch.float32, launch, gather,
+            "lk_uknn_search: neighbour pool overflow; pass a larger capacity",
+        )  # fmt: skip
 
 
 # ---------------------------------------------------------------------------
@@ -1109,12 +1123,8 @@ class CoocPlan:
             units = units[(h[None, :] + 1) * CW > order[:, None] + 1]
         sched = units.reshape(-1).to(torch.int32).contiguous()
         width = (n - 1 - torch.arange(n, device=dev)) if not full_rows else torch.full((n,), n - 1, device=dev)
-        capacity = max(int(torch.minimum(cost, width).sum().item()), 1)  # a row has at most min(cost, width) entries
+        capacity = int(torch.minimum(cost, width).sum().item())  # a row has at most min(cost, width) entries
         max_cost = int(cost.max().item()) if n else 0
-        pool_cols = torch.empty(capacity, dtype=torch.int32, device=dev)
-        pool_vals = torch.empty(capacity, dtype=torch.int32, device=dev)
-        pool_off = torch.zeros(n * H, dtype=torch.int64, device=dev)
-        part_cnt = torch.zeros(n * H, dtype=torch.int32, device=dev)
         a = self._args(full_rows)
         if attach is not None:
             self.cancel = attach(self.work_counter, sched.numel())
@@ -1122,21 +1132,23 @@ class CoocPlan:
         a.method, a.d_item_count, a.damping = int(method), ptr(item_count), float(damping)
         a.max_row_cost = max_cost
         a.d_sched, a.n_work = ptr(sched), sched.numel()
-        a.d_pool_cols, a.d_pool_vals, a.pool_capacity = ptr(pool_cols), ptr(pool_vals), capacity
-        a.d_pool_off, a.d_part_cnt = ptr(pool_off), ptr(part_cnt)
-        check(lib().lk_cooc_count(C.byref(a), stream_ptr()), "lk_cooc_count")
-        if int(self.status.item()) == 1:
-            raise _lib.EngineError("lk_cooc_count: pool overflow")
-        indptr = torch.zeros(n + 1, dtype=torch.int64, device=dev)
-        torch.cumsum(part_cnt.view(n, H).sum(dim=1, dtype=torch.int64), 0, out=indptr[1:])
-        nnz = int(indptr[-1].item())
-        cols = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
-        vals = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
-        check(lib().lk_cooc_pool_to_csr(C.byref(a), ptr(indptr), ptr(cols), ptr(vals), stream_ptr()), "lk_cooc_pool_to_csr")
-        torch.cuda.current_stream().synchronize()
+
+        def launch(pool_cols, pool_vals, pool_off, part_cnt):
+            a.d_pool_cols, a.d_pool_vals, a.pool_capacity = ptr(pool_cols), ptr(pool_vals), pool_cols.numel()
+            a.d_pool_off, a.d_part_cnt = ptr(pool_off), ptr(part_cnt)
+            check(lib().lk_cooc_count(C.byref(a), stream_ptr()), "lk_cooc_count")
+            return int(self.status.item())
+
+        def gather(indptr, cols, vals):
+            rc = lib().lk_cooc_pool_to_csr(C.byref(a), ptr(indptr), ptr(cols), ptr(vals), stream_ptr())
+            check(rc, "lk_cooc_pool_to_csr")
+
+        indptr, cols, vals = pool_to_csr(
+            dev, n, H, capacity, torch.int32, launch, gather, "lk_cooc_count: pool overflow"
+        )
         if method != _lib.LK_COOC_COUNT:
             vals = vals.view(torch.float32)
-        return indptr, cols[:nnz], vals[:nnz]
+        return indptr, cols, vals
 
     def diagonal(self) -> torch.Tensor:
         """``sum_g #i (#i + 1) / 2`` for every item (int32 [n_items]); a count of 2**31 or more raises."""

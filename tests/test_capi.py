@@ -103,6 +103,97 @@ def test_knn_geometry(cuda_lib, lk_options):
     assert cuda_lib.lk_set_option(b"LK_NO_SUCH_SWITCH", 1) != _lib.LK_OK
 
 
+# (n_users, n_items) -> every lk_knn_geom field (n_users, n_items, warps, tile_cols, n_halves, n_subtiles,
+# smem_bytes, ctas_per_sm) of lk_knn_geometry(n_users, n_items), lk_uknn_geometry(n_users, n_items, ctas) for
+# ctas 0, 1, 2, and lk_cooc_geometry(n_users, n_items), from one to a few hundred column tiles
+GEOMETRIES = {
+    (1_000, 1): (
+        [1000, 1, 16, 32, 1, 16, 10384, 2],
+        [[1, 1000, 16, 64, 1, 16, 8272, 2], [1, 1000, 16, 64, 1, 16, 8272, 1], [1, 1000, 16, 64, 1, 16, 8272, 2]],
+        [1000, 1, 16, 32, 1, 16, 10320, 2],
+    ),
+    (610, 9_724): (
+        [610, 9724, 16, 608, 1, 16, 47248, 2],
+        [[9724, 610, 16, 64, 1, 16, 8272, 2], [9724, 610, 16, 64, 1, 16, 8272, 1], [9724, 610, 16, 64, 1, 16, 8272, 2]],
+        [610, 9724, 16, 608, 1, 16, 47184, 2],
+    ),
+    (162_541, 59_047): (
+        [162541, 59047, 16, 1248, 3, 48, 88208, 2],
+        [
+            [59047, 162541, 16, 864, 12, 192, 110672, 2],
+            [59047, 162541, 16, 1696, 6, 96, 217168, 1],
+            [59047, 162541, 16, 864, 12, 192, 110672, 2],
+        ],
+        [162541, 59047, 16, 1248, 3, 48, 88144, 2],
+    ),
+    (100, 28_000): (
+        [100, 28000, 16, 896, 2, 32, 65680, 2],
+        [
+            [28000, 100, 16, 32, 1, 16, 4176, 2],
+            [28000, 100, 16, 32, 1, 16, 4176, 1],
+            [28000, 100, 16, 32, 1, 16, 4176, 2],
+        ],
+        [100, 28000, 16, 896, 2, 32, 65616, 2],
+    ),
+    (59_047, 162_541): (
+        [59047, 162541, 16, 1472, 7, 112, 102544, 2],
+        [
+            [162541, 59047, 16, 768, 5, 80, 98384, 2],
+            [162541, 59047, 16, 1248, 3, 48, 159824, 1],
+            [162541, 59047, 16, 768, 5, 80, 98384, 2],
+        ],
+        [59047, 162541, 16, 1472, 7, 112, 102480, 2],
+    ),
+    (5_000, 500_000): (
+        [5000, 500000, 16, 1664, 19, 304, 114832, 2],
+        [
+            [500000, 5000, 16, 320, 1, 16, 41040, 2],
+            [500000, 5000, 16, 320, 1, 16, 41040, 1],
+            [500000, 5000, 16, 320, 1, 16, 41040, 2],
+        ],
+        [5000, 500000, 16, 1664, 19, 304, 114768, 2],
+    ),
+    (7, 3_000_000): (
+        [7, 3000000, 16, 1664, 113, 1808, 114832, 2],
+        [
+            [3000000, 7, 16, 32, 1, 16, 4176, 2],
+            [3000000, 7, 16, 32, 1, 16, 4176, 1],
+            [3000000, 7, 16, 32, 1, 16, 4176, 2],
+        ],
+        [7, 3000000, 16, 1664, 113, 1808, 114768, 2],
+    ),
+    (3_000_000, 20): (
+        [3000000, 20, 16, 32, 1, 16, 10384, 2],
+        [
+            [20, 3000000, 16, 896, 210, 3360, 114768, 2],
+            [20, 3000000, 16, 1792, 105, 1680, 229456, 1],
+            [20, 3000000, 16, 896, 210, 3360, 114768, 2],
+        ],
+        [3000000, 20, 16, 32, 1, 16, 10320, 2],
+    ),
+}
+
+
+@pytest.mark.parametrize("shape", list(GEOMETRIES))
+def test_tile_geometries_are_pinned(cuda_lib, lk_options, shape):
+    lk_options("LK_KNN_WARPS", -1)  # the built-in choices, whatever the environment says
+    lk_options("LK_KNN_CTAS", -1)
+    n_users, n_items = shape
+    want_knn, want_uknn, want_cooc = GEOMETRIES[shape]
+    g = _lib.LkKnnGeom()
+
+    def fields():
+        return [getattr(g, f) for f, _ in _lib.LkKnnGeom._fields_]
+
+    _lib.check(cuda_lib.lk_knn_geometry(n_users, n_items, C.byref(g)))
+    assert fields() == want_knn
+    for ctas, want in enumerate(want_uknn):
+        _lib.check(cuda_lib.lk_uknn_geometry(n_users, n_items, ctas, C.byref(g)))
+        assert fields() == want, ctas
+    _lib.check(cuda_lib.lk_cooc_geometry(n_users, n_items, C.byref(g)))
+    assert fields() == want_cooc
+
+
 def test_component_configs():
     from lkpy_b200.als import BiasedMFScorer, ImplicitMFScorer
     from lkpy_b200.knn import ItemKNNConfig, ItemKNNScorer

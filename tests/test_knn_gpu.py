@@ -124,6 +124,18 @@ def test_build_row_subset(cuda_lib, ml_small):
     assert got[:1000].nnz == 0 and got[3000:].nnz == 0
 
 
+def test_build_unbounded_pool_overflow_is_reported(cuda_lib, ml_small):
+    """A similarity pool too small for the kept pairs raises instead of returning a truncated matrix, and the
+    plan builds the whole matrix afterwards."""
+    ui, iu, _ = data.knn_item_matrices(ml_small, True)
+    dev = _lib.require_device()
+    plan = engine.KnnBuildPlan.create(engine.DeviceCSR.from_host(ui, dev), engine.DeviceCSR.from_host(iu, dev))
+    with pytest.raises(_lib.EngineError, match="overflow"):
+        plan.build_unbounded(1e-6, capacity=3)
+    indptr, _c, _v = plan.build_unbounded(1e-6)
+    assert int(indptr[-1]) == 8_780_790
+
+
 def _score_gpu(S, queries, max_nbrs, min_nbrs, explicit=True):
     dev = _lib.require_device()
     st = engine.KnnScorerState.create(S.shape[0], S.indptr, S.indices, S.data, dev)
