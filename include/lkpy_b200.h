@@ -19,6 +19,7 @@
  *   ALS scorer + TopNRanker (score_matrix/recommend_batch) src/lenskit/als/_common.py:133-175 lk_als_recommend_batch
  *   _accel.data.count_cooc / dense_cooc           src/accel/data/cooc.rs:49-214     lk_cooc_count (+ _diagonal, _dense)
  *   AssociationScorer.train / __call__            src/lenskit/knn/association.py    lk_cooc_count (LK_ASSOC_*), lk_assoc_score_batch
+ *   EASEScorer.__call__ (q_vec @ weights)         src/lenskit/knn/ease.py           lk_ease_score_batch
  *
  * Conventions
  *   - plain C: pointers and sizes only; no C++/torch types cross this boundary;
@@ -545,6 +546,34 @@ typedef struct lk_assoc_score_args {
 } lk_assoc_score_args;
 
 LK_API int lk_assoc_score_batch(const lk_assoc_score_args *args, void *stream);
+
+/* ------------------------------------------------------------------------
+ * EASE scoring (ease.cu): EASEScorer.__call__ (src/lenskit/knn/ease.py), `q_vec @ weights` with a 0/1 query
+ * vector, batched, and its composition with TrainingItemsCandidateSelector and TopNRanker.  W is the dense
+ * f32 weight matrix [n_items][n_items], row-major.  For query q with history H_q = d_hist_items[
+ * d_hist_indptr[q] .. d_hist_indptr[q+1]) (ascending, no repeats, all in [0, n_items)) and item j:
+ *     s = +0.0f;  for h in H_q in order: s = s + W[h][j]      (f32 adds, round to nearest)
+ *   H_q empty: every score is NaN (score mode), an empty list (rank mode).
+ *   n == 0  score mode: d_scores [n_queries][n_items].
+ *   n >= 1  rank mode (n <= lk_topn_max()): argtopn over every item ascending minus the query's excluded items
+ *           (ascending within a query), ties included; outputs as lk_assoc_score_batch's rank mode.
+ * n_queries * ceil(n_items / 1024) < 2^31.
+ * ---------------------------------------------------------------------- */
+typedef struct lk_ease_score_args {
+    int32_t n_items;
+    const float *d_w;                  /* [n_items][n_items] */
+    int32_t n_queries;
+    const int64_t *d_hist_indptr;      /* [n_queries+1] */
+    const int32_t *d_hist_items;
+    int32_t n;                         /* 0: score mode; 1..lk_topn_max(): rank mode */
+    float *d_scores;                   /* score mode: [n_queries][n_items] */
+    const int64_t *d_excl_indptr;      /* rank mode: [n_queries+1] or NULL */
+    const int32_t *d_excl_items;
+    int32_t *d_out_idx; float *d_out_val; /* rank mode: [n_queries * n] */
+    int32_t *d_out_cnt;                /* rank mode: [n_queries] */
+} lk_ease_score_args;
+
+LK_API int lk_ease_score_batch(const lk_ease_score_args *args, void *stream);
 
 #ifdef __cplusplus
 }

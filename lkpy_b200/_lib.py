@@ -248,6 +248,23 @@ class LkAssocScoreArgs(C.Structure):
     ]
 
 
+class LkEaseScoreArgs(C.Structure):
+    _fields_ = [
+        ("n_items", C.c_int32),
+        ("d_w", vp),
+        ("n_queries", C.c_int32),
+        ("d_hist_indptr", vp),
+        ("d_hist_items", vp),
+        ("n", C.c_int32),
+        ("d_scores", vp),
+        ("d_excl_indptr", vp),
+        ("d_excl_items", vp),
+        ("d_out_idx", vp),
+        ("d_out_val", vp),
+        ("d_out_cnt", vp),
+    ]
+
+
 #: every symbol ``include/lkpy_b200.h`` declares: name -> (restype, argtypes)
 SYMBOLS: dict[str, tuple] = {
     "lk_version": (C.c_int, []),
@@ -290,6 +307,7 @@ SYMBOLS: dict[str, tuple] = {
     "lk_cooc_dense": (C.c_int, [C.c_int32, vp, vp, vp, vp, vp, vp]),
     "lk_assoc_tile_pointers": (C.c_int, [C.POINTER(LkKnnGeom), vp, vp, vp, vp]),
     "lk_assoc_score_batch": (C.c_int, [C.POINTER(LkAssocScoreArgs), vp]),
+    "lk_ease_score_batch": (C.c_int, [C.POINTER(LkEaseScoreArgs), vp]),
 }
 
 _lib = None

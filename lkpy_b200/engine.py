@@ -17,8 +17,8 @@ import torch
 
 from . import _lib
 from ._lib import (
-    LkAlsArgs, LkAlsRecArgs, LkAssocScoreArgs, LkCoocArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs,
-    LkUknnSearchArgs, check, lib, ptr, stream_ptr,
+    LkAlsArgs, LkAlsRecArgs, LkAssocScoreArgs, LkCoocArgs, LkEaseScoreArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs,
+    LkKnnScoreArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr,
 )  # fmt: skip
 from .data import InteractionCSR
 
@@ -1248,4 +1248,90 @@ class AssocState:
         a.d_excl_indptr, a.d_excl_items = ptr(excl_indptr), ptr(excl_items)
         a.d_out_idx, a.d_out_val, a.d_out_cnt = ptr(idx), ptr(val), ptr(cnt)
         check(lib().lk_assoc_score_batch(C.byref(a), stream_ptr()), "lk_assoc_score_batch")
+        return idx, val, cnt[:B]
+
+
+# ---------------------------------------------------------------------------
+# EASE scoring
+# ---------------------------------------------------------------------------
+
+
+def ease_histories(hists: list[np.ndarray], dev) -> tuple[torch.Tensor, torch.Tensor]:
+    """The batch's histories as ``lk_ease_score_batch`` takes them: a device CSR (int64 offsets, int32 items), each
+    history deduplicated and ascending (``q_vec[q_good] = 1.0`` counts a repeated item once)."""
+    hs = [np.unique(np.asarray(h, dtype=np.int64)).astype(np.int32) for h in hists]
+    indptr = np.zeros(len(hs) + 1, dtype=np.int64)
+    np.cumsum([len(h) for h in hs], out=indptr[1:])
+    items = np.concatenate(hs) if hs else np.zeros(0, np.int32)
+    return torch.from_numpy(indptr).to(dev), torch.from_numpy(items).to(dev)
+
+
+@dataclass
+class EaseState:
+    """The EASE weight matrix in HBM (f32 [n_items, n_items], row-major).  Read-only once built: every call
+    allocates its own outputs, so concurrent callers need no lock."""
+
+    weights: torch.Tensor
+
+    @property
+    def n_items(self) -> int:
+        return int(self.weights.shape[0])
+
+    @classmethod
+    def create(cls, weights, device=None) -> "EaseState":
+        device = device or _lib.require_device()
+        w = torch.as_tensor(weights).to(device=device, dtype=torch.float32).contiguous()
+        if w.dim() != 2 or w.shape[0] != w.shape[1] or w.shape[0] < 1:
+            raise ValueError("EASE weights must be a non-empty square matrix")
+        if w.shape[0] >= 2**31:
+            raise _lib.EngineError("EASE with 2**31 or more items is not supported")
+        return cls(w)
+
+    def _args(self, hist_indptr: torch.Tensor, hist_items: torch.Tensor) -> LkEaseScoreArgs:
+        a = LkEaseScoreArgs()
+        a.n_items, a.d_w = self.n_items, ptr(self.weights)
+        a.n_queries = hist_indptr.numel() - 1
+        a.d_hist_indptr, a.d_hist_items = ptr(hist_indptr), ptr(_nonempty(hist_items))
+        return a
+
+    def score(self, hist_indptr: torch.Tensor, hist_items: torch.Tensor) -> torch.Tensor:
+        """
+        Scores of every item for every query (f32 [B, n_items]): query q's history is ``hist_items[hist_indptr[q]:
+        hist_indptr[q+1]]``, ascending without repeats (:func:`ease_histories`); each score is the f32 sum of the
+        history rows' entries in that order; a query without history scores NaN everywhere.
+        """
+        B = hist_indptr.numel() - 1
+        out = torch.empty((B, self.n_items), dtype=torch.float32, device=self.weights.device)
+        if B == 0:
+            return out
+        a = self._args(hist_indptr, hist_items)
+        a.n, a.d_scores = 0, ptr(out)
+        check(lib().lk_ease_score_batch(C.byref(a), stream_ptr()), "lk_ease_score_batch")
+        return out
+
+    def recommend(
+        self, hist_indptr: torch.Tensor, hist_items: torch.Tensor, n: int,
+        excl_indptr: torch.Tensor | None = None, excl_items: torch.Tensor | None = None,
+    ):  # fmt: skip
+        """
+        Top-``n`` of every query over all items minus ``excl_items[excl_indptr[q]:excl_indptr[q+1]]`` (any order),
+        with ``argtopn``'s order and ties: ``(idx [B, n] int32, -1 padding; val [B, n] f32, NaN padding; cnt [B])``.
+        A query without history gets an empty list.
+        """
+        n_max = int(lib().lk_topn_max())
+        if not 1 <= int(n) <= n_max:
+            raise ValueError(f"n must be in 1..{n_max}")
+        n, dev, B = int(n), self.weights.device, hist_indptr.numel() - 1
+        idx = torch.empty((B, n), dtype=torch.int32, device=dev)
+        val = torch.empty((B, n), dtype=torch.float32, device=dev)
+        cnt = torch.empty(max(B, 1), dtype=torch.int32, device=dev)
+        if B == 0:
+            return idx, val, cnt[:0]
+        if excl_indptr is not None:
+            excl_indptr, excl_items = _sorted_exclusions(excl_indptr, excl_items, self.n_items, B, dev)
+        a = self._args(hist_indptr, hist_items)
+        a.n = n
+        a.d_excl_indptr, a.d_excl_items = ptr(excl_indptr), ptr(excl_items)
+        a.d_out_idx, a.d_out_val, a.d_out_cnt = ptr(idx), ptr(val), ptr(cnt)
+        check(lib().lk_ease_score_batch(C.byref(a), stream_ptr()), "lk_ease_score_batch")
         return idx, val, cnt[:B]
