@@ -20,6 +20,8 @@
  *   _accel.data.count_cooc / dense_cooc           src/accel/data/cooc.rs:49-214     lk_cooc_count (+ _diagonal, _dense)
  *   AssociationScorer.train / __call__            src/lenskit/knn/association.py    lk_cooc_count (LK_ASSOC_*), lk_assoc_score_batch
  *   EASEScorer.__call__ (q_vec @ weights)         src/lenskit/knn/ease.py           lk_ease_score_batch
+ *   _accel.slim.train_slim                        src/accel/slim/mod.rs:57-93       lk_slim_train (+ lk_slim_pool_to_csr)
+ *   SLIMScorer.__call__ (x @ weights)             src/lenskit/knn/slim.py           lk_assoc_score_batch (agg 2)
  *
  * Conventions
  *   - plain C: pointers and sizes only; no C++/torch types cross this boundary;
@@ -514,7 +516,8 @@ LK_API int lk_cooc_dense(int32_t n_items, const int64_t *d_indptr, const int32_t
  *   agg 0 (mean, max_nbrs = None):  s = +0.0f;  for t = 0 .. R-1: s = s + A[r_t, c]  (f32 adds in query order,
  *                                   absent entries add nothing);  score = f32(f64(s) / f64(R))
  *   agg 1 (max, max_nbrs = 1):      score = max over t of A[r_t, c], absent entries 0
- *   R == 0: every score is NaN.
+ *   agg 2 (sum, SLIMScorer):        s as for agg 0, score = s (no divide)
+ *   R == 0: every score is NaN (agg 0, 1; rank mode recommends nothing), +0.0 (agg 2; rank mode ranks the zeros).
  * A is the association CSR (int64 offsets, rows sorted by column); d_tile_ptr [n_items * (n_subtiles+1)] holds,
  * for each row and s = 0..n_subtiles, the position of its first column >= s * tile_cols RELATIVE to the row
  * start (lk_assoc_tile_pointers).
@@ -534,7 +537,7 @@ typedef struct lk_assoc_score_args {
     const float *d_vals;
     const int32_t *d_tile_ptr;
     int32_t n_queries;
-    int32_t agg;                       /* 0 mean, 1 max */
+    int32_t agg;                       /* 0 mean, 1 max, 2 sum */
     const int64_t *d_ref_indptr;       /* [n_queries+1] */
     const int32_t *d_ref_items;
     int32_t n;                         /* 0: score mode; 1..lk_topn_max(): rank mode */
@@ -574,6 +577,55 @@ typedef struct lk_ease_score_args {
 } lk_ease_score_args;
 
 LK_API int lk_ease_score_batch(const lk_ease_score_args *args, void *stream);
+
+/* ------------------------------------------------------------------------
+ * SLIM training (slim.cu): `_accel.slim.train_slim` (src/accel/slim/mod.rs:57-93), one weight column per target
+ * item i, rows of the result in item order.  UI (users x items) and IU (items x users) are CSR structures walked in
+ * stored order (UI rows need not be sorted; an IU row must not repeat a user).  For target i with users U_i:
+ *   resid[u] = 1 on U_i, 0 elsewhere; active = the items j != i of the UI rows of U_i in first-encounter order,
+ *   pc[j] their encounter counts; with 0 <= max_nbrs < |active|, active is stably sorted by the f64 key
+ *   -pc[j] / (sqrt(|U_i|) * sqrt(|U_j|)) and cut to max_nbrs.  Up to max_iters rounds over active, each j:
+ *   upd = +0.0f, upd += (resid[u] + W[j]) over U_j in order; new = upd >= l1 ? (upd - l1) / (f32(|U_j|) + l2) : 0;
+ *   diff = new - W[j]; W[j] = new; resid[u] -= diff over U_j; the round stops CD when max |diff| <= 1e-3f.
+ *   All f32 operations rounded to nearest, none contracted.  Row i: every j ascending with W[j] >= 1e-12f.
+ * Work units are target items (d_sched, a permutation of a subset of the items, most expensive first: see
+ * lk_cooc_row_cost with full rows over GI = UI, IG = IU); rows not listed keep the d_part_cnt given (zeroed by the
+ * caller).  Each warp of the grid owns lk_slim_workspace_bytes / warps of d_workspace, which must be zero before
+ * the first call and is zero again after every call.  Survivors go to a bump-allocated pool (one segment per row);
+ * lk_slim_pool_to_csr gathers them into a row-sorted CSR with int64 offsets.  d_work_counter counts the rows handed
+ * out (progress); the optional d_cancel flag stops handing out rows.
+ * Statuses: 1 = pool too small (nothing is usable; never a truncated result).
+ * ---------------------------------------------------------------------- */
+typedef struct lk_slim_args {
+    int32_t n_users, n_items;
+    const int32_t *d_ui_indptr;        /* [n_users+1] */
+    const int32_t *d_ui_cols;          /* items, in [0, n_items) */
+    const int32_t *d_iu_indptr;        /* [n_items+1] */
+    const int32_t *d_iu_cols;          /* users, in [0, n_users) */
+    float l1_reg, l2_reg;
+    int32_t max_iters;                 /* >= 0 */
+    int32_t max_nbrs;                  /* fsSLIM neighbours, or -1 (SLIM) */
+    const int32_t *d_sched;            /* [n_work] target items */
+    int64_t n_work;                    /* <= n_items */
+    void *d_workspace;
+    int64_t workspace_bytes;
+    int32_t *d_pool_cols;              /* [pool_capacity] */
+    float *d_pool_vals;                /* [pool_capacity] */
+    int64_t pool_capacity;
+    int64_t *d_pool_off;               /* [n_items] */
+    int32_t *d_part_cnt;               /* [n_items] */
+    unsigned long long *d_pool_cursor; /* [1] zeroed by the call */
+    int32_t *d_work_counter;           /* [1] zeroed by the call */
+    int32_t *d_status;                 /* [1] zeroed by the call */
+    const int32_t *d_cancel;           /* optional device flag (see lk_als_args.d_cancel) */
+} lk_slim_args;
+
+/* *bytes: the workspace lk_slim_train needs for n_work rows on the current device */
+LK_API int lk_slim_workspace_bytes(int32_t n_users, int32_t n_items, int64_t n_work, int64_t *bytes);
+LK_API int lk_slim_train(const lk_slim_args *args, void *stream);
+/* d_out_indptr [n_items+1]: exclusive scan of d_part_cnt */
+LK_API int lk_slim_pool_to_csr(const lk_slim_args *args, const int64_t *d_out_indptr, int32_t *d_out_cols,
+                               float *d_out_vals, void *stream);
 
 #ifdef __cplusplus
 }

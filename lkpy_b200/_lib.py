@@ -265,6 +265,34 @@ class LkEaseScoreArgs(C.Structure):
     ]
 
 
+class LkSlimArgs(C.Structure):
+    _fields_ = [
+        ("n_users", C.c_int32),
+        ("n_items", C.c_int32),
+        ("d_ui_indptr", vp),
+        ("d_ui_cols", vp),
+        ("d_iu_indptr", vp),
+        ("d_iu_cols", vp),
+        ("l1_reg", C.c_float),
+        ("l2_reg", C.c_float),
+        ("max_iters", C.c_int32),
+        ("max_nbrs", C.c_int32),
+        ("d_sched", vp),
+        ("n_work", C.c_int64),
+        ("d_workspace", vp),
+        ("workspace_bytes", C.c_int64),
+        ("d_pool_cols", vp),
+        ("d_pool_vals", vp),
+        ("pool_capacity", C.c_int64),
+        ("d_pool_off", vp),
+        ("d_part_cnt", vp),
+        ("d_pool_cursor", vp),
+        ("d_work_counter", vp),
+        ("d_status", vp),
+        ("d_cancel", vp),
+    ]
+
+
 #: every symbol ``include/lkpy_b200.h`` declares: name -> (restype, argtypes)
 SYMBOLS: dict[str, tuple] = {
     "lk_version": (C.c_int, []),
@@ -308,6 +336,9 @@ SYMBOLS: dict[str, tuple] = {
     "lk_assoc_tile_pointers": (C.c_int, [C.POINTER(LkKnnGeom), vp, vp, vp, vp]),
     "lk_assoc_score_batch": (C.c_int, [C.POINTER(LkAssocScoreArgs), vp]),
     "lk_ease_score_batch": (C.c_int, [C.POINTER(LkEaseScoreArgs), vp]),
+    "lk_slim_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, C.c_int64, i64p]),
+    "lk_slim_train": (C.c_int, [C.POINTER(LkSlimArgs), vp]),
+    "lk_slim_pool_to_csr": (C.c_int, [C.POINTER(LkSlimArgs), vp, vp, vp, vp]),
 }
 
 _lib = None

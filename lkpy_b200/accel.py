@@ -641,6 +641,62 @@ def dense_cooc(n_groups: int, n_items: int, groups: Any, cols: Any, *, diagonal:
     return AccelTask(run, total=n_items)
 
 
+def _unsigned(name: str, v: Any, bits: int) -> int:
+    """What PyO3 accepts for an unsigned Rust integer: an ``int`` (not a float), non-negative, in range."""
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+        raise TypeError(f"{name} must be an integer")
+    if v < 0 or v >= 2**bits:
+        raise OverflowError(f"{name} out of range for an unsigned {bits}-bit integer")
+    return int(v)
+
+
+def train_slim(ui_matrix: Any, iu_matrix: Any, l1_reg: float, l2_reg: float, max_iters: int, max_nbrs: int | None):
+    """
+    ``_accel.slim.train_slim`` (src/accel/slim/mod.rs:57-93): the CSR structures of the user-item matrix and its
+    transpose (values, if any, are ignored) in; an ``AccelTask`` whose result is a list of ``LargeListArray<Struct{
+    index, value: float32}>`` chunks, row ``i`` the SLIM weight column of item ``i``.  ``l1_reg`` and ``l2_reg`` are
+    rounded to float32; progress counts items.
+    """
+    ui = as_host_csr(ui_matrix)
+    iu = as_host_csr(iu_matrix)
+    if ui.shape[0] != iu.shape[1]:
+        raise ValueError("user count mismatch")
+    if ui.shape[1] != iu.shape[0]:
+        raise ValueError("item count mismatch")
+    if ui.nnz != iu.nnz:
+        raise ValueError("rating count mismatch")
+    l1, l2 = float(np.float32(l1_reg)), float(np.float32(l2_reg))
+    iters = _unsigned("max_iters", max_iters, 32)
+    if iters >= 2**31:
+        raise ValueError("max_iters must be below 2**31")
+    nbrs = None if max_nbrs is None else _unsigned("max_nbrs", max_nbrs, 64)
+    n_users, n_items = ui.shape
+
+    def run(task: AccelTask) -> list:
+        if n_items == 0:
+            e = np.zeros(0, np.int32)
+            return csr_to_arrow_chunks(InteractionCSR(np.zeros(1, np.int64), e, e.astype(np.float32), (0, 0)))
+        with _engine_lock:
+            out = _slim_rows(ui, iu, l1, l2, iters, nbrs, task)
+        return csr_to_arrow_chunks(out, RESULT_CHUNK_ROWS)
+
+    return AccelTask(run, total=n_items)
+
+
+def _slim_rows(ui: InteractionCSR, iu: InteractionCSR, l1: float, l2: float, iters: int, nbrs: int | None,
+               task: AccelTask) -> InteractionCSR:  # fmt: skip
+    """The device part of ``train_slim``: the weight rows as a host CSR, after a cancel check."""
+    dev = _lib.require_device()
+    up = lambda a: torch.from_numpy(np.require(a, requirements=["C", "W"])).to(dev)  # noqa: E731
+    (n_users, n_items) = ui.shape
+    plan = engine.SlimPlan.create(n_users, n_items, up(ui.indptr), up(ui.indices), up(iu.indptr), up(iu.indices),
+                                  l1, l2, iters, nbrs)  # fmt: skip
+    indptr, c, v = plan.train(attach=task._attach)
+    torch.cuda.current_stream().synchronize()
+    task._check_cancelled()
+    return InteractionCSR(indptr.cpu().numpy(), c.cpu().numpy(), v.cpu().numpy(), (n_items, n_items))
+
+
 #: ``from lkpy_b200.accel import als, knn`` mirrors ``from lenskit._accel import als, knn``
 data = SimpleNamespace(argtopn=argtopn, argtopn_batch=argtopn_batch, count_cooc=count_cooc, dense_cooc=dense_cooc)
 als = SimpleNamespace(
@@ -650,3 +706,4 @@ knn = SimpleNamespace(
     compute_similarities=compute_similarities, score_explicit=score_explicit, score_implicit=score_implicit,
     user_score_items_explicit=user_score_items_explicit, user_score_items_implicit=user_score_items_implicit,
 )
+slim = SimpleNamespace(train_slim=train_slim)

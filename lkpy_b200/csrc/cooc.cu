@@ -12,7 +12,8 @@
 // one bump-allocated pool segment, optionally turned into the association value (the f64-divide chain of
 // association.py:117-124) on the way, and lk_cooc_pool_to_csr gathers the segments into a row-sorted CSR.
 //
-// Scoring replaces AssociationScorer.__call__: one CTA per (query, column tile) in score mode, one CTA per
+// Scoring replaces AssociationScorer.__call__ (and, as a plain sum, SLIMScorer.__call__'s x @ weights): one CTA per
+// (query, column tile) in score mode, one CTA per
 // query sweeping the column tiles in ascending order in rank mode.  Each warp owns a sub-tile of f32
 // accumulators and walks the query's reference rows in query order (the input rows of the tile core, applied one
 // row per round), so every accumulator sees the same sequence of f32
@@ -216,7 +217,7 @@ __global__ void __launch_bounds__(CO_NT, CO_CTAS) assoc_score_kernel(const lk_as
     const float qnan = __int_as_float(0x7fc00000);
     const int n = a.n;
 
-    if (R == 0) {  // no reference items: every score is NaN, nothing is recommended
+    if (R == 0 && a.agg != 2) {  // no reference items: every score is NaN, nothing is recommended (a sum is +0.0)
         if constexpr (RANK) {
             for (int t = tid; t < n; t += CO_NT) {
                 a.d_out_idx[(int64_t)q * n + t] = -1;
@@ -263,7 +264,7 @@ __global__ void __launch_bounds__(CO_NT, CO_CTAS) assoc_score_kernel(const lk_as
                 }
                 // reference rows in query order
                 warp_apply_in_owner_order(valid, own, [&] {
-                    my[j] = a.agg == 0 ? __fadd_rn(my[j], v) : fmaxf(my[j], v);
+                    my[j] = a.agg != 1 ? __fadd_rn(my[j], v) : fmaxf(my[j], v);
                 });
             });
         }
@@ -448,7 +449,8 @@ int lk_assoc_score_batch(const lk_assoc_score_args *args, void *stream)
     const lk_assoc_score_args &a = *args;
     LK_REQUIRE(a.geom.warps == CO_WARPS && a.geom.n_halves >= 1 && a.geom.n_users == a.geom.n_items, LK_ERR_INVALID,
                "lk_assoc_score_batch: geometry not from lk_cooc_geometry(n_items, n_items)");
-    LK_REQUIRE(a.agg == 0 || a.agg == 1, LK_ERR_INVALID, "lk_assoc_score_batch: agg must be 0 (mean) or 1 (max)");
+    LK_REQUIRE(a.agg >= 0 && a.agg <= 2, LK_ERR_INVALID,
+               "lk_assoc_score_batch: agg must be 0 (mean), 1 (max) or 2 (sum)");
     LK_REQUIRE(a.n_queries >= 0 && (int64_t)a.n_queries * a.geom.n_halves < 0x7fffffffLL, LK_ERR_UNSUPPORTED,
                "lk_assoc_score_batch: n_queries * n_halves must be < 2^31");
     const bool rank = a.n != 0;

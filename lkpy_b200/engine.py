@@ -18,7 +18,7 @@ import torch
 from . import _lib
 from ._lib import (
     LkAlsArgs, LkAlsRecArgs, LkAssocScoreArgs, LkCoocArgs, LkEaseScoreArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs,
-    LkKnnScoreArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr,
+    LkKnnScoreArgs, LkSlimArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr,
 )  # fmt: skip
 from .data import InteractionCSR
 
@@ -1335,3 +1335,136 @@ class EaseState:
         a.d_out_idx, a.d_out_val, a.d_out_cnt = ptr(idx), ptr(val), ptr(cnt)
         check(lib().lk_ease_score_batch(C.byref(a), stream_ptr()), "lk_ease_score_batch")
         return idx, val, cnt[:B]
+
+
+# ---------------------------------------------------------------------------
+# SLIM training
+# ---------------------------------------------------------------------------
+
+
+@dataclass
+class SlimPlan:
+    """
+    The inputs of ``lk_slim_train`` for one training run: the UI and IU structures (int32 offsets and indices, rows
+    in the caller's stored order), the f32 regularisation, the iteration and neighbour limits, and the target items
+    most expensive first.  ``columns`` restricts training to some target items (their rows are computed exactly as
+    in a full run; the others stay empty), so that a sample of the items can be checked or timed.
+    """
+
+    n_users: int
+    n_items: int
+    ui_indptr: torch.Tensor
+    ui_cols: torch.Tensor
+    iu_indptr: torch.Tensor
+    iu_cols: torch.Tensor
+    l1_reg: float
+    l2_reg: float
+    max_iters: int
+    max_nbrs: int  # -1: SLIM
+    sched: torch.Tensor  # int32 target items, most expensive first
+    capacity_bound: int  # entries the result can have at most
+    work_counter: torch.Tensor
+    status: torch.Tensor
+    cursor: torch.Tensor
+    #: optional device int32 flag checked whenever a warp fetches a target item
+    cancel: torch.Tensor | None = None
+
+    @classmethod
+    def create(
+        cls, n_users: int, n_items: int, ui_indptr, ui_cols, iu_indptr, iu_cols, l1_reg: float, l2_reg: float,
+        max_iters: int, max_nbrs: int | None, columns=None,
+    ) -> "SlimPlan":  # fmt: skip
+        """Device tensors in (any integer dtype; nnz < 2**31).  Raises ``ValueError`` for an index out of range or an
+        IU row that repeats a user (coordinate descent updates each of a row's residuals once per entry)."""
+        if n_items < 1 or n_users < 0:
+            raise ValueError("SLIM needs at least one item")
+        dev = ui_indptr.device
+        i32 = lambda t: _nonempty(torch.as_tensor(t).to(device=dev, dtype=torch.int32).contiguous())  # noqa: E731
+        for name, ip, c, rows, ncols in (("ui_matrix", ui_indptr, ui_cols, n_users, n_items),
+                                         ("iu_matrix", iu_indptr, iu_cols, n_items, n_users)):  # fmt: skip
+            if ip.numel() != rows + 1 or int(ip[-1].item()) != c.numel():
+                raise ValueError(f"{name}: offsets do not match the shape")
+            if c.numel() >= 2**31:
+                raise _lib.EngineError("SLIM input with 2**31 or more entries is not supported")
+            if c.numel() and (int(c.min().item()) < 0 or int(c.max().item()) >= ncols):
+                raise ValueError(f"{name}: index out of range")
+        nnz = iu_cols.numel()
+        if nnz:
+            row = torch.repeat_interleave(torch.arange(n_items, device=dev), (iu_indptr[1:] - iu_indptr[:-1]).long())
+            key = torch.sort(row * max(n_users, 1) + iu_cols.long()).values
+            if bool((key[1:] == key[:-1]).any()):
+                raise ValueError("iu_matrix: a row repeats a user")
+        ui_p, ui_c, iu_p, iu_c = i32(ui_indptr), i32(ui_cols), i32(iu_indptr), i32(iu_cols)
+        # cost of target i: sum over its users of their UI row lengths, the entries the active-set walk reads
+        geom = LkKnnGeom()
+        check(lib().lk_cooc_geometry(max(n_users, 0), n_items, C.byref(geom)), "lk_cooc_geometry")
+        ca = LkCoocArgs()
+        ca.geom, ca.full_rows = geom, 1
+        ca.d_gi_indptr, ca.d_gi_items, ca.d_ig_indptr, ca.d_ig_groups = ptr(ui_p), ptr(ui_c), ptr(iu_p), ptr(iu_c)
+        cost = torch.empty(n_items, dtype=torch.int64, device=dev)
+        check(lib().lk_cooc_row_cost(C.byref(ca), ptr(cost), stream_ptr()), "lk_cooc_row_cost")
+        if columns is None:
+            cols = torch.arange(n_items, device=dev)
+        else:
+            cols = torch.unique(torch.as_tensor(columns, device=dev).long())
+            if cols.numel() and (int(cols[0].item()) < 0 or int(cols[-1].item()) >= n_items):
+                raise ValueError("columns: item out of range")
+        sched = cols[torch.argsort(cost[cols], descending=True, stable=True)].to(torch.int32).contiguous()
+        k = -1 if max_nbrs is None or int(max_nbrs) >= n_items else int(max_nbrs)
+        width = min(n_items - 1, k) if k >= 0 else n_items - 1
+        bound = int(torch.clamp(cost[cols], max=max(width, 0)).sum().item())
+        z = lambda dt: torch.zeros(1, dtype=dt, device=dev)  # noqa: E731
+        return cls(
+            n_users, n_items, ui_p, ui_c, iu_p, iu_c, float(np.float32(l1_reg)), float(np.float32(l2_reg)),
+            int(max_iters), k, sched, bound, z(torch.int32), z(torch.int32), z(torch.int64),
+        )  # fmt: skip
+
+    def train(self, attach=None, capacity: int | None = None):
+        """
+        The weight rows as a device CSR (int64 indptr [n_items+1], int32 columns ascending, f32 values).
+        ``attach(counter, units)``, if given, is called before the launch and returns the device cancel flag.  The
+        result pool starts at ``capacity`` entries (a guess by default) and a run that overflows it is repeated
+        with a larger pool, up to the bound that cannot overflow.
+        """
+        dev = self.ui_indptr.device
+        n = self.n_items
+        a = LkSlimArgs()
+        a.n_users, a.n_items = self.n_users, n
+        a.d_ui_indptr, a.d_ui_cols = ptr(self.ui_indptr), ptr(self.ui_cols)
+        a.d_iu_indptr, a.d_iu_cols = ptr(self.iu_indptr), ptr(self.iu_cols)
+        a.l1_reg, a.l2_reg, a.max_iters, a.max_nbrs = self.l1_reg, self.l2_reg, self.max_iters, self.max_nbrs
+        a.d_sched, a.n_work = ptr(self.sched), self.sched.numel()
+        a.d_work_counter, a.d_status, a.d_pool_cursor = ptr(self.work_counter), ptr(self.status), ptr(self.cursor)
+        if attach is not None:
+            self.cancel = attach(self.work_counter, self.sched.numel())
+        a.d_cancel = ptr(self.cancel)
+        ws_bytes = C.c_int64()
+        check(lib().lk_slim_workspace_bytes(self.n_users, n, self.sched.numel(), C.byref(ws_bytes)),
+              "lk_slim_workspace_bytes")  # fmt: skip
+        ws = torch.zeros(max(int(ws_bytes.value), 1), dtype=torch.uint8, device=dev)
+        a.d_workspace, a.workspace_bytes = ptr(ws), ws.numel()
+        if capacity is None:
+            capacity = max(4 * self.iu_cols.numel(), 1 << 22)
+        capacity = max(1, min(int(capacity), self.capacity_bound))
+        overflowed = False
+
+        def launch(pool_cols, pool_vals, pool_off, part_cnt):
+            nonlocal overflowed
+            a.d_pool_cols, a.d_pool_vals, a.pool_capacity = ptr(pool_cols), ptr(pool_vals), pool_cols.numel()
+            a.d_pool_off, a.d_part_cnt = ptr(pool_off), ptr(part_cnt)
+            check(lib().lk_slim_train(C.byref(a), stream_ptr()), "lk_slim_train")
+            st = int(self.status.item())
+            overflowed = st == 1
+            return st
+
+        def gather(indptr, cols, vals):
+            check(lib().lk_slim_pool_to_csr(C.byref(a), ptr(indptr), ptr(cols), ptr(vals), stream_ptr()),
+                  "lk_slim_pool_to_csr")  # fmt: skip
+
+        while True:
+            try:
+                return pool_to_csr(dev, n, 1, capacity, torch.float32, launch, gather, "lk_slim_train: pool overflow")
+            except _lib.EngineError:
+                if not overflowed or capacity >= self.capacity_bound:
+                    raise
+                capacity = min(4 * capacity, self.capacity_bound)
