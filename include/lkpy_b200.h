@@ -22,6 +22,9 @@
  *   EASEScorer.__call__ (q_vec @ weights)         src/lenskit/knn/ease.py           lk_ease_score_batch
  *   _accel.slim.train_slim                        src/accel/slim/mod.rs:57-93       lk_slim_train (+ lk_slim_pool_to_csr)
  *   SLIMScorer.__call__ (x @ weights)             src/lenskit/knn/slim.py           lk_assoc_score_batch (agg 2)
+ *   sample_negatives (host, per minibatch)        src/accel/data/sampling.rs:38-58  lk_flexmf_sample_negatives
+ *   FlexMFImplicitTrainer.train_batch (autograd)  src/lenskit/flexmf/_implicit.py:253-274 lk_flexmf_step
+ *   FlexMFScorerBase.__call__ + TopNRanker        src/lenskit/flexmf/_base.py:117-157 lk_als_recommend_batch (biases as offsets)
  *
  * Conventions
  *   - plain C: pointers and sizes only; no C++/torch types cross this boundary;
@@ -626,6 +629,110 @@ LK_API int lk_slim_train(const lk_slim_args *args, void *stream);
 /* d_out_indptr [n_items+1]: exclusive scan of d_part_cnt */
 LK_API int lk_slim_pool_to_csr(const lk_slim_args *args, const int64_t *d_out_indptr, int32_t *d_out_cols,
                                float *d_out_vals, void *stream);
+
+/* ------------------------------------------------------------------------
+ * FlexMF implicit (flexmf.cu): gradient-trained matrix factorisation with logistic or pairwise (BPR) loss,
+ * FlexMFImplicitTrainer (src/lenskit/flexmf/_implicit.py, _training.py, _model.py).  Score of (u, i):
+ * s = ub[u] + ib[i] + <U[u], I[i]>, an absent bias vector counting as 0.
+ *
+ * Negative sampling.  For sample g of d_rows (a user), step = step0 + g / batch_size, pos = g % batch_size, and
+ * rep < n: draw columns attempt = 0, 1, ... and keep the first that is not a column of the user's CSR row, or the
+ * draw of attempt == max_attempts whatever it is (the procedure of sampling.rs:38-58; the stream is this
+ * library's own).  With all arithmetic in uint64, wrapping:
+ *     mix(x):  x ^= x >> 30;  x *= 0xbf58476d1ce4e5b9;  x ^= x >> 27;  x *= 0x94d049bb133111eb;  x ^= x >> 31
+ *     G = 0x9e3779b97f4a7c15
+ *     h = mix(seed + G * (step + 1));  h = mix(h + G * (pos + 1));  h = mix(h + G * ((rep << 32) + attempt + 1))
+ *     draw(m) = ((h >> 32) * m) >> 32                      in [0, m); no value is more than m / 2^32 (relative)
+ *                                                          more likely than another
+ *   uniform: column = draw(n_items);  popular: column = d_coo_items[draw(nnz)], a uniformly drawn training
+ *   interaction's item.  d_out [n_samples][n].  CSR columns ascending within a row (membership is a binary search).
+ * ---------------------------------------------------------------------- */
+typedef struct lk_flexmf_sample_args {
+    int32_t n_users, n_items;
+    const int32_t *d_ui_indptr;        /* [n_users+1] */
+    const int32_t *d_ui_cols;          /* items, ascending within a row */
+    const int32_t *d_coo_items;        /* [nnz] item of every training interaction (popular only) */
+    int64_t nnz;                       /* < 2^32 */
+    const int32_t *d_rows;             /* [n_samples] users */
+    int64_t n_samples;
+    int32_t batch_size;                /* samples per step (>= 1) */
+    int32_t n;                         /* negatives per sample (>= 1) */
+    int32_t max_attempts;              /* rejected draws before one is kept regardless (the reference: 10) */
+    int32_t popular;                   /* 0 uniform, 1 popularity-weighted */
+    uint64_t seed;
+    int64_t step0;                     /* step number of sample 0 */
+    int32_t *d_out;                    /* [n_samples][n] */
+} lk_flexmf_sample_args;
+
+LK_API int lk_flexmf_sample_negatives(const lk_flexmf_sample_args *args, void *stream);
+
+#define LK_FLEXMF_LOGISTIC 0
+#define LK_FLEXMF_PAIRWISE 1
+#define LK_FLEXMF_REG_NONE 0   /* torch.optim.SparseAdam */
+#define LK_FLEXMF_REG_L2 1     /* explicit norm term in the loss, SparseAdam */
+#define LK_FLEXMF_REG_ADAMW 2  /* torch.optim.AdamW(weight_decay = regularization) over every parameter */
+
+/*
+ * The occurrences of one side's rows (users, or items) in the batches, grouped by the caller.  Users occur once per
+ * sample (entry: the sample's position b in its batch); items once per (sample, slot) with slot 0 the positive and
+ * 1..n the negatives (entry: b * (n + 1) + slot).  Entries are sorted by (step, row, entry) in d_occ; every maximal
+ * run of one (step, row) is a "uniq", cut into "units" of at most 64 consecutive entries.  All indices are into the
+ * arrays given, which may cover many steps; a step uses units [unit0, unit0 + n_units) and uniqs [uniq0, uniq0 + n_uniq).
+ */
+typedef struct lk_flexmf_groups {
+    const int32_t *d_occ;
+    const int64_t *d_unit_start;       /* [units + 1] offsets into d_occ */
+    const int32_t *d_unit_uniq;        /* [units] the uniq a unit belongs to */
+    const int32_t *d_uniq_row;         /* [uniqs] row number */
+    const int32_t *d_uniq_unit;        /* [uniqs + 1] first unit of every uniq */
+    int64_t unit0, uniq0;
+    int32_t n_uniq;
+    int64_t *d_mark;                   /* AdamW: [n_rows], zero before step 1; (step << 32 | uniq) of the last touch */
+} lk_flexmf_groups;
+
+/*
+ * One minibatch step, in place: the loss of the batch as the reference defines it
+ *   logistic: (sum_b -log sigma(s+_b) * positive_weight + sum_{b,r} -log sigma(-s-_{b,r})) / (B + B n)
+ *   pairwise: mean over the B n pairs of -log sigma(s+_b - s-_{b,r})
+ *   LK_FLEXMF_REG_L2 adds regularization * 0.5 * (mean_b norm+ + mean_{b,r} norm-), norm = ub^2 + ib^2 + |U[u]| + |I[i]|
+ *   (vector norms not squared; the gradient of |x| at x = 0 is 0),
+ * its gradient with every row's contributions added in a fixed order (ascending entry within a unit, a user's
+ * items of one sample combined first, units of a row ascending), then the optimiser (betas, eps as given;
+ * the host passes the scalars that depend on the step number):
+ *   AdamW      every row:  w *= decay;  m += (g - m)(1 - beta1);  v = v beta2 + (1 - beta2) g^2;
+ *                          w -= step_size * m / (sqrt(v) / bias2_sqrt + eps)     with step_size = lr / (1 - beta1^t)
+ *   SparseAdam rows of the batch only:  m += (g - m)(1 - beta1);  v += (g^2 - v)(1 - beta2);
+ *                          w -= step_size * m / (sqrt(v) + eps)     with step_size = lr sqrt(1 - beta2^t) / (1 - beta1^t)
+ * d_loss[0] receives the batch loss (f32, summed in f64 in a fixed order).  No float atomics: the result is a pure
+ * function of the arguments.  k <= lk_als_max_features().
+ */
+typedef struct lk_flexmf_step_args {
+    int32_t n_users, n_items, k;
+    int32_t batch;                     /* B: samples in this step */
+    int32_t n_neg;                     /* n */
+    int32_t loss;                      /* LK_FLEXMF_LOGISTIC / _PAIRWISE */
+    int32_t reg_method;                /* LK_FLEXMF_REG_* */
+    float positive_weight, regularization;
+    float decay;                       /* AdamW: 1 - lr * regularization */
+    float one_minus_beta1, beta2, one_minus_beta2, eps;
+    float step_size, bias2_sqrt;       /* see above; bias2_sqrt = sqrt(1 - beta2^t), AdamW only */
+    int64_t step;                      /* t >= 1, below 2^31 */
+    float *d_u_emb, *d_u_emb_m, *d_u_emb_v;    /* [n_users][k] parameters and the two moments */
+    float *d_i_emb, *d_i_emb_m, *d_i_emb_v;    /* [n_items][k] */
+    float *d_u_bias, *d_u_bias_m, *d_u_bias_v; /* [n_users] or all NULL */
+    float *d_i_bias, *d_i_bias_m, *d_i_bias_v; /* [n_items] or all NULL */
+    const int32_t *d_users;            /* [B] */
+    const int32_t *d_pos;              /* [B] */
+    const int32_t *d_neg;              /* [B][n] */
+    lk_flexmf_groups u_groups, i_groups;
+    int32_t n_u_units, n_i_units;
+    void *d_workspace;
+    int64_t workspace_bytes;           /* >= lk_flexmf_workspace_bytes(batch, n_neg, k) */
+    float *d_loss;                     /* [1] */
+} lk_flexmf_step_args;
+
+LK_API int lk_flexmf_workspace_bytes(int32_t batch, int32_t n_neg, int32_t k, int64_t *bytes);
+LK_API int lk_flexmf_step(const lk_flexmf_step_args *args, void *stream);
 
 #ifdef __cplusplus
 }

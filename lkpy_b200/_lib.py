@@ -18,6 +18,8 @@ LK_DTYPE_F32, LK_DTYPE_BF16 = 0, 1
 LK_ALS_IMPLICIT, LK_ALS_EXPLICIT = 0, 1
 LK_MAX_REPLICAS = 8
 LK_COOC_COUNT, LK_ASSOC_PROBABILITY, LK_ASSOC_LIFT = 0, 1, 2
+LK_FLEXMF_LOGISTIC, LK_FLEXMF_PAIRWISE = 0, 1
+LK_FLEXMF_REG_NONE, LK_FLEXMF_REG_L2, LK_FLEXMF_REG_ADAMW = 0, 1, 2
 
 i32p = C.POINTER(C.c_int32)
 i64p = C.POINTER(C.c_int64)
@@ -293,6 +295,76 @@ class LkSlimArgs(C.Structure):
     ]
 
 
+class LkFlexmfSampleArgs(C.Structure):
+    _fields_ = [
+        ("n_users", C.c_int32),
+        ("n_items", C.c_int32),
+        ("d_ui_indptr", vp),
+        ("d_ui_cols", vp),
+        ("d_coo_items", vp),
+        ("nnz", C.c_int64),
+        ("d_rows", vp),
+        ("n_samples", C.c_int64),
+        ("batch_size", C.c_int32),
+        ("n", C.c_int32),
+        ("max_attempts", C.c_int32),
+        ("popular", C.c_int32),
+        ("seed", C.c_uint64),
+        ("step0", C.c_int64),
+        ("d_out", vp),
+    ]
+
+
+class LkFlexmfGroups(C.Structure):
+    _fields_ = [
+        ("d_occ", vp),
+        ("d_unit_start", vp),
+        ("d_unit_uniq", vp),
+        ("d_uniq_row", vp),
+        ("d_uniq_unit", vp),
+        ("unit0", C.c_int64),
+        ("uniq0", C.c_int64),
+        ("n_uniq", C.c_int32),
+        ("d_mark", vp),
+    ]
+
+
+class LkFlexmfStepArgs(C.Structure):
+    _fields_ = [
+        ("n_users", C.c_int32),
+        ("n_items", C.c_int32),
+        ("k", C.c_int32),
+        ("batch", C.c_int32),
+        ("n_neg", C.c_int32),
+        ("loss", C.c_int32),
+        ("reg_method", C.c_int32),
+        ("positive_weight", C.c_float),
+        ("regularization", C.c_float),
+        ("decay", C.c_float),
+        ("one_minus_beta1", C.c_float),
+        ("beta2", C.c_float),
+        ("one_minus_beta2", C.c_float),
+        ("eps", C.c_float),
+        ("step_size", C.c_float),
+        ("bias2_sqrt", C.c_float),
+        ("step", C.c_int64),
+        ("d_u_emb", vp), ("d_u_emb_m", vp), ("d_u_emb_v", vp),
+        ("d_i_emb", vp), ("d_i_emb_m", vp), ("d_i_emb_v", vp),
+        ("d_u_bias", vp), ("d_u_bias_m", vp), ("d_u_bias_v", vp),
+        ("d_i_bias", vp), ("d_i_bias_m", vp), ("d_i_bias_v", vp),
+        ("d_users", vp),
+        ("d_pos", vp),
+        ("d_neg", vp),
+        ("u_groups", LkFlexmfGroups),
+        ("i_groups", LkFlexmfGroups),
+        ("n_u_units", C.c_int32),
+        ("n_i_units", C.c_int32),
+        ("d_workspace", vp),
+        ("workspace_bytes", C.c_int64),
+        ("d_loss", vp),
+    ]  # fmt: skip
+
+
 #: every symbol ``include/lkpy_b200.h`` declares: name -> (restype, argtypes)
 SYMBOLS: dict[str, tuple] = {
     "lk_version": (C.c_int, []),
@@ -339,6 +411,9 @@ SYMBOLS: dict[str, tuple] = {
     "lk_slim_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, C.c_int64, i64p]),
     "lk_slim_train": (C.c_int, [C.POINTER(LkSlimArgs), vp]),
     "lk_slim_pool_to_csr": (C.c_int, [C.POINTER(LkSlimArgs), vp, vp, vp, vp]),
+    "lk_flexmf_sample_negatives": (C.c_int, [C.POINTER(LkFlexmfSampleArgs), vp]),
+    "lk_flexmf_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, i64p]),
+    "lk_flexmf_step": (C.c_int, [C.POINTER(LkFlexmfStepArgs), vp]),
 }
 
 _lib = None

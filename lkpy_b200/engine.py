@@ -17,8 +17,8 @@ import torch
 
 from . import _lib
 from ._lib import (
-    LkAlsArgs, LkAlsRecArgs, LkAssocScoreArgs, LkCoocArgs, LkEaseScoreArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs,
-    LkKnnScoreArgs, LkSlimArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr,
+    LkAlsArgs, LkAlsRecArgs, LkAssocScoreArgs, LkCoocArgs, LkEaseScoreArgs, LkFlexmfSampleArgs, LkFlexmfStepArgs,
+    LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkSlimArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr,
 )  # fmt: skip
 from .data import InteractionCSR
 
@@ -1468,3 +1468,225 @@ class SlimPlan:
                 if not overflowed or capacity >= self.capacity_bound:
                     raise
                 capacity = min(4 * capacity, self.capacity_bound)
+
+
+# ---------------------------------------------------------------------------
+# FlexMF implicit
+# ---------------------------------------------------------------------------
+
+FLEXMF_LOSSES = {"logistic": _lib.LK_FLEXMF_LOGISTIC, "pairwise": _lib.LK_FLEXMF_PAIRWISE}
+FLEXMF_REG_METHODS = {None: _lib.LK_FLEXMF_REG_NONE, "L2": _lib.LK_FLEXMF_REG_L2, "AdamW": _lib.LK_FLEXMF_REG_ADAMW}
+FLEXMF_MAX_ATTEMPTS = 10  # rejected draws per negative, as the reference's sampler
+FLEXMF_UNIT = 64  # occurrences of a row per gradient unit (flexmf.cu)
+_ADAM_BETA1, _ADAM_BETA2, _ADAM_EPS = 0.9, 0.999, 1e-8  # torch.optim defaults
+
+
+def flexmf_workspace_bytes(batch: int, n_neg: int, k: int) -> int:
+    out = C.c_int64()
+    check(lib().lk_flexmf_workspace_bytes(batch, n_neg, k, C.byref(out)), "lk_flexmf_workspace_bytes")
+    return int(out.value)
+
+
+def flexmf_adam_scalars(reg_method: str | None, lr: float, regularization: float, step: int) -> dict[str, float]:
+    """The step-dependent scalars of ``lk_flexmf_step``, computed in double as torch's optimisers do."""
+    bc1, bc2 = 1 - _ADAM_BETA1**step, 1 - _ADAM_BETA2**step
+    if reg_method == "AdamW":
+        return {"decay": 1 - lr * regularization, "step_size": lr / bc1, "bias2_sqrt": bc2**0.5}
+    return {"decay": 1.0, "step_size": lr * bc2**0.5 / bc1, "bias2_sqrt": 1.0}
+
+
+@dataclass
+class _FlexmfGroups:
+    """One side's occurrences in a run of batches, grouped for ``lk_flexmf_step`` (``lk_flexmf_groups``)."""
+
+    occ: torch.Tensor
+    unit_start: torch.Tensor
+    unit_uniq: torch.Tensor
+    uniq_row: torch.Tensor
+    uniq_unit: torch.Tensor
+    step_uniq: np.ndarray  # host: first uniq of every step, and the total
+    step_unit: np.ndarray  # host: first unit of every step, and the total
+
+    @classmethod
+    def build(cls, keys: torch.Tensor, entries: torch.Tensor, n_rows: int, n_steps: int) -> "_FlexmfGroups":
+        """``keys`` = step * n_rows + row of every occurrence, ``entries`` ascending within a step.  Index plumbing
+        only (a stable sort, flags and prefix sums); the additions these groups order are the kernel's."""
+        dev = keys.device
+        E = keys.numel()
+        if E >= 2**31:  # uniq and unit numbers are int32 in lk_flexmf_groups
+            raise _lib.EngineError(f"{E} row occurrences in one run of batches; the grouping holds fewer than 2**31")
+        skey, order = torch.sort(keys, stable=True)  # stable: entries stay ascending within a (step, row)
+        new_row = torch.ones(E, dtype=torch.bool, device=dev)
+        new_row[1:] = skey[1:] != skey[:-1]
+        uniq_at = torch.nonzero(new_row).flatten()
+        uniq_of = torch.cumsum(new_row, 0) - 1
+        # every run of one (step, row) is cut from its own start, so a batch's units do not depend on its neighbours
+        new_unit = (torch.arange(E, device=dev) - uniq_at[uniq_of]) % FLEXMF_UNIT == 0
+        unit_at = torch.nonzero(new_unit).flatten()
+        unit_uniq = uniq_of[unit_at].to(torch.int32)
+        uniq_unit = torch.searchsorted(unit_at, uniq_at)
+        ukey = skey[uniq_at]
+        step_uniq = torch.searchsorted(ukey, torch.arange(n_steps + 1, device=dev) * n_rows)
+        uniq_unit = torch.cat([uniq_unit, torch.tensor([unit_at.numel()], device=dev)])
+        step_unit = uniq_unit[step_uniq]
+        return cls(
+            entries[order].contiguous(), torch.cat([unit_at, torch.tensor([E], device=dev)]), unit_uniq,
+            (ukey % n_rows).to(torch.int32), uniq_unit.to(torch.int32), step_uniq.cpu().numpy(), step_unit.cpu().numpy(),
+        )  # fmt: skip
+
+    def fill(self, g, step: int, mark: torch.Tensor | None) -> int:
+        g.d_occ, g.d_unit_start, g.d_unit_uniq = ptr(self.occ), ptr(self.unit_start), ptr(self.unit_uniq)
+        g.d_uniq_row, g.d_uniq_unit, g.d_mark = ptr(self.uniq_row), ptr(self.uniq_unit), ptr(mark)
+        g.unit0, g.uniq0 = int(self.step_unit[step]), int(self.step_uniq[step])
+        g.n_uniq = int(self.step_uniq[step + 1] - self.step_uniq[step])
+        return int(self.step_unit[step + 1] - self.step_unit[step])
+
+
+@dataclass
+class _FlexmfBatches:
+    users: torch.Tensor
+    pos: torch.Tensor
+    neg: torch.Tensor
+    u_groups: _FlexmfGroups
+    i_groups: _FlexmfGroups
+    n_steps: int
+
+
+class FlexMFState:
+    """
+    Device state of one FlexMF implicit training run: the four parameter tables with their Adam moments, the
+    users x items CSR the sampler tests membership in, the step workspace, the optimiser step count and the sampler
+    seed.  The only caller of ``lk_flexmf_sample_negatives`` and ``lk_flexmf_step``.
+
+    ``params`` maps the reference's state-dict names (``u_bias.weight`` / ``i_bias.weight`` [n, 1], optional;
+    ``u_embed.weight`` / ``i_embed.weight`` [n, k]) to f32 arrays or tensors; ``users`` / ``items`` are the training
+    interactions sorted by (user, item).
+    """
+
+    def __init__(self, params: dict, users, items, *, loss: str, reg_method: str | None, negative_count: int = 1,
+                 popular: bool = False, batch_size: int = 8192, learning_rate: float = 0.01,
+                 regularization: float = 0.01, positive_weight: float = 1.0, seed: int = 0, device=None):  # fmt: skip
+        dev = device or _lib.require_device()
+        if loss not in FLEXMF_LOSSES:
+            raise ValueError(f"loss={loss!r} is not one of {sorted(FLEXMF_LOSSES)}")
+        if reg_method not in FLEXMF_REG_METHODS:
+            raise ValueError(f"reg_method={reg_method!r} is not one of 'AdamW', 'L2', None")
+        self.loss, self.reg_method, self.n_neg, self.popular = loss, reg_method, int(negative_count), bool(popular)
+        self.batch_size, self.lr, self.reg = int(batch_size), float(learning_rate), float(regularization)
+        self.positive_weight, self.seed = float(positive_weight), int(seed) & (2**64 - 1)
+        self.params: dict[str, torch.Tensor] = {}
+        for name in ("u_bias.weight", "i_bias.weight", "u_embed.weight", "i_embed.weight"):
+            if params.get(name) is not None:
+                self.params[name] = torch.as_tensor(params[name]).to(dev, torch.float32).contiguous().clone()
+        self.n_users, self.k = self.params["u_embed.weight"].shape
+        self.n_items = self.params["i_embed.weight"].shape[0]
+        if self.params["i_embed.weight"].shape[1] != self.k or not 1 <= self.k <= ALS_MAX_FEATURES:
+            raise ValueError(f"embedding sizes must agree and be in 1..{ALS_MAX_FEATURES}")
+        self.moments = {n: (torch.zeros_like(t), torch.zeros_like(t)) for n, t in self.params.items()}
+        self.users = torch.as_tensor(users).to(dev, torch.int32).contiguous()
+        self.items = torch.as_tensor(items).to(dev, torch.int32).contiguous()
+        self.ui_indptr = torch.zeros(self.n_users + 1, dtype=torch.int64, device=dev)
+        torch.cumsum(torch.bincount(self.users.long(), minlength=self.n_users), 0, out=self.ui_indptr[1:])
+        if self.items.numel() >= 2**31:
+            raise _lib.EngineError("more than 2**31 - 1 interactions need sharding first")
+        self.ui_indptr = self.ui_indptr.to(torch.int32)
+        dense = reg_method == "AdamW"
+        self.u_mark = torch.zeros(self.n_users, dtype=torch.int64, device=dev) if dense else None
+        self.i_mark = torch.zeros(self.n_items, dtype=torch.int64, device=dev) if dense else None
+        self.workspace = torch.empty(flexmf_workspace_bytes(self.batch_size, self.n_neg, self.k), dtype=torch.uint8,
+                                     device=dev)  # fmt: skip
+        self.steps_done = 0
+        self.device = dev
+
+    def sample(self, rows: torch.Tensor, step0: int | None = None, *, n: int | None = None,
+               popular: bool | None = None, max_attempts: int = FLEXMF_MAX_ATTEMPTS) -> torch.Tensor:  # fmt: skip
+        """Negatives [len(rows), n] for the users ``rows``, cut into batches of ``batch_size`` whose step numbers
+        start at ``step0`` (default: the steps done so far)."""
+        rows = rows.to(self.device, torch.int32).contiguous()
+        a = LkFlexmfSampleArgs()
+        a.n_users, a.n_items, a.d_ui_indptr, a.d_ui_cols = self.n_users, self.n_items, ptr(self.ui_indptr), ptr(self.items)
+        a.d_coo_items, a.nnz, a.d_rows, a.n_samples = ptr(self.items), self.items.numel(), ptr(rows), rows.numel()
+        a.batch_size, a.n, a.max_attempts = self.batch_size, self.n_neg if n is None else int(n), int(max_attempts)
+        a.popular = int(self.popular if popular is None else popular)
+        a.seed, a.step0 = self.seed, self.steps_done if step0 is None else int(step0)
+        out = torch.empty((rows.numel(), a.n), dtype=torch.int32, device=self.device)
+        a.d_out = ptr(out)
+        check(lib().lk_flexmf_sample_negatives(C.byref(a), stream_ptr()), "lk_flexmf_sample_negatives")
+        return out
+
+    def _step_args(self) -> LkFlexmfStepArgs:
+        a = LkFlexmfStepArgs()
+        a.n_users, a.n_items, a.k, a.n_neg = self.n_users, self.n_items, self.k, self.n_neg
+        a.loss, a.reg_method = FLEXMF_LOSSES[self.loss], FLEXMF_REG_METHODS[self.reg_method]
+        a.positive_weight, a.regularization = self.positive_weight, self.reg
+        a.one_minus_beta1, a.beta2, a.one_minus_beta2, a.eps = 1 - _ADAM_BETA1, _ADAM_BETA2, 1 - _ADAM_BETA2, _ADAM_EPS
+        for field_, name in (("u_emb", "u_embed.weight"), ("i_emb", "i_embed.weight"), ("u_bias", "u_bias.weight"),
+                             ("i_bias", "i_bias.weight")):  # fmt: skip
+            if name in self.params:
+                m, v = self.moments[name]
+                setattr(a, f"d_{field_}", ptr(self.params[name]))
+                setattr(a, f"d_{field_}_m", ptr(m))
+                setattr(a, f"d_{field_}_v", ptr(v))
+        a.d_workspace, a.workspace_bytes = ptr(self.workspace), self.workspace.numel()
+        return a
+
+    def plan_batches(self, users: torch.Tensor, pos: torch.Tensor, neg: torch.Tensor | None = None) -> "_FlexmfBatches":
+        """
+        Everything about a run of consecutive batches (``batch_size`` samples each, the last may be short) that does
+        not depend on the model: the negatives (``neg`` [S, n], default this state's sampler at the current step
+        count) and the grouping of every batch's rows.  Made once for all the steps, so an epoch pays one sampler
+        launch and two sorts instead of one of each per step.
+        """
+        dev, B, n = self.device, self.batch_size, self.n_neg
+        users = users.to(dev, torch.int32).contiguous()
+        pos = pos.to(dev, torch.int32).contiguous()
+        S = users.numel()
+        neg = self.sample(users) if neg is None else neg.to(dev, torch.int32).contiguous()
+        if S == 0 or pos.numel() != S or tuple(neg.shape) != (S, n):
+            raise ValueError(f"expected {S} > 0 users, as many positives and negatives of shape ({S}, {n})")
+        n_steps = -(-S // B)
+        at = torch.arange(S, device=dev)
+        step_of, local = at // B, (at % B).to(torch.int32)
+        ug = _FlexmfGroups.build(step_of * self.n_users + users.long(), local, self.n_users, n_steps)
+        slots = torch.cat([pos[:, None], neg], dim=1).long()
+        entries = local[:, None] * (n + 1) + torch.arange(n + 1, device=dev, dtype=torch.int32)[None, :]
+        ig = _FlexmfGroups.build((step_of[:, None] * self.n_items + slots).flatten(), entries.flatten(),
+                                 self.n_items, n_steps)  # fmt: skip
+        return _FlexmfBatches(users, pos, neg, ug, ig, n_steps)
+
+    def run_batches(self, plan: "_FlexmfBatches") -> torch.Tensor:
+        """The steps of ``plan``, four launches each; the batch losses as a device vector, not synchronised on."""
+        B, n, S = self.batch_size, self.n_neg, plan.users.numel()
+        if self.steps_done + plan.n_steps >= 2**31:
+            raise _lib.EngineError("the optimiser step count must stay below 2**31")
+        losses = torch.empty(plan.n_steps, dtype=torch.float32, device=self.device)
+        a = self._step_args()
+        stream = stream_ptr()
+        for s in range(plan.n_steps):
+            lo, hi = s * B, min(S, (s + 1) * B)
+            a.batch, a.step = hi - lo, self.steps_done + 1
+            for name, value in flexmf_adam_scalars(self.reg_method, self.lr, self.reg, a.step).items():
+                setattr(a, name, value)
+            a.d_users, a.d_pos = plan.users.data_ptr() + 4 * lo, plan.pos.data_ptr() + 4 * lo
+            a.d_neg = plan.neg.data_ptr() + 4 * lo * n
+            a.n_u_units = plan.u_groups.fill(a.u_groups, s, self.u_mark)
+            a.n_i_units = plan.i_groups.fill(a.i_groups, s, self.i_mark)
+            a.d_loss = losses.data_ptr() + 4 * s
+            check(lib().lk_flexmf_step(C.byref(a), stream), "lk_flexmf_step")
+            self.steps_done += 1
+        return losses
+
+    def train_batches(self, users: torch.Tensor, pos: torch.Tensor, neg: torch.Tensor | None = None) -> torch.Tensor:
+        """``run_batches(plan_batches(...))``."""
+        return self.run_batches(self.plan_batches(users, pos, neg))
+
+    def step(self, users: torch.Tensor, pos: torch.Tensor, neg: torch.Tensor | None = None) -> torch.Tensor:
+        """One minibatch (at most ``batch_size`` samples); the loss as a device scalar."""
+        if users.numel() > self.batch_size:
+            raise ValueError(f"a step takes at most batch_size={self.batch_size} samples")
+        return self.train_batches(users, pos, neg)[0]
+
+    def epoch(self, perm: torch.Tensor) -> torch.Tensor:
+        """One pass over the training interactions in the order ``perm``; the batch losses (device)."""
+        perm = perm.to(self.device, torch.int64)
+        return self.train_batches(self.users[perm], self.items[perm])

@@ -1,0 +1,261 @@
+"""
+FlexMF implicit-feedback scorer on the H100 engine — the component surface of
+``lenskit.flexmf.FlexMFImplicitScorer`` (``src/lenskit/flexmf/_implicit.py``, ``_base.py``, ``_training.py``,
+``_model.py``): matrix factorisation trained by minibatch Adam on the logistic or the pairwise (BPR) loss over
+sampled negatives.
+
+Same config fields, aliases, presets and defaults, the same initial parameters for a seed (torch's ``normal_`` on a
+CPU generator: user bias, item bias, user embeddings, item embeddings; rows without interactions zeroed), the same
+first-epoch sample order (``rng.permutation``), and the same step mathematics to rounding.  What differs:
+
+* negatives are drawn on the device by ``lk_flexmf_sample_negatives`` from this library's counter-based generator,
+  seeded once per trainer from the NumPy generator, not from the reference's PCG64 stream;
+* a step is ``lk_flexmf_step`` (no autograd, no float atomics): two trainings with one seed are bit-identical;
+* ``loss="warp"`` / ``negative_strategy="misranked"`` and ``convolution_layers > 0`` (LightGCN) are rejected when the
+  configuration is made.
+
+Inference is ``ub + ib + u·i``: the ALS scorers' batched scoring and fused top-n (``lk_als_recommend_batch``) with
+the item bias as the item offset and the user bias as the query offset.
+"""
+
+from __future__ import annotations
+
+from typing import Literal
+
+import numpy as np
+import torch
+from pydantic import BaseModel, NonNegativeInt, PositiveFloat, PositiveInt, field_validator, model_validator
+
+from . import _lib, engine
+from .als import ALSBase, _as_dataset
+from .components import ItemList, ModelTrainer, RecQuery, TrainingOptions, Vocabulary
+
+PRESETS = {"bpr": {"loss": "pairwise", "user_bias": False, "item_bias": False}}
+PARAM_NAMES = ("u_bias.weight", "i_bias.weight", "u_embed.weight", "i_embed.weight")
+
+
+class FlexMFImplicitConfig(BaseModel):
+    embedding_size: PositiveInt = 64
+    batch_size: PositiveInt = 8 * 1024
+    learning_rate: float = 0.01
+    epochs: int = 10
+    regularization: float = 0.01
+    reg_method: Literal["AdamW", "L2"] | None = "AdamW"
+    preset: Literal["bpr", "warp", "lightgcn"] | None = None
+    loss: Literal["logistic", "pairwise", "warp"] = "logistic"
+    negative_strategy: Literal["uniform", "popular", "misranked"] | None = None
+    negative_count: PositiveInt = 1
+    positive_weight: PositiveFloat = 1.0
+    user_bias: bool | None = None
+    item_bias: bool = True
+    convolution_layers: NonNegativeInt = 0
+
+    @model_validator(mode="before")
+    @classmethod
+    def apply_aliases_and_preset(cls, data):
+        if not isinstance(data, dict):
+            return data
+        if "embedding_size_exp" in data:  # EmbeddingSizeMixin: the size as a power of two
+            data = {k: v for k, v in data.items() if k not in ("embedding_size_exp", "embedding_size")} | {
+                "embedding_size": 2 ** data["embedding_size_exp"]
+            }
+        preset = data.get("preset")
+        if preset in ("warp", "lightgcn"):
+            raise ValueError(f"preset={preset!r} is not covered by the engine (DESIGN.md §6)")
+        if preset is not None:
+            if preset not in PRESETS:
+                raise ValueError(f"unknown preset '{preset}'")
+            data = PRESETS[preset] | data
+        return data
+
+    @field_validator("embedding_size", mode="after")
+    @staticmethod
+    def check_embedding_size(k) -> int:
+        if k > engine.ALS_MAX_FEATURES:
+            raise ValueError(f"embedding_size={k} exceeds the engine limit of {engine.ALS_MAX_FEATURES}")
+        return k
+
+    @model_validator(mode="after")
+    def check_covered(self):
+        if self.loss == "warp":
+            raise ValueError("loss='warp' is not covered by the engine (DESIGN.md §6)")
+        if self.negative_strategy == "misranked":
+            raise ValueError("negative_strategy='misranked' is not covered by the engine (DESIGN.md §6)")
+        if self.convolution_layers > 0:
+            raise ValueError("convolution_layers > 0 (LightGCN) is not covered by the engine (DESIGN.md §6)")
+        return self
+
+    def selected_negative_strategy(self) -> str:
+        return self.negative_strategy or "uniform"
+
+    def selected_user_bias(self) -> bool:
+        return self.loss == "logistic" if self.user_bias is None else self.user_bias
+
+
+def _torch_seed(rng_input) -> int | None:
+    """
+    The integer a ``TrainingOptions.rng`` value seeds torch with, chosen so that the initial parameters equal the
+    reference's for the same value: an integer is itself, a seed sequence (or the sequence of integers that makes
+    one) gives its first 32-bit state word, a bit generator its next raw output, and a NumPy generator one draw from
+    the int32 range, which moves that generator on.  ``None`` leaves torch's default seed.
+    """
+    if rng_input is None or isinstance(rng_input, (int, np.integer)):
+        return None if rng_input is None else int(rng_input)
+    if isinstance(rng_input, np.random.Generator):
+        return int(rng_input.integers(-(2**31), 2**31 - 1))
+    if isinstance(rng_input, np.random.BitGenerator):
+        return int(rng_input.random_raw())
+    words = rng_input if isinstance(rng_input, np.random.SeedSequence) else np.random.SeedSequence(rng_input)
+    return int(words.generate_state(1)[0])
+
+
+def _torch_generator(rng_input) -> torch.Generator:
+    gen, seed = torch.Generator(), _torch_seed(rng_input)
+    return gen if seed is None else gen.manual_seed(seed)
+
+
+def initial_parameters(n_users: int, n_items: int, k: int, user_bias: bool, item_bias: bool, gen: torch.Generator,
+                       user_counts=None, item_counts=None) -> dict[str, torch.Tensor]:  # fmt: skip
+    """The reference's initial model (``_model.py:84-90``, ``_training.py:108-112``) as a state dict on the CPU."""
+    shapes = {"u_bias.weight": (n_users, 1), "i_bias.weight": (n_items, 1), "u_embed.weight": (n_users, k),
+              "i_embed.weight": (n_items, k)}  # fmt: skip
+    have = {"u_bias.weight": user_bias, "i_bias.weight": item_bias, "u_embed.weight": True, "i_embed.weight": True}
+    out = {}
+    for name in PARAM_NAMES:
+        if have[name]:
+            out[name] = torch.nn.init.normal_(torch.empty(shapes[name], dtype=torch.float32), std=0.1, generator=gen)
+    for prefix, counts in (("u_", user_counts), ("i_", item_counts)):
+        if counts is not None:
+            empty = torch.as_tensor(np.asarray(counts) == 0)
+            for name, t in out.items():
+                if name.startswith(prefix):
+                    t[empty] = 0
+    return out
+
+
+class FlexMFImplicitScorer(ALSBase):
+    """``FlexMFImplicitScorer``: ``train``, ``__call__``, and the batched ``score_matrix`` / ``score_batch`` /
+    ``recommend_batch`` (inherited from the ALS scorers, with the biases as the kernel's offsets)."""
+
+    CONFIG_CLASS = FlexMFImplicitConfig
+    config: FlexMFImplicitConfig
+    user_bias: np.ndarray | None = None
+    item_bias: np.ndarray | None = None
+
+    def create_trainer(self, data, options):
+        return FlexMFImplicitTrainer(self, data, options)
+
+    def embed_batch(self, queries):
+        """Known users' embeddings; a query without a known user is unscorable (``_base.py:126-133``)."""
+        dev = _lib.require_device()
+        queries = [RecQuery.create(q) for q in queries]
+        nums = [None if q.user_id is None else self.users.number(q.user_id, missing=None) for q in queries]
+        user_nums = np.array([-1 if u is None else u for u in nums], dtype=np.int64)
+        scorable = user_nums >= 0
+        X = np.zeros((len(queries), self.item_embeddings.shape[1]), dtype=np.float32)
+        X[scorable] = self.user_embeddings[user_nums[scorable]]
+        return torch.from_numpy(X).to(dev), scorable, user_nums, None
+
+    def batch_offsets(self, user_nums: np.ndarray, fold_bias):
+        ub = None
+        if self.user_bias is not None:
+            ub = np.where(user_nums >= 0, self.user_bias[np.maximum(user_nums, 0)], 0.0).astype(np.float32)
+        return self.item_bias, ub
+
+    def score_batch(self, queries, targets: list[ItemList]) -> list[ItemList]:
+        """Score ``targets[i]`` for ``queries[i]``: columns of :meth:`score_matrix` picked out on the device.
+        Unknown items, and every item of a query without a known user, score NaN."""
+        S = self.score_matrix(queries)
+        out = []
+        for b, tgt in enumerate(targets):
+            tn = tgt.numbers(vocabulary=self.items, missing="negative").astype(np.int64)
+            s = np.full(len(tn), np.nan, dtype=np.float32)
+            ok = tn >= 0
+            if ok.any():
+                s[ok] = S[torch.from_numpy(tn[ok]).to(S.device), b].cpu().numpy()
+            out.append(ItemList(tgt, scores=s))
+        return out
+
+    def __call__(self, query, items: ItemList) -> ItemList:
+        return self.score_batch([query], [items])[0]
+
+    def __getstate__(self):
+        d = dict(self.__dict__)
+        d.pop("_d_items_cache", None)  # host arrays are the pickled state
+        return d
+
+
+class FlexMFImplicitTrainer(ModelTrainer):
+    """``FlexMFImplicitTrainer`` (``_implicit.py:164-290`` over ``_training.py:39-258``) with device-resident state."""
+
+    def __init__(self, scorer: FlexMFImplicitScorer, data, options: TrainingOptions):
+        from .prep import DeviceInteractions
+
+        self.scorer = scorer
+        self.device = _lib.require_device()
+        self.rng = options.random_generator()
+        torch_rng = _torch_generator(options.rng)
+        if isinstance(data, DeviceInteractions):
+            scorer.users = Vocabulary(np.arange(data.n_users), "user")
+            scorer.items = Vocabulary(np.arange(data.n_items), "item")
+            users, items, n_users, n_items = data.users, data.items, data.n_users, data.n_items
+        else:
+            ds = _as_dataset(data)
+            scorer.users, scorer.items = ds.users, ds.items
+            it = ds.interactions
+            users, items, n_users, n_items = torch.from_numpy(it.users), torch.from_numpy(it.items), it.n_users, it.n_items
+        users, items = users.to(self.device), items.to(self.device)
+        c = self.config
+        params = initial_parameters(
+            n_users, n_items, c.embedding_size, c.selected_user_bias(), c.item_bias, torch_rng,
+            torch.bincount(users.long(), minlength=n_users).cpu().numpy(),
+            torch.bincount(items.long(), minlength=n_items).cpu().numpy(),
+        )  # fmt: skip
+        self.state = engine.FlexMFState(
+            params, users, items, loss=c.loss, reg_method=c.reg_method, negative_count=c.negative_count,
+            popular=c.selected_negative_strategy() == "popular", batch_size=c.batch_size,
+            learning_rate=c.learning_rate, regularization=c.regularization, positive_weight=c.positive_weight,
+            device=self.device,
+        )  # fmt: skip
+        self._seeded = False
+        self.n_samples = int(users.numel())
+        self.epochs_trained = 0  # the scorer gets its host arrays after the first epoch: until then it is not trained
+
+    @property
+    def config(self) -> FlexMFImplicitConfig:
+        return self.scorer.config
+
+    def epoch_permutation(self) -> np.ndarray:
+        """The epoch's sample order, as the reference draws it (``_training.py:205-215``)."""
+        return np.require(self.rng.permutation(self.n_samples), dtype=np.int32)
+
+    def train_epoch(self) -> dict[str, float]:
+        perm = self.epoch_permutation()
+        if not self._seeded:
+            # after the first permutation, so that the first epoch's order is the reference's for the same seed
+            self.state.seed = int(self.rng.integers(0, 2**63))
+            self._seeded = True
+        losses = self.state.epoch(torch.from_numpy(perm))
+        loss = float(losses.double().mean().item())  # the epoch's one read of the batch losses
+        self.epochs_trained += 1
+        self._sync_host()
+        return {"loss": loss}
+
+    def _sync_host(self) -> None:
+        p = {n: t.cpu().numpy() for n, t in self.state.params.items()}
+        s = self.scorer
+        s.user_embeddings, s.item_embeddings = p["u_embed.weight"], p["i_embed.weight"]
+        s.user_bias = p["u_bias.weight"][:, 0].copy() if "u_bias.weight" in p else None
+        s.item_bias = p["i_bias.weight"][:, 0].copy() if "i_bias.weight" in p else None
+
+    def finalize(self) -> None:
+        self._sync_host()
+        del self.state
+
+    def get_parameters(self) -> dict[str, object]:
+        return {n: t.cpu() for n, t in self.state.params.items()}
+
+    def load_parameters(self, state) -> None:
+        for n, t in self.state.params.items():
+            t.copy_(torch.as_tensor(state[n]).to(torch.float32).reshape(t.shape))
+        self._sync_host()
