@@ -205,54 +205,28 @@ class ALSBase(UsesTrainer, Component):
         ``recommend_batch`` defaults to ``"query"``.)  An unscorable query gets an empty list.  The kernel sweeps
         every item once per 64 queries, so batch widely.
         """
-        from .knn import _check_exclude
+        from .batch import check_exclude, empty_list, history_csr, rank_size, ranked_lists
 
-        _check_exclude(exclude)
+        check_exclude(exclude)
         queries = [RecQuery.create(q) for q in queries]
-        n_items = self.item_embeddings.shape[0]
-        n_eff = min(int(n), n_items)
-        if n_eff <= 0:
-            return [ItemList([], scores=np.empty(0, dtype=np.float32)) for _ in queries]
-        n_max = int(_lib.lib().lk_topn_max())
-        if n_eff > n_max:
-            raise ValueError(f"n={n_eff} exceeds the engine limit of {n_max}")
+        n_eff = rank_size(n, self.item_embeddings.shape[0])
+        if n_eff == 0:
+            return [empty_list(self.items) for _ in queries]
         X, scorable, user_nums, fold_bias = self.embed_batch(queries)
-        out = [_empty_list(self.items) for _ in queries]
         at = np.flatnonzero(scorable)
         if len(at) == 0:
-            return out
+            return [empty_list(self.items) for _ in queries]
         dev = X.device
         item_off, query_off = self._offsets(user_nums, fold_bias, dev)
-        excl_ptr = excl_items = None
+        excl = (None, None)
         if exclude == "query":
-            ptr_, nums = [0], []
-            for b in at:
-                qi = queries[b].query_items
-                e = qi.numbers(vocabulary=self.items, missing="negative") if qi is not None else np.zeros(0)
-                nums.append(np.asarray(e, dtype=np.int32))
-                ptr_.append(ptr_[-1] + len(e))
-            excl_ptr = torch.tensor(ptr_, dtype=torch.int64, device=dev)
-            excl_items = torch.from_numpy(np.concatenate(nums)).to(dev)
+            excl = history_csr([queries[b] for b in at], self.items, dev)[1:]
         sel = torch.from_numpy(at).to(dev)
         idx, val, cnt = engine.als_recommend(
             self._device_items(), X[sel].contiguous(), n_eff, item_off,
-            query_off[sel] if query_off is not None else None, excl_ptr, excl_items,
+            query_off[sel] if query_off is not None else None, *excl,
         )  # fmt: skip
-        idx, val, cnt = idx.cpu().numpy(), val.cpu().numpy(), cnt.cpu().numpy()
-        for j, b in enumerate(at):
-            c = int(cnt[j])
-            out[b] = ItemList(
-                item_ids=self.items.ids(idx[j, :c]), item_nums=idx[j, :c].copy(), vocabulary=self.items,
-                scores=val[j, :c].copy(),
-            )  # fmt: skip
-        return out
-
-
-def _empty_list(vocabulary) -> ItemList:
-    return ItemList(
-        item_ids=vocabulary.ids(np.zeros(0, np.int32)), item_nums=np.zeros(0, np.int32), vocabulary=vocabulary,
-        scores=np.zeros(0, np.float32),
-    )  # fmt: skip
+        return ranked_lists(self.items, len(queries), at, idx, val, cnt)
 
 
 def _solve_cholesky(A: np.ndarray, y: np.ndarray) -> np.ndarray:

@@ -21,8 +21,8 @@ from pydantic import BaseModel, NonNegativeFloat, PositiveInt
 
 from . import _lib, engine
 from .als import _as_dataset
-from .components import Component, ItemList, RecQuery, Trainable, TrainingOptions
-from .knn import _check_exclude, _empty_list
+from .components import Component, ItemList, Trainable, TrainingOptions
+from .batch import check_exclude, empty_list, history_csr, rank_size, ranked_lists, target_scores
 
 
 class AssociationConfig(BaseModel, extra="forbid"):
@@ -65,15 +65,7 @@ class AssociationScorer(Component, Trainable):
         """Association values, reference items on rows and targets on columns (SciPy ``csr_array``, rows sorted)."""
         m = self.__dict__.get("_assoc_host")
         if m is None:
-            import scipy.sparse as sps
-
-            st = self._state
-            n = st.n_items
-            nnz = int(st.indptr[-1].item())
-            m = sps.csr_array(
-                (st.vals[:nnz].cpu().numpy(), st.cols[:nnz].cpu().numpy(), st.indptr.cpu().numpy()), shape=(n, n)
-            )
-            self._assoc_host = m
+            m = self._assoc_host = self._state.host_csr()
         return m
 
     def _device_state(self) -> engine.AssocState:
@@ -97,36 +89,13 @@ class AssociationScorer(Component, Trainable):
             return 1
         raise NotImplementedError("limited reference items not yet implemented")  # association.py:155
 
-    def _refs(self, queries, dev) -> tuple[list[np.ndarray], torch.Tensor, torch.Tensor]:
-        """Each query's known reference items in query order (repeats kept), and the batch as a device CSR."""
-        refs = []
-        for q in queries:
-            hist = RecQuery.create(q).query_items
-            if hist is None or len(hist) == 0:
-                refs.append(np.zeros(0, np.int32))
-                continue
-            r = hist.numbers(vocabulary=self.items, missing="negative").astype(np.int32)
-            refs.append(r[r >= 0])
-        ptr = np.concatenate([[0], np.cumsum([len(r) for r in refs])]).astype(np.int64)
-        items = np.concatenate(refs) if refs else np.zeros(0, np.int32)
-        return refs, torch.from_numpy(ptr).to(dev), torch.from_numpy(items.astype(np.int32)).to(dev)
-
     def score_batch(self, queries, targets: list[ItemList]) -> list[ItemList]:
         """Score ``targets[i]`` for query ``queries[i]`` (a history ``ItemList`` or a ``RecQuery``), in one launch."""
         agg = self._agg()
         st = self._device_state()
         dev = st.indptr.device
-        _refs, r_ptr, r_items = self._refs(queries, dev)
-        scores = st.score(r_ptr, r_items, agg)
-        out = []
-        for b, tgt in enumerate(targets):
-            tn = tgt.numbers(vocabulary=self.items, missing="negative").astype(np.int64)
-            s = np.full(len(tn), np.nan, dtype=np.float32)
-            ok = tn >= 0
-            if ok.any():
-                s[ok] = scores[b, torch.from_numpy(tn[ok]).to(dev)].cpu().numpy()
-            out.append(ItemList(tgt, scores=s))
-        return out
+        _has, r_ptr, r_items = history_csr(queries, self.items, dev)
+        return target_scores(st.score(r_ptr, r_items, agg), targets, self.items)
 
     def __call__(self, query, items: ItemList) -> ItemList:
         return self.score_batch([query], [items])[0]
@@ -138,21 +107,14 @@ class AssociationScorer(Component, Trainable):
         ``__call__`` and ``TopNRanker``, bit for bit.  Zero scores are ranked like any other; a query without known
         reference items gets an empty list.
         """
-        _check_exclude(exclude)
+        check_exclude(exclude)
         agg = self._agg()
         st = self._device_state()
         dev = st.indptr.device
-        n_eff = min(int(n), st.n_items)
-        if n_eff <= 0:
-            return [_empty_list(self.items) for _ in queries]
-        if n_eff > int(_lib.lib().lk_topn_max()):
-            raise ValueError(f"n={n_eff} exceeds the engine limit of {int(_lib.lib().lk_topn_max())}")
-        _refs, r_ptr, r_items = self._refs(queries, dev)
+        n_eff = rank_size(n, st.n_items)
+        if n_eff == 0:
+            return [empty_list(self.items) for _ in queries]
+        _has, r_ptr, r_items = history_csr(queries, self.items, dev)
         excl = (r_ptr, r_items) if exclude == "query" else (None, None)
-        idx, val, cnt = (t.cpu().numpy() for t in st.recommend(r_ptr, r_items, agg, n_eff, *excl))
-        out = []
-        for b in range(len(cnt)):
-            c = int(cnt[b])
-            out.append(ItemList(item_ids=self.items.ids(idx[b, :c]), item_nums=idx[b, :c].copy(),
-                                vocabulary=self.items, scores=val[b, :c].copy()))  # fmt: skip
-        return out
+        idx, val, cnt = st.recommend(r_ptr, r_items, agg, n_eff, *excl)
+        return ranked_lists(self.items, len(queries), range(len(queries)), idx, val, cnt)

@@ -59,19 +59,6 @@ static size_t ar_smem_bytes(bool rank, int k, int n)
     return b;
 }
 
-// one query's heap, entry p at [p * AR_QT] (the CTA's heaps interleaved)
-struct ArHeap {
-    struct Ent {
-        float v;
-        int32_t k;
-    };
-    float *hv;
-    int32_t *hk;
-    __device__ __forceinline__ float val(const int p) const { return hv[p * AR_QT]; }
-    __device__ __forceinline__ Ent get(const int p) const { return {hv[p * AR_QT], hk[p * AR_QT]}; }
-    __device__ __forceinline__ void put(const int p, const Ent e) { hv[p * AR_QT] = e.v, hk[p * AR_QT] = e.k; }
-};
-
 template <bool RANK>
 __global__ void __launch_bounds__(AR_THREADS, 2) als_recommend_kernel(const lk_als_rec_args a)
 {
@@ -97,10 +84,10 @@ __global__ void __launch_bounds__(AR_THREADS, 2) als_recommend_kernel(const lk_a
     const int my_b = q0 + tid;
     const bool selector = RANK && tid < AR_QT && my_b < B;
     int64_t *s_ec = reinterpret_cast<int64_t *>(s_root + AR_QT);
-    auto my_heap = [&]() {
+    auto my_heap = [&]() {  // one query's heap, interleaved with the CTA's others
         float *hv = n <= AR_HEAP_SMEM_N ? reinterpret_cast<float *>(s_ec + AR_QT)
                                         : reinterpret_cast<float *>(a.d_workspace) + (size_t)blockIdx.x * AR_QT * n * 2;
-        return ArHeap{hv + tid, reinterpret_cast<int32_t *>(hv + AR_QT * n) + tid};
+        return PairHeap<AR_QT>{hv + tid, reinterpret_cast<int32_t *>(hv + AR_QT * n) + tid};
     };
     if constexpr (RANK) {
         if (tid < AR_QT) {
@@ -215,7 +202,7 @@ __global__ void __launch_bounds__(AR_THREADS, 2) als_recommend_kernel(const lk_a
                 int64_t ec = s_ec[tid];
                 int count = s_cnt[tid];
                 float root = s_root[tid];
-                ArHeap heap = my_heap();
+                PairHeap<AR_QT> heap = my_heap();
 #pragma unroll 1
                 for (int w = 0; w < 4; w++) {
                     uint32_t m = mask[w * AR_QT + tid];
@@ -225,9 +212,8 @@ __global__ void __launch_bounds__(AR_THREADS, 2) als_recommend_kernel(const lk_a
                         const int il = w * 32 + __ffs(m) - 1;
                         m &= m - 1u;
                         const int32_t item = (int32_t)(t0 + il);
-                        while (ec < ee && ex[ec] < item) ec++;
-                        if (ec < ee && ex[ec] == item) continue;  // excluded: argtopn's NaN offer
-                        topn_heap_offer(heap, count, root, n, ArHeap::Ent{U[il * AR_SS + tid], item});
+                        if (topn_excluded(ex, ec, ee, item)) continue;  // argtopn's NaN offer
+                        topn_heap_offer(heap, count, root, n, PairHeap<AR_QT>::Ent{U[il * AR_SS + tid], item});
                     } while (m != 0u);
                 }
                 s_cnt[tid] = count;
@@ -239,7 +225,7 @@ __global__ void __launch_bounds__(AR_THREADS, 2) als_recommend_kernel(const lk_a
 
     if (selector) {
         const int count = s_cnt[tid];
-        ArHeap heap = my_heap();
+        PairHeap<AR_QT> heap = my_heap();
         topn_heap_sort(heap, count);
         const int64_t o = (int64_t)my_b * n;
         for (int t = 0; t < n; t++) {
@@ -287,8 +273,8 @@ int lk_als_recommend_batch(const lk_als_rec_args *args, void *stream)
     LK_REQUIRE(a.n_items < (int64_t)INT32_MAX, LK_ERR_UNSUPPORTED, "lk_als_recommend_batch: int32 item numbers");
     const bool rank = a.n != 0;
     if (rank) {
-        LK_REQUIRE(a.n >= 1 && a.n <= lk_topn_max(), LK_ERR_UNSUPPORTED,
-                   "lk_als_recommend_batch: n must be 0 (score mode) or in 1..%d", lk_topn_max());
+        LK_REQUIRE(a.n >= 1 && a.n <= TOPN_MAX, LK_ERR_UNSUPPORTED,
+                   "lk_als_recommend_batch: n must be 0 (score mode) or in 1..%d", TOPN_MAX);
         LK_REQUIRE(a.d_excl_indptr == nullptr || a.d_excl_items != nullptr, LK_ERR_INVALID,
                    "lk_als_recommend_batch: d_excl_items is required with d_excl_indptr");
         LK_REQUIRE(lk_als_recommend_workspace_bytes(a.n_queries, a.n) == 0 || a.d_workspace != nullptr,

@@ -28,10 +28,9 @@ namespace lk {
 
 constexpr int CO_WARPS = 16;
 constexpr int CO_NT = CO_WARPS * 32;
-constexpr int CO_HEAP_MAX = 1024;  // lk_topn_max()
 constexpr int CO_CTAS = 2;
 
-constexpr int CO_FIXED_SMEM = CO_HEAP_MAX * 8 + CO_WARPS * 4 + 16;  // argtopn heap, per-warp counts
+constexpr int CO_FIXED_SMEM = TOPN_MAX * 8 + CO_WARPS * 4 + 16;  // argtopn heap, per-warp counts
 
 static int co_smem_bytes(const lk_knn_geom &g) { return g.warps * g.tile_cols * 4 + CO_FIXED_SMEM; }
 
@@ -186,18 +185,6 @@ __global__ void assoc_tile_ptr_kernel(const lk_knn_geom g, const int64_t *__rest
     }
 }
 
-struct CoHeap {
-    struct Ent {
-        float v;
-        int32_t k;
-    };
-    float *hv;
-    int32_t *hk;
-    __device__ __forceinline__ float val(const int p) const { return hv[p]; }
-    __device__ __forceinline__ Ent get(const int p) const { return {hv[p], hk[p]}; }
-    __device__ __forceinline__ void put(const int p, const Ent e) { hv[p] = e.v, hk[p] = e.k; }
-};
-
 template <bool RANK>
 __global__ void __launch_bounds__(CO_NT, CO_CTAS) assoc_score_kernel(const lk_assoc_score_args a)
 {
@@ -207,7 +194,7 @@ __global__ void __launch_bounds__(CO_NT, CO_CTAS) assoc_score_kernel(const lk_as
     const int TW = g.tile_cols, S1 = g.n_subtiles + 1, H = g.n_halves, NI = g.n_items;
     const int CW = W * TW;
     float *acc = reinterpret_cast<float *>(smem_raw);  // [CW]
-    CoHeap heap{acc + CW, reinterpret_cast<int32_t *>(acc + CW + CO_HEAP_MAX)};
+    PairHeap<1> heap{acc + CW, reinterpret_cast<int32_t *>(acc + CW + TOPN_MAX)};
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int q = RANK ? (int)blockIdx.x : (int)(blockIdx.x / H);
@@ -293,9 +280,8 @@ __global__ void __launch_bounds__(CO_NT, CO_CTAS) assoc_score_kernel(const lk_as
                             const int l = __ffs(b) - 1;
                             b &= b - 1u;
                             const int item = h * CW + j0 + l;
-                            while (ec < ee && ex[ec] < item) ec++;
-                            if (ec < ee && ex[ec] == item) continue;  // excluded: argtopn's NaN offer
-                            topn_heap_offer(heap, count, root, n, CoHeap::Ent{acc[j0 + l], item});
+                            if (topn_excluded(ex, ec, ee, item)) continue;  // argtopn's NaN offer
+                            topn_heap_offer(heap, count, root, n, PairHeap<1>::Ent{acc[j0 + l], item});
                         }
                     }
                     count = __shfl_sync(FULL, count, 0);
@@ -455,8 +441,8 @@ int lk_assoc_score_batch(const lk_assoc_score_args *args, void *stream)
                "lk_assoc_score_batch: n_queries * n_halves must be < 2^31");
     const bool rank = a.n != 0;
     if (rank)
-        LK_REQUIRE(a.n >= 1 && a.n <= CO_HEAP_MAX, LK_ERR_UNSUPPORTED,
-                   "lk_assoc_score_batch: n must be 0 (score mode) or in 1..%d", CO_HEAP_MAX);
+        LK_REQUIRE(a.n >= 1 && a.n <= TOPN_MAX, LK_ERR_UNSUPPORTED,
+                   "lk_assoc_score_batch: n must be 0 (score mode) or in 1..%d", TOPN_MAX);
     if (a.n_queries == 0) return LK_OK;
     LK_REQUIRE(a.d_indptr && a.d_cols && a.d_vals && a.d_tile_ptr && a.d_ref_indptr && a.d_ref_items, LK_ERR_INVALID,
                "lk_assoc_score_batch: null input");

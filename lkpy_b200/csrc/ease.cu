@@ -21,20 +21,7 @@ namespace lk {
 
 constexpr int EASE_CT = 256;             // compute threads per CTA
 constexpr int EASE_TW = EASE_CT * 4;     // columns per tile
-constexpr int EASE_HEAP_MAX = 1024;      // lk_topn_max()
 constexpr int EASE_UNROLL = 4;           // rows loaded ahead of their adds
-
-struct EaseHeap {
-    struct Ent {
-        float v;
-        int32_t k;
-    };
-    float *hv;
-    int32_t *hk;
-    __device__ __forceinline__ float val(const int p) const { return hv[p]; }
-    __device__ __forceinline__ Ent get(const int p) const { return {hv[p], hk[p]}; }
-    __device__ __forceinline__ void put(const int p, const Ent e) { hv[p] = e.v, hk[p] = e.k; }
-};
 
 // columns c .. c+3 of one row; columns at or beyond NI read as +0.0 (never stored)
 template <bool VEC>
@@ -105,8 +92,8 @@ __global__ void __launch_bounds__(EASE_CT + (RANK ? 32 : 0)) ease_score_kernel(c
         }
     } else {
         __shared__ __align__(16) float buf[2][EASE_TW];
-        __shared__ float s_hv[EASE_HEAP_MAX];
-        __shared__ int32_t s_hk[EASE_HEAP_MAX];
+        __shared__ float s_hv[TOPN_MAX];
+        __shared__ int32_t s_hk[TOPN_MAX];
         const int n = a.n;
         const int64_t o = (int64_t)q * n;
         if (R == 0) {  // no history: nothing is recommended
@@ -119,7 +106,7 @@ __global__ void __launch_bounds__(EASE_CT + (RANK ? 32 : 0)) ease_score_kernel(c
         }
         const bool heap_warp = tid >= EASE_CT;
         const int lane = tid & 31;
-        EaseHeap heap{s_hv, s_hk};
+        PairHeap<1> heap{s_hv, s_hk};
         int count = 0;  // heap warp: heap size and root, exclusion cursor
         float root = 0.0f;
         int64_t ec = 0, ee = 0;
@@ -139,7 +126,7 @@ __global__ void __launch_bounds__(EASE_CT + (RANK ? 32 : 0)) ease_score_kernel(c
                         const int item = k * EASE_TW + j0 + l;
                         while (ec < ee && a.d_excl_items[ec] < item) ec++;
                         if (ec < ee && a.d_excl_items[ec] == item) continue;  // excluded: argtopn's NaN offer
-                        topn_heap_offer(heap, count, root, n, EaseHeap::Ent{b[j0 + l], item});
+                        topn_heap_offer(heap, count, root, n, PairHeap<1>::Ent{b[j0 + l], item});
                     }
                 }
                 count = __shfl_sync(FULL, count, 0);
@@ -199,8 +186,8 @@ int lk_ease_score_batch(const lk_ease_score_args *args, void *stream)
                "lk_ease_score_batch: n_queries * column tiles must be < 2^31");
     const bool rank = a.n != 0;
     if (rank)
-        LK_REQUIRE(a.n >= 1 && a.n <= EASE_HEAP_MAX, LK_ERR_UNSUPPORTED,
-                   "lk_ease_score_batch: n must be 0 (score mode) or in 1..%d", EASE_HEAP_MAX);
+        LK_REQUIRE(a.n >= 1 && a.n <= TOPN_MAX, LK_ERR_UNSUPPORTED,
+                   "lk_ease_score_batch: n must be 0 (score mode) or in 1..%d", TOPN_MAX);
     if (a.n_queries == 0) return LK_OK;
     LK_REQUIRE(a.d_w && a.d_hist_indptr && a.d_hist_items, LK_ERR_INVALID, "lk_ease_score_batch: null input");
     if (rank) {

@@ -430,15 +430,14 @@ __device__ __forceinline__ int block_excl_scan(int v, int *s_scan, int *s_carry,
 // them to the heap of topn_heap.cuh.  The heap and the candidate buffer live in DenseSmem, which steps 1-3 no
 // longer need at that point, so the ranking mode costs no shared memory of its own.
 // ---------------------------------------------------------------------------------------------
-constexpr int RANK_NMAX = 1024;  // lk_topn_max()
 constexpr int RANK_UNITS = 8;    // items per thread and chunk
 constexpr int RANK_CHUNK = DENSE_THREADS * RANK_UNITS;
 constexpr int RANK_WARPS = DENSE_THREADS / 32;
 
 struct RankSmem {
-    float hv[RANK_NMAX];  // heap: score, item number, accumulator length
-    int32_t hk[RANK_NMAX];
-    int32_t hc[RANK_NMAX];
+    float hv[TOPN_MAX];  // heap: score, item number, accumulator length
+    int32_t hk[TOPN_MAX];
+    int32_t hc[TOPN_MAX];
     float cv[RANK_CHUNK];  // the chunk's candidates, in item order
     int32_t ck[RANK_CHUNK];
     int32_t cc[RANK_CHUNK];
@@ -884,8 +883,8 @@ int lk_knn_recommend_batch(const lk_knn_score_args *score, const lk_knn_rank_arg
     if (rc != LK_OK) return rc;
     LK_REQUIRE(a.d_tgt_items == nullptr && a.d_tgt_indptr == nullptr, LK_ERR_INVALID,
                "lk_knn_recommend_batch: ranks all items (dense mode: d_tgt_indptr and d_tgt_items must be NULL)");
-    LK_REQUIRE(rk.n >= 1 && rk.n <= RANK_NMAX && rk.n <= lk_topn_max(), LK_ERR_UNSUPPORTED,
-               "lk_knn_recommend_batch: n must be in 1..%d", lk_topn_max());
+    LK_REQUIRE(rk.n >= 1 && rk.n <= TOPN_MAX, LK_ERR_UNSUPPORTED, "lk_knn_recommend_batch: n must be in 1..%d",
+               TOPN_MAX);
     LK_REQUIRE(rk.d_spill && rk.d_out_idx && rk.d_out_val && rk.d_out_nbrs && rk.d_out_cnt, LK_ERR_INVALID,
                "lk_knn_recommend_batch: null pointer (spill rows or outputs)");
     LK_REQUIRE(rk.d_excl_indptr == nullptr || rk.d_excl_items != nullptr, LK_ERR_INVALID,

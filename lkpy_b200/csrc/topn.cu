@@ -24,19 +24,6 @@
 
 namespace lk {
 
-// the heap in the thread's own arrays (local memory)
-struct TopnLocalHeap {
-    struct Ent {
-        float v;
-        int32_t k;
-    };
-    float *hv;
-    int32_t *hk;
-    __device__ __forceinline__ float val(const int p) const { return hv[p]; }
-    __device__ __forceinline__ Ent get(const int p) const { return {hv[p], hk[p]}; }
-    __device__ __forceinline__ void put(const int p, const Ent e) { hv[p] = e.v, hk[p] = e.k; }
-};
-
 template <int NMAX>
 __global__ void __launch_bounds__(128)
 topn_columns_kernel(const float *__restrict__ scores, const int64_t n_rows, const int64_t n_cols, const int64_t ld,
@@ -47,13 +34,13 @@ topn_columns_kernel(const float *__restrict__ scores, const int64_t n_rows, cons
     if (u >= n_cols) return;
     float hv[NMAX];
     int32_t hk[NMAX];
-    TopnLocalHeap h{hv, hk};
+    PairHeap<1> h{hv, hk};  // the heap in the thread's own arrays (local memory)
     int count = 0;
     float root = 0.0f;  // hv[0] once the heap is full
 
     auto offer = [&](const float s, const int32_t i) {
         if (s != s) return;  // sorting.rs:142 accept = !is_nan
-        topn_heap_offer(h, count, root, n, TopnLocalHeap::Ent{s, i});
+        topn_heap_offer(h, count, root, n, PairHeap<1>::Ent{s, i});
     };
 
     const float *col = scores + u;
@@ -75,8 +62,6 @@ topn_columns_kernel(const float *__restrict__ scores, const int64_t n_rows, cons
     }
     out_cnt[u] = count;
 }
-
-constexpr int TOPN_MAX = 1024;
 
 }  // namespace lk
 

@@ -1,6 +1,10 @@
 // topn_heap.cuh — the one device copy of argtopn's indirect min-heap (src/accel/indirect/heap.rs,
-// src/accel/data/sorting.rs:131-170), shared by topn.cu, the ranking mode of knn_score.cu and
-// als_recommend.cu.
+// src/accel/data/sorting.rs:131-170) and of its output contract, shared by every batched top-n kernel: topn.cu,
+// the ranking mode of knn_score.cu, als_recommend.cu, cooc.cu and ease.cu.
+//
+// The contract: candidates are offered in ascending item order, an excluded item counts as a NaN offer (never
+// accepted), and each query's row of n is written in descending score order, padded with -1 items and NaN scores,
+// beside its count.
 //
 // The heap is reached through a storage policy H so that each kernel keeps its own layout (per-thread local
 // arrays, shared memory, a strided workspace) and its own payload:
@@ -12,6 +16,22 @@
 #pragma once
 
 namespace lk {
+
+constexpr int TOPN_MAX = 1024;  // the largest n of every top-n entry point: lk_topn_max()
+
+// (score, item) entries, entry p at hv[p * STRIDE] and hk[p * STRIDE] (STRIDE > 1 interleaves several heaps)
+template <int STRIDE>
+struct PairHeap {
+    struct Ent {
+        float v;
+        int32_t k;
+    };
+    float *hv;
+    int32_t *hk;
+    __device__ __forceinline__ float val(const int p) const { return hv[p * STRIDE]; }
+    __device__ __forceinline__ Ent get(const int p) const { return {hv[p * STRIDE], hk[p * STRIDE]}; }
+    __device__ __forceinline__ void put(const int p, const Ent e) { hv[p * STRIDE] = e.v, hk[p * STRIDE] = e.k; }
+};
 
 // heap.rs:67-89 downheap: the smaller child, the left one on a tie, while strictly smaller than the moving entry
 template <class H>
@@ -71,6 +91,14 @@ __device__ __forceinline__ void topn_heap_sort(H &h, const int count)
         h.put(m, t);
         topn_heap_down(h, 0, m);
     }
+}
+
+// whether item is among the query's ascending exclusions ex[ec .. ee), advancing the cursor ec past smaller items;
+// items are asked in ascending order, and an excluded item is argtopn's NaN offer
+__device__ __forceinline__ bool topn_excluded(const int32_t *ex, int64_t &ec, const int64_t ee, const int item)
+{
+    while (ec < ee && ex[ec] < item) ec++;
+    return ec < ee && ex[ec] == item;
 }
 
 }  // namespace lk

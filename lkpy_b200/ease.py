@@ -27,8 +27,8 @@ from pydantic import BaseModel, PositiveFloat
 
 from . import _lib, engine
 from .als import _as_dataset
-from .components import Component, ItemList, RecQuery, Trainable, TrainingOptions
-from .knn import _check_exclude, _empty_list
+from .components import Component, ItemList, Trainable, TrainingOptions
+from .batch import check_exclude, empty_list, history_csr, rank_size, ranked_lists, target_scores
 
 MIN_SCIPY_VERSION = "1.17"
 #: one device Cholesky at a time (ease.py's ``_chol_lock``)
@@ -152,33 +152,14 @@ class EASEScorer(Component, Trainable):
         d.pop("_state", None)
         return d
 
-    def _histories(self, queries, dev) -> tuple[torch.Tensor, torch.Tensor]:
-        """Each query's known history items, deduplicated and ascending, as a device CSR."""
-        hists = []
-        for q in queries:
-            hist = RecQuery.create(q).query_items
-            if hist is None or len(hist) == 0:
-                hists.append(np.zeros(0, np.int32))
-                continue
-            h = hist.numbers(vocabulary=self.items, missing="negative")
-            hists.append(h[h >= 0])
-        return engine.ease_histories(hists, dev)
-
     def score_batch(self, queries, targets: list[ItemList]) -> list[ItemList]:
         """Score ``targets[i]`` for query ``queries[i]`` (a history ``ItemList`` or a ``RecQuery``), in one launch.
         Unknown targets, and every target of a query without known history items, score NaN."""
         st = self._device_state()
         dev = st.weights.device
-        scores = st.score(*self._histories(queries, dev))
-        out = []
-        for b, tgt in enumerate(targets):
-            tn = tgt.numbers(vocabulary=self.items, missing="negative").astype(np.int64)
-            s = np.full(len(tn), np.nan, dtype=np.float32)
-            ok = tn >= 0
-            if ok.any():
-                s[ok] = scores[b, torch.from_numpy(tn[ok]).to(dev)].cpu().numpy()
-            out.append(ItemList(tgt, scores=s))
-        return out
+        # q_vec[q_good] = 1.0 counts a repeated item once: each history ascending without repeats
+        _has, h_ptr, h_items = history_csr(queries, self.items, dev, unique=True)
+        return target_scores(st.score(h_ptr, h_items), targets, self.items)
 
     def __call__(self, query, items: ItemList) -> ItemList:
         return self.score_batch([query], [items])[0]
@@ -190,20 +171,13 @@ class EASEScorer(Component, Trainable):
         ``__call__`` and ``TopNRanker``, bit for bit with the scores of ``score_batch``.  A query without known
         history items gets an empty list.
         """
-        _check_exclude(exclude)
+        check_exclude(exclude)
         st = self._device_state()
         dev = st.weights.device
-        n_eff = min(int(n), st.n_items)
-        if n_eff <= 0:
-            return [_empty_list(self.items) for _ in queries]
-        if n_eff > int(_lib.lib().lk_topn_max()):
-            raise ValueError(f"n={n_eff} exceeds the engine limit of {int(_lib.lib().lk_topn_max())}")
-        h_ptr, h_items = self._histories(queries, dev)
+        n_eff = rank_size(n, st.n_items)
+        if n_eff == 0:
+            return [empty_list(self.items) for _ in queries]
+        _has, h_ptr, h_items = history_csr(queries, self.items, dev, unique=True)
         excl = (h_ptr, h_items) if exclude == "query" else (None, None)
-        idx, val, cnt = (t.cpu().numpy() for t in st.recommend(h_ptr, h_items, n_eff, *excl))
-        out = []
-        for b in range(len(cnt)):
-            c = int(cnt[b])
-            out.append(ItemList(item_ids=self.items.ids(idx[b, :c]), item_nums=idx[b, :c].copy(),
-                                vocabulary=self.items, scores=val[b, :c].copy()))  # fmt: skip
-        return out
+        idx, val, cnt = st.recommend(h_ptr, h_items, n_eff, *excl)
+        return ranked_lists(self.items, len(queries), range(len(queries)), idx, val, cnt)

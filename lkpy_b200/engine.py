@@ -602,16 +602,11 @@ class KnnScorerState:
         lengths, 0 padding; cnt [B] int32)``.
         """
         _check_max_nbrs(max_nbrs)
-        n_max = int(lib().lk_topn_max())
-        if not 1 <= int(n) <= n_max:
-            raise ValueError(f"n must be in 1..{n_max}")
-        n = int(n)
+        n = _check_topn(n)
         dev = self.sim_cols.device
         B = ref_indptr.numel() - 1
-        idx = torch.empty((B, n), dtype=torch.int32, device=dev)
-        val = torch.empty((B, n), dtype=torch.float32, device=dev)
+        idx, val, cnt = _topn_outputs(B, n, dev)
         nbrs = torch.empty((B, n), dtype=torch.int32, device=dev)
-        cnt = torch.empty(max(B, 1), dtype=torch.int32, device=dev)
         if excl_items is not None and excl_items.numel() == 0:  # NULL address; never read (bounded by the indptr)
             excl_items = torch.full((1,), -1, dtype=torch.int32, device=dev)
 
@@ -920,13 +915,9 @@ def topn_columns(scores: torch.Tensor, n: int, with_values: bool = True):
     if scores.dtype != torch.float32 or scores.dim() != 2 or (scores.shape[1] > 1 and scores.stride(1) != 1):
         raise TypeError("scores must be a 2-D float32 tensor with contiguous columns")
     n_rows, n_cols = scores.shape
-    n = int(n)
-    if not 1 <= n <= int(lib().lk_topn_max()):
-        raise ValueError(f"n must be in 1..{int(lib().lk_topn_max())}")
-    dev = scores.device
-    idx = torch.empty((n_cols, n), dtype=torch.int32, device=dev)
-    val = torch.empty((n_cols, n), dtype=torch.float32, device=dev) if with_values else None
-    cnt = torch.empty((max(n_cols, 1),), dtype=torch.int32, device=dev)
+    n = _check_topn(n)
+    idx, val, cnt = _topn_outputs(n_cols, n, scores.device)
+    val = val if with_values else None
     check(
         lib().lk_topn_columns(
             ptr(scores), n_rows, n_cols, scores.stride(0) if n_rows > 1 else max(n_cols, 1), n,
@@ -980,21 +971,45 @@ def als_recommend(
         a.n, a.d_scores = 0, ptr(S)
         check(lib().lk_als_recommend_batch(C.byref(a), stream_ptr()), "lk_als_recommend_batch")
         return S
+    ws_bytes = int(lib().lk_als_recommend_workspace_bytes(B, _check_topn(n)))
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes > 0 else None
+    a.d_workspace = ptr(ws)
+    return _rank_launch(a, lib().lk_als_recommend_batch, "lk_als_recommend_batch", n, n_items, B, dev, excl_indptr,
+                        excl_items)  # fmt: skip
+
+
+def _check_topn(n) -> int:
+    """``n`` as an int, or ``ValueError`` unless it is in 1..``lk_topn_max()``."""
     n_max = int(lib().lk_topn_max())
     if not 1 <= int(n) <= n_max:
         raise ValueError(f"n must be in 1..{n_max}")
-    n = int(n)
-    if excl_indptr is not None:
-        excl_indptr, excl_items = _sorted_exclusions(excl_indptr, excl_items, n_items, B, dev)
+    return int(n)
+
+
+def _topn_outputs(B: int, n: int, dev):
+    """The outputs of a top-n launch over B queries: ``idx [B, n]`` int32, ``val [B, n]`` f32 and ``cnt`` int32
+    (at least one entry, so that its address is never NULL)."""
     idx = torch.empty((B, n), dtype=torch.int32, device=dev)
     val = torch.empty((B, n), dtype=torch.float32, device=dev)
-    cnt = torch.empty(max(B, 1), dtype=torch.int32, device=dev)
-    ws_bytes = int(lib().lk_als_recommend_workspace_bytes(B, n))
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes > 0 else None
-    a.n = n
-    a.d_excl_indptr, a.d_excl_items, a.d_workspace = ptr(excl_indptr), ptr(excl_items), ptr(ws)
-    a.d_out_idx, a.d_out_val, a.d_out_cnt = ptr(idx), ptr(val), ptr(cnt)
-    check(lib().lk_als_recommend_batch(C.byref(a), stream_ptr()), "lk_als_recommend_batch")
+    return idx, val, torch.empty(max(B, 1), dtype=torch.int32, device=dev)
+
+
+def _rank_launch(args, entry, name: str, n: int, n_items: int, B: int, dev, excl_indptr, excl_items):
+    """
+    The rank mode of a fused scoring entry point: sorts the exclusions (:func:`_sorted_exclusions`), sets ``n``, the
+    exclusions and the outputs in ``args``, calls ``entry(args, stream)`` and returns ``(idx [B, n], val [B, n],
+    cnt [B])``.  ``args`` carries the mode's own fields already.
+    """
+    n = _check_topn(n)
+    idx, val, cnt = _topn_outputs(B, n, dev)
+    if B == 0:
+        return idx, val, cnt[:0]
+    if excl_indptr is not None:
+        excl_indptr, excl_items = _sorted_exclusions(excl_indptr, excl_items, n_items, B, dev)
+    args.n = n
+    args.d_excl_indptr, args.d_excl_items = ptr(excl_indptr), ptr(excl_items)
+    args.d_out_idx, args.d_out_val, args.d_out_cnt = ptr(idx), ptr(val), ptr(cnt)
+    check(entry(C.byref(args), stream_ptr()), name)
     return idx, val, cnt[:B]
 
 
@@ -1232,38 +1247,21 @@ class AssocState:
         Top-``n`` of every query over all items minus ``excl_items[excl_indptr[q]:excl_indptr[q+1]]`` (any order),
         with ``argtopn``'s order and ties: ``(idx [B, n] int32, -1 padding; val [B, n] f32, NaN padding; cnt [B])``.
         """
-        n_max = int(lib().lk_topn_max())
-        if not 1 <= int(n) <= n_max:
-            raise ValueError(f"n must be in 1..{n_max}")
-        n, dev, B = int(n), self.indptr.device, ref_indptr.numel() - 1
-        idx = torch.empty((B, n), dtype=torch.int32, device=dev)
-        val = torch.empty((B, n), dtype=torch.float32, device=dev)
-        cnt = torch.empty(max(B, 1), dtype=torch.int32, device=dev)
-        if B == 0:
-            return idx, val, cnt[:0]
-        if excl_indptr is not None:
-            excl_indptr, excl_items = _sorted_exclusions(excl_indptr, excl_items, self.n_items, B, dev)
-        a = self._args(ref_indptr, ref_items, agg)
-        a.n = n
-        a.d_excl_indptr, a.d_excl_items = ptr(excl_indptr), ptr(excl_items)
-        a.d_out_idx, a.d_out_val, a.d_out_cnt = ptr(idx), ptr(val), ptr(cnt)
-        check(lib().lk_assoc_score_batch(C.byref(a), stream_ptr()), "lk_assoc_score_batch")
-        return idx, val, cnt[:B]
+        return _rank_launch(self._args(ref_indptr, ref_items, agg), lib().lk_assoc_score_batch, "lk_assoc_score_batch",
+                            n, self.n_items, ref_indptr.numel() - 1, self.indptr.device, excl_indptr, excl_items)
+
+    def host_csr(self):
+        """The matrix on the host as a SciPy ``csr_array`` (rows sorted)."""
+        import scipy.sparse as sps
+
+        nnz = int(self.indptr[-1].item())
+        return sps.csr_array((self.vals[:nnz].cpu().numpy(), self.cols[:nnz].cpu().numpy(), self.indptr.cpu().numpy()),
+                             shape=(self.n_items, self.n_items))  # fmt: skip
 
 
 # ---------------------------------------------------------------------------
 # EASE scoring
 # ---------------------------------------------------------------------------
-
-
-def ease_histories(hists: list[np.ndarray], dev) -> tuple[torch.Tensor, torch.Tensor]:
-    """The batch's histories as ``lk_ease_score_batch`` takes them: a device CSR (int64 offsets, int32 items), each
-    history deduplicated and ascending (``q_vec[q_good] = 1.0`` counts a repeated item once)."""
-    hs = [np.unique(np.asarray(h, dtype=np.int64)).astype(np.int32) for h in hists]
-    indptr = np.zeros(len(hs) + 1, dtype=np.int64)
-    np.cumsum([len(h) for h in hs], out=indptr[1:])
-    items = np.concatenate(hs) if hs else np.zeros(0, np.int32)
-    return torch.from_numpy(indptr).to(dev), torch.from_numpy(items).to(dev)
 
 
 @dataclass
@@ -1297,7 +1295,7 @@ class EaseState:
     def score(self, hist_indptr: torch.Tensor, hist_items: torch.Tensor) -> torch.Tensor:
         """
         Scores of every item for every query (f32 [B, n_items]): query q's history is ``hist_items[hist_indptr[q]:
-        hist_indptr[q+1]]``, ascending without repeats (:func:`ease_histories`); each score is the f32 sum of the
+        hist_indptr[q+1]]``, ascending without repeats (``batch.history_csr(..., unique=True)``); each score is the f32 sum of the
         history rows' entries in that order; a query without history scores NaN everywhere.
         """
         B = hist_indptr.numel() - 1
@@ -1318,23 +1316,8 @@ class EaseState:
         with ``argtopn``'s order and ties: ``(idx [B, n] int32, -1 padding; val [B, n] f32, NaN padding; cnt [B])``.
         A query without history gets an empty list.
         """
-        n_max = int(lib().lk_topn_max())
-        if not 1 <= int(n) <= n_max:
-            raise ValueError(f"n must be in 1..{n_max}")
-        n, dev, B = int(n), self.weights.device, hist_indptr.numel() - 1
-        idx = torch.empty((B, n), dtype=torch.int32, device=dev)
-        val = torch.empty((B, n), dtype=torch.float32, device=dev)
-        cnt = torch.empty(max(B, 1), dtype=torch.int32, device=dev)
-        if B == 0:
-            return idx, val, cnt[:0]
-        if excl_indptr is not None:
-            excl_indptr, excl_items = _sorted_exclusions(excl_indptr, excl_items, self.n_items, B, dev)
-        a = self._args(hist_indptr, hist_items)
-        a.n = n
-        a.d_excl_indptr, a.d_excl_items = ptr(excl_indptr), ptr(excl_items)
-        a.d_out_idx, a.d_out_val, a.d_out_cnt = ptr(idx), ptr(val), ptr(cnt)
-        check(lib().lk_ease_score_batch(C.byref(a), stream_ptr()), "lk_ease_score_batch")
-        return idx, val, cnt[:B]
+        return _rank_launch(self._args(hist_indptr, hist_items), lib().lk_ease_score_batch, "lk_ease_score_batch", n,
+                            self.n_items, hist_indptr.numel() - 1, self.weights.device, excl_indptr, excl_items)
 
 
 # ---------------------------------------------------------------------------

@@ -28,6 +28,7 @@ from pydantic import BaseModel, NonNegativeInt, PositiveFloat, PositiveInt, fiel
 
 from . import _lib, engine
 from .als import ALSBase, _as_dataset
+from .batch import target_scores
 from .components import ItemList, ModelTrainer, RecQuery, TrainingOptions, Vocabulary
 
 PRESETS = {"bpr": {"loss": "pairwise", "user_bias": False, "item_bias": False}}
@@ -165,16 +166,7 @@ class FlexMFImplicitScorer(ALSBase):
     def score_batch(self, queries, targets: list[ItemList]) -> list[ItemList]:
         """Score ``targets[i]`` for ``queries[i]``: columns of :meth:`score_matrix` picked out on the device.
         Unknown items, and every item of a query without a known user, score NaN."""
-        S = self.score_matrix(queries)
-        out = []
-        for b, tgt in enumerate(targets):
-            tn = tgt.numbers(vocabulary=self.items, missing="negative").astype(np.int64)
-            s = np.full(len(tn), np.nan, dtype=np.float32)
-            ok = tn >= 0
-            if ok.any():
-                s[ok] = S[torch.from_numpy(tn[ok]).to(S.device), b].cpu().numpy()
-            out.append(ItemList(tgt, scores=s))
-        return out
+        return target_scores(self.score_matrix(queries).T, targets, self.items)
 
     def __call__(self, query, items: ItemList) -> ItemList:
         return self.score_batch([query], [items])[0]

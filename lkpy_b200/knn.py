@@ -22,6 +22,7 @@ from pydantic import AliasChoices, BaseModel, Field, PositiveFloat, PositiveInt,
 
 from . import _lib, engine
 from .als import _as_dataset
+from .batch import check_exclude, empty_list, rank_size, ranked_lists
 from .components import Component, ItemList, RecQuery, Trainable, TrainingOptions
 from .data import InteractionCSR, knn_item_matrices
 
@@ -177,15 +178,13 @@ class ItemKNNScorer(Component, Trainable):
         ``exclude="query"``), ``__call__`` and ``TopNRanker``, bit for bit, with ``nbr_counts``.  A query without
         history gets an empty list.
         """
-        _check_exclude(exclude)
+        check_exclude(exclude)
         st = self._device_state()
         dev = st.sim_cols.device
-        n_eff = min(int(n), st.n_items)
+        n_eff = rank_size(n, st.n_items)
         hists = [RecQuery.create(q).query_items for q in queries]
-        if n_eff <= 0:
-            return [_empty_list(self.items) for _ in hists]
-        if n_eff > int(_lib.lib().lk_topn_max()):
-            raise ValueError(f"n={n_eff} exceeds the engine limit of {int(_lib.lib().lk_topn_max())}")
+        if n_eff == 0:
+            return [empty_list(self.items) for _ in hists]
         at, r_ptr, r_items, r_vals = [], [0], [], []
         for i, hist in enumerate(hists):
             if hist is None or len(hist) == 0:  # knn/item.py:238-245: every score is null
@@ -202,9 +201,8 @@ class ItemKNNScorer(Component, Trainable):
             at.append(i)
             r_items.append(rn)
             r_ptr.append(r_ptr[-1] + len(rn))
-        out = [_empty_list(self.items) for _ in hists]
         if not at:
-            return out
+            return [empty_list(self.items) for _ in hists]
         ref_ptr = torch.tensor(r_ptr, dtype=torch.int64, device=dev)
         ref_items = torch.from_numpy(np.concatenate(r_items)).to(dev)
         idx, val, nbrs, cnt = st.recommend(
@@ -216,23 +214,4 @@ class ItemKNNScorer(Component, Trainable):
             excl_indptr=ref_ptr if exclude == "query" else None,
             excl_items=ref_items if exclude == "query" else None,
         )  # fmt: skip
-        idx, val, nbrs, cnt = idx.cpu().numpy(), val.cpu().numpy(), nbrs.cpu().numpy(), cnt.cpu().numpy()
-        for j, i in enumerate(at):
-            c = int(cnt[j])
-            out[i] = ItemList(
-                item_ids=self.items.ids(idx[j, :c]), item_nums=idx[j, :c].copy(), vocabulary=self.items,
-                scores=val[j, :c].copy(), nbr_counts=nbrs[j, :c].copy(),
-            )  # fmt: skip
-        return out
-
-
-def _check_exclude(exclude) -> None:
-    if exclude not in ("query", None):
-        raise ValueError(f'exclude must be "query" or None, not {exclude!r}')
-
-
-def _empty_list(vocabulary) -> ItemList:
-    return ItemList(
-        item_ids=vocabulary.ids(np.zeros(0, np.int32)), item_nums=np.zeros(0, np.int32), vocabulary=vocabulary,
-        scores=np.zeros(0, np.float32),
-    )  # fmt: skip
+        return ranked_lists(self.items, len(hists), at, idx, val, cnt, nbr_counts=nbrs)

@@ -39,7 +39,7 @@ from . import _lib, engine
 from .als import _as_dataset
 from .components import Component, ItemList, RecQuery, Trainable, TrainingOptions
 from .data import InteractionCSR
-from .knn import _check_exclude, _empty_list
+from .batch import check_exclude, empty_list, history_csr, rank_size, ranked_lists
 
 
 class UserKNNConfig(BaseModel, extra="forbid"):
@@ -204,43 +204,31 @@ class UserKNNScorer(Component, Trainable):
         ``exclude="query"``; a query given only a user id excludes nothing), ``__call__`` and ``TopNRanker``, bit
         for bit.  A query without neighbours or usable data gets an empty list.
         """
-        _check_exclude(exclude)
+        check_exclude(exclude)
         st = self._device_state()
         dev = st.sim_cols.device
-        n_eff = min(int(n), st.n_items)
+        n_eff = rank_size(n, st.n_items)
         rqs = [RecQuery.create(q) for q in queries]
-        if n_eff <= 0:
-            return [_empty_list(self.items) for _ in rqs]
-        if n_eff > int(_lib.lib().lk_topn_max()):
-            raise ValueError(f"n={n_eff} exceeds the engine limit of {int(_lib.lib().lk_topn_max())}")
-        specs, at, means, excl = [], [], [], []
+        if n_eff == 0:
+            return [empty_list(self.items) for _ in rqs]
+        specs, at, means = [], [], []
         for i, rq in enumerate(rqs):
             qd = self._query(rq)
             if qd is not None:
                 specs.append(qd[0])
                 at.append(i)
                 means.append(qd[1])
-                ex = np.zeros(0, np.int32)
-                if exclude == "query" and rq.query_items is not None:
-                    ex = rq.query_items.numbers(vocabulary=self.items, missing="negative").astype(np.int32)
-                excl.append(ex)
-        out = [_empty_list(self.items) for _ in rqs]
         if not specs:
-            return out
+            return [empty_list(self.items) for _ in rqs]
         ns = self._neighbour_state()
         nb_indptr, nb_rows, nb_sims = ns.neighbours(ns.queries(specs), self.config.min_sim)
-        e_ptr = np.concatenate([[0], np.cumsum([len(e) for e in excl])]).astype(np.int64)
+        excl = (None, None)
+        if exclude == "query":  # the known items of query_items; a query given only a user id excludes nothing
+            excl = history_csr([rqs[i] for i in at], self.items, dev)[1:]
         idx, val, _nbrs, cnt = st.recommend(
             nb_indptr, nb_rows, nb_sims, self.config.max_nbrs, self.config.min_nbrs, n_eff,
             query_offset=torch.tensor(means, dtype=torch.float32, device=dev),  # scores += umean (user.py:243-244)
-            excl_indptr=torch.from_numpy(e_ptr).to(dev) if exclude == "query" else None,
-            excl_items=torch.from_numpy(np.concatenate(excl)).to(dev) if exclude == "query" else None,
+            excl_indptr=excl[0], excl_items=excl[1],
         )  # fmt: skip
-        idx, val, cnt = idx.cpu().numpy(), val.cpu().numpy(), cnt.cpu().numpy()
-        for j, i in enumerate(at):
-            c = int(cnt[j])  # 0 for a query without neighbours: every score is null
-            out[i] = ItemList(
-                item_ids=self.items.ids(idx[j, :c]), item_nums=idx[j, :c].copy(), vocabulary=self.items,
-                scores=val[j, :c].copy(),
-            )  # fmt: skip
-        return out
+        # cnt is 0 for a query without neighbours: every score is null
+        return ranked_lists(self.items, len(rqs), at, idx, val, cnt)

@@ -24,8 +24,8 @@ from pydantic import BaseModel, PositiveFloat, PositiveInt
 
 from . import _lib, engine
 from .als import _as_dataset
-from .components import Component, ItemList, RecQuery, Trainable, TrainingOptions
-from .knn import _check_exclude, _empty_list
+from .components import Component, ItemList, Trainable, TrainingOptions
+from .batch import check_exclude, empty_list, history_csr, rank_size, ranked_lists, target_scores
 
 _AGG_SUM = 2
 
@@ -86,13 +86,7 @@ class SLIMScorer(Component, Trainable):
         """The transposed SLIM weights, history items on rows and targets on columns (SciPy ``csr_array``)."""
         m = self.__dict__.get("_weights_host")
         if m is None:
-            import scipy.sparse as sps
-
-            st = self._state
-            nnz = int(st.indptr[-1].item())
-            m = sps.csr_array((st.vals[:nnz].cpu().numpy(), st.cols[:nnz].cpu().numpy(), st.indptr.cpu().numpy()),
-                              shape=(st.n_items, st.n_items))  # fmt: skip
-            self._weights_host = m
+            m = self._weights_host = self._state.host_csr()
         return m
 
     def _device_state(self) -> engine.AssocState:
@@ -109,38 +103,13 @@ class SLIMScorer(Component, Trainable):
         d.pop("_state", None)
         return d
 
-    def _refs(self, queries, dev):
-        """Whether each query has a history, and the batch's known history items (query order, repeats kept) as a
-        device CSR."""
-        has, refs = [], []
-        for q in queries:
-            hist = RecQuery.create(q).query_items
-            has.append(hist is not None and len(hist) > 0)
-            if not has[-1]:
-                refs.append(np.zeros(0, np.int32))
-                continue
-            r = hist.numbers(vocabulary=self.items, missing="negative").astype(np.int32)
-            refs.append(r[r >= 0])
-        ptr = np.concatenate([[0], np.cumsum([len(r) for r in refs])]).astype(np.int64)
-        items = np.concatenate(refs) if refs else np.zeros(0, np.int32)
-        return has, torch.from_numpy(ptr).to(dev), torch.from_numpy(items.astype(np.int32)).to(dev)
-
     def score_batch(self, queries, targets: list[ItemList]) -> list[ItemList]:
         """Score ``targets[i]`` for query ``queries[i]`` (a history ``ItemList`` or a ``RecQuery``), in one launch.
         A query without history scores NaN everywhere; one whose items are all unknown scores 0."""
         st = self._device_state()
         dev = st.indptr.device
-        has, r_ptr, r_items = self._refs(queries, dev)
-        scores = st.score(r_ptr, r_items, _AGG_SUM)
-        out = []
-        for b, tgt in enumerate(targets):
-            tn = tgt.numbers(vocabulary=self.items, missing="negative").astype(np.int64)
-            s = np.full(len(tn), np.nan, dtype=np.float32)
-            ok = tn >= 0
-            if has[b] and ok.any():
-                s[ok] = scores[b, torch.from_numpy(tn[ok]).to(dev)].cpu().numpy()
-            out.append(ItemList(tgt, scores=s))
-        return out
+        has, r_ptr, r_items = history_csr(queries, self.items, dev)
+        return target_scores(st.score(r_ptr, r_items, _AGG_SUM), targets, self.items, has)
 
     def __call__(self, query, items: ItemList) -> ItemList:
         return self.score_batch([query], [items])[0]
@@ -152,23 +121,15 @@ class SLIMScorer(Component, Trainable):
         ``__call__`` and ``TopNRanker``, bit for bit.  A query without history gets an empty list; one whose items
         are all unknown ranks the all-zero scores in ``argtopn``'s tie order.
         """
-        _check_exclude(exclude)
+        check_exclude(exclude)
         st = self._device_state()
         dev = st.indptr.device
-        n_eff = min(int(n), st.n_items)
-        if n_eff <= 0:
-            return [_empty_list(self.items) for _ in queries]
-        if n_eff > int(_lib.lib().lk_topn_max()):
-            raise ValueError(f"n={n_eff} exceeds the engine limit of {int(_lib.lib().lk_topn_max())}")
-        has, r_ptr, r_items = self._refs(queries, dev)
+        n_eff = rank_size(n, st.n_items)
+        if n_eff == 0:
+            return [empty_list(self.items) for _ in queries]
+        has, r_ptr, r_items = history_csr(queries, self.items, dev)
         excl = (r_ptr, r_items) if exclude == "query" else (None, None)
-        idx, val, cnt = (t.cpu().numpy() for t in st.recommend(r_ptr, r_items, _AGG_SUM, n_eff, *excl))
-        out = []
-        for b in range(len(cnt)):
-            if not has[b]:
-                out.append(_empty_list(self.items))
-                continue
-            c = int(cnt[b])
-            out.append(ItemList(item_ids=self.items.ids(idx[b, :c]), item_nums=idx[b, :c].copy(),
-                                vocabulary=self.items, scores=val[b, :c].copy()))  # fmt: skip
-        return out
+        idx, val, cnt = st.recommend(r_ptr, r_items, _AGG_SUM, n_eff, *excl)
+        at = np.flatnonzero(has)  # the kernel ranks the all-zero sums of a query without history: dropped
+        sel = torch.from_numpy(at).to(dev)
+        return ranked_lists(self.items, len(queries), at, idx[sel], val[sel], cnt[sel])

@@ -31,6 +31,7 @@ import torch
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 
 from lkpy_b200 import _lib, data, engine  # noqa: E402
+from lkpy_b200.batch import history_csr  # noqa: E402
 from lkpy_b200 import ease as ease_mod  # noqa: E402
 from lkpy_b200.components import Dataset, ItemList  # noqa: E402
 from lkpy_b200.ease import EASEScorer  # noqa: E402
@@ -128,7 +129,7 @@ def main() -> None:
     lo = np.searchsorted(it.users, users.astype(it.users.dtype))
     hi = np.searchsorted(it.users, (users + 1).astype(it.users.dtype))
     hist = [ItemList(item_nums=it.items[a:b], vocabulary=ds.items) for a, b in zip(lo, hi)]
-    h_ptr, h_items = engine.ease_histories([h.numbers() for h in hist], dev)
+    _has, h_ptr, h_items = history_csr(hist, ds.items, dev, unique=True)
     rows = int(h_items.numel())
     alg = 4 * n_items * rows
     _log(f"{len(users)} queries, {rows} history rows, {alg / 1e12:.3f} TB to read")
