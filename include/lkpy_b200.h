@@ -24,6 +24,7 @@
  *   SLIMScorer.__call__ (x @ weights)             src/lenskit/knn/slim.py           lk_assoc_score_batch (agg 2)
  *   sample_negatives (host, per minibatch)        src/accel/data/sampling.rs:38-58  lk_flexmf_sample_negatives
  *   FlexMFImplicitTrainer.train_batch (autograd)  src/lenskit/flexmf/_implicit.py:253-274 lk_flexmf_step
+ *   FlexMFExplicitTrainer.train_batch (autograd)  src/lenskit/flexmf/_explicit.py:108-125 lk_flexmf_step (LK_FLEXMF_MSE)
  *   FlexMFScorerBase.__call__ + TopNRanker        src/lenskit/flexmf/_base.py:117-157 lk_als_recommend_batch (biases as offsets)
  *
  * Conventions
@@ -631,8 +632,9 @@ LK_API int lk_slim_pool_to_csr(const lk_slim_args *args, const int64_t *d_out_in
                                float *d_out_vals, void *stream);
 
 /* ------------------------------------------------------------------------
- * FlexMF implicit (flexmf.cu): gradient-trained matrix factorisation with logistic or pairwise (BPR) loss,
- * FlexMFImplicitTrainer (src/lenskit/flexmf/_implicit.py, _training.py, _model.py).  Score of (u, i):
+ * FlexMF (flexmf.cu): gradient-trained matrix factorisation with logistic or pairwise (BPR) loss,
+ * FlexMFImplicitTrainer (src/lenskit/flexmf/_implicit.py, _training.py, _model.py), or with squared error on
+ * centred ratings, FlexMFExplicitTrainer (src/lenskit/flexmf/_explicit.py).  Score of (u, i):
  * s = ub[u] + ib[i] + <U[u], I[i]>, an absent bias vector counting as 0.
  *
  * Negative sampling.  For sample g of d_rows (a user), step = step0 + g / batch_size, pos = g % batch_size, and
@@ -668,6 +670,7 @@ LK_API int lk_flexmf_sample_negatives(const lk_flexmf_sample_args *args, void *s
 
 #define LK_FLEXMF_LOGISTIC 0
 #define LK_FLEXMF_PAIRWISE 1
+#define LK_FLEXMF_MSE 2        /* rating regression: n_neg = 0 and d_ratings required */
 #define LK_FLEXMF_REG_NONE 0   /* torch.optim.SparseAdam */
 #define LK_FLEXMF_REG_L2 1     /* explicit norm term in the loss, SparseAdam */
 #define LK_FLEXMF_REG_ADAMW 2  /* torch.optim.AdamW(weight_decay = regularization) over every parameter */
@@ -694,8 +697,15 @@ typedef struct lk_flexmf_groups {
  * One minibatch step, in place: the loss of the batch as the reference defines it
  *   logistic: (sum_b -log sigma(s+_b) * positive_weight + sum_{b,r} -log sigma(-s-_{b,r})) / (B + B n)
  *   pairwise: mean over the B n pairs of -log sigma(s+_b - s-_{b,r})
- *   LK_FLEXMF_REG_L2 adds regularization * 0.5 * (mean_b norm+ + mean_{b,r} norm-), norm = ub^2 + ib^2 + |U[u]| + |I[i]|
- *   (vector norms not squared; the gradient of |x| at x = 0 is 0),
+ *   MSE:      mean_b (s_b - t_b)^2 with t = d_ratings (n_neg = 0: every sample has only its rated item, slot 0)
+ *   LK_FLEXMF_REG_L2 adds regularization * 0.5 * (mean_b norm+ + mean_{b,r} norm-) to the logistic and pairwise
+ *   losses and regularization * mean_b norm_b to MSE, norm = ub^2 + ib^2 + |U[u]| + |I[i]| (vector norms not
+ *   squared; the gradient of |x| at x = 0 is 0).  Per occurrence in the batch, its gradient is
+ *     user rows (every loss):            regularization / B * (U / |U|, 2 ub)
+ *     item rows, logistic and pairwise:  0.5 regularization / B * (I / |I|, 2 ib) as the positive,
+ *                                        0.5 regularization / (B n) * (I / |I|, 2 ib) as a negative
+ *     item rows, MSE:                    regularization / B * (I / |I|, 2 ib), twice the implicit positive's
+ *   MSE's d_loss is the squared error alone, without the norm term (the reference's train_batch returns that),
  * its gradient with every row's contributions added in a fixed order (ascending entry within a unit, a user's
  * items of one sample combined first, units of a row ascending), then the optimiser (betas, eps as given;
  * the host passes the scalars that depend on the step number):
@@ -709,8 +719,8 @@ typedef struct lk_flexmf_groups {
 typedef struct lk_flexmf_step_args {
     int32_t n_users, n_items, k;
     int32_t batch;                     /* B: samples in this step */
-    int32_t n_neg;                     /* n */
-    int32_t loss;                      /* LK_FLEXMF_LOGISTIC / _PAIRWISE */
+    int32_t n_neg;                     /* n: >= 1, or 0 with MSE */
+    int32_t loss;                      /* LK_FLEXMF_LOGISTIC / _PAIRWISE / _MSE */
     int32_t reg_method;                /* LK_FLEXMF_REG_* */
     float positive_weight, regularization;
     float decay;                       /* AdamW: 1 - lr * regularization */
@@ -723,12 +733,13 @@ typedef struct lk_flexmf_step_args {
     float *d_i_bias, *d_i_bias_m, *d_i_bias_v; /* [n_items] or all NULL */
     const int32_t *d_users;            /* [B] */
     const int32_t *d_pos;              /* [B] */
-    const int32_t *d_neg;              /* [B][n] */
+    const int32_t *d_neg;              /* [B][n]; unused (may be NULL) with MSE */
     lk_flexmf_groups u_groups, i_groups;
     int32_t n_u_units, n_i_units;
     void *d_workspace;
     int64_t workspace_bytes;           /* >= lk_flexmf_workspace_bytes(batch, n_neg, k) */
     float *d_loss;                     /* [1] */
+    const float *d_ratings;            /* [B] targets t = r - mu, MSE only */
 } lk_flexmf_step_args;
 
 LK_API int lk_flexmf_workspace_bytes(int32_t batch, int32_t n_neg, int32_t k, int64_t *bytes);

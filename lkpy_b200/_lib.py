@@ -18,7 +18,7 @@ LK_DTYPE_F32, LK_DTYPE_BF16 = 0, 1
 LK_ALS_IMPLICIT, LK_ALS_EXPLICIT = 0, 1
 LK_MAX_REPLICAS = 8
 LK_COOC_COUNT, LK_ASSOC_PROBABILITY, LK_ASSOC_LIFT = 0, 1, 2
-LK_FLEXMF_LOGISTIC, LK_FLEXMF_PAIRWISE = 0, 1
+LK_FLEXMF_LOGISTIC, LK_FLEXMF_PAIRWISE, LK_FLEXMF_MSE = 0, 1, 2
 LK_FLEXMF_REG_NONE, LK_FLEXMF_REG_L2, LK_FLEXMF_REG_ADAMW = 0, 1, 2
 
 i32p = C.POINTER(C.c_int32)
@@ -362,6 +362,7 @@ class LkFlexmfStepArgs(C.Structure):
         ("d_workspace", vp),
         ("workspace_bytes", C.c_int64),
         ("d_loss", vp),
+        ("d_ratings", vp),
     ]  # fmt: skip
 
 

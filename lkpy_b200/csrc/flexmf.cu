@@ -1,9 +1,10 @@
-// flexmf.cu — gradient-trained implicit matrix factorisation (FlexMFImplicitScorer: logistic and pairwise/BPR loss):
-// the negative sampler and one minibatch step (forward, loss, per-row gradient sums, Adam update).
+// flexmf.cu — gradient-trained matrix factorisation: FlexMFImplicitScorer (logistic and pairwise/BPR loss over sampled
+// negatives) and FlexMFExplicitScorer (squared error on centred ratings, no negatives): the negative sampler and one
+// minibatch step (forward, loss, per-row gradient sums, Adam update).
 //
 // A step is four launches on the caller's stream:
-//   flexmf_forward_kernel   one warp per sample: the scores of the positive and the n negatives, dL/ds of each
-//                           (coef [B][1+n]) and the sample's share of the loss;
+//   flexmf_forward_kernel   one warp per sample: the scores of the positive and the n negatives (n = 0 for MSE), dL/ds
+//                           of each (coef [B][1+n]) and the sample's share of the loss;
 //   flexmf_loss_kernel      one block adds the B shares in a fixed order (f64) into d_loss[0];
 //   flexmf_grad_kernel      one warp per unit.  The occurrences of a row in the batch are sorted by position and cut
 //                           into units of at most 64, so that a row that fills half the batch is spread over the
@@ -122,13 +123,14 @@ __global__ void __launch_bounds__(256) flexmf_forward_kernel(lk_flexmf_step_args
     int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (w >= a.batch) return;
     const int n = a.n_neg, k = a.k;
-    const bool l2 = a.reg_method == LK_FLEXMF_REG_L2;
+    const bool mse = a.loss == LK_FLEXMF_MSE;
+    const bool l2 = a.reg_method == LK_FLEXMF_REG_L2 && !mse;  // the MSE loss reported is without the norm term
     int u = a.d_users[w];
     float uv[4], iv[4];
     load_row<V4>(uv, a.d_u_emb + int64_t(u) * k, k, lane);
     float ub = a.d_u_bias ? a.d_u_bias[u] : 0.f;
     float nu = l2 ? sqrtf(dot4(uv, uv)) : 0.f;
-    float inv_pos = 1.f / float(a.batch), inv_neg = 1.f / (float(a.batch) * float(n));
+    float inv_pos = 1.f / float(a.batch), inv_neg = n > 0 ? 1.f / (float(a.batch) * float(n)) : 0.f;
     float inv_all = 1.f / (float(a.batch) + float(a.batch) * float(n));
     float loss = 0.f, s_pos = 0.f, c_pos = 0.f;
     for (int j = 0; j <= n; ++j) {
@@ -141,7 +143,11 @@ __global__ void __launch_bounds__(256) flexmf_forward_kernel(lk_flexmf_step_args
             loss += a.regularization * 0.5f * nrm * (j == 0 ? inv_pos : inv_neg);
         }
         float c;
-        if (a.loss == LK_FLEXMF_LOGISTIC) {
+        if (mse) {  // n = 0: the rating's target t = r - mu
+            float d = s - a.d_ratings[w];
+            loss = d * d * inv_pos;
+            c = 2.f * d * inv_pos;
+        } else if (a.loss == LK_FLEXMF_LOGISTIC) {
             if (j == 0) {
                 loss += a.positive_weight * softplus(-s) * inv_all;
                 c = -a.positive_weight * sigmoid(-s) * inv_all;
@@ -162,7 +168,7 @@ __global__ void __launch_bounds__(256) flexmf_forward_kernel(lk_flexmf_step_args
         if (lane == 0) coef[int64_t(w) * (n + 1) + j] = c;
     }
     if (lane == 0) {
-        if (a.loss != LK_FLEXMF_LOGISTIC) coef[int64_t(w) * (n + 1)] = c_pos;
+        if (a.loss == LK_FLEXMF_PAIRWISE) coef[int64_t(w) * (n + 1)] = c_pos;
         sample_loss[w] = loss;
     }
 }
@@ -194,11 +200,14 @@ __global__ void flexmf_grad_kernel(lk_flexmf_step_args a, const float *coef, flo
     const bool user_side = x < a.n_u_units;
     const lk_flexmf_groups &g = user_side ? a.u_groups : a.i_groups;
     const int64_t unit = (user_side ? x : x - a.n_u_units) + g.unit0;
+    // the item rows' L2 weight per occurrence, over regularization / B: 1/2 for the implicit positive (half of
+    // reg/2 (mean norm+ + mean norm-)), 1 for MSE (reg mean norm)
+    const float i_l2 = a.loss == LK_FLEXMF_MSE ? 1.f : 0.5f;
     const int32_t uniq = g.d_unit_uniq[unit];
     const int row = g.d_uniq_row[uniq];
     const int64_t p0 = g.d_unit_start[unit], p1 = g.d_unit_start[unit + 1];
     float acc[4] = {0.f, 0.f, 0.f, 0.f}, accb = 0.f, ov[4];
-    const float inv_pos = 1.f / float(a.batch), inv_neg = 1.f / (float(a.batch) * float(n));
+    const float inv_pos = 1.f / float(a.batch), inv_neg = n > 0 ? 1.f / (float(a.batch) * float(n)) : 0.f;
     if (user_side) {
         for (int64_t p = p0; p < p1; ++p) {
             int b = g.d_occ[p];
@@ -215,9 +224,11 @@ __global__ void flexmf_grad_kernel(lk_flexmf_step_args a, const float *coef, flo
             for (int q = 0; q < 4; ++q) acc[q] += t[q];
             // the user bias cancels in s+ - s-: its pairwise gradient is exactly 0, not the rounding residue of
             // c_pos + sum(c_r)
-            if (a.loss == LK_FLEXMF_LOGISTIC) accb += tb;
+            if (a.loss != LK_FLEXMF_PAIRWISE) accb += tb;
         }
-        if (l2) {  // d/du of reg/2 (mean(norm+) + mean(norm-)): the user is in the positive and in all n negatives
+        // d/du of reg/2 (mean(norm+) + mean(norm-)): the user is in the positive and in all n negatives; of MSE's
+        // reg mean(norm): once per sample.  Either way reg/B per occurrence
+        if (l2) {
             float cnt = float(p1 - p0);
             load_row<V4>(ov, a.d_u_emb + int64_t(row) * k, k, lane);
             float nrm = sqrtf(dot4(ov, ov));
@@ -241,10 +252,10 @@ __global__ void flexmf_grad_kernel(lk_flexmf_step_args a, const float *coef, flo
         if (l2) {
             load_row<V4>(ov, a.d_i_emb + int64_t(row) * k, k, lane);
             float nrm = sqrtf(dot4(ov, ov));
-            float wv = nrm > 0.f ? 0.5f * a.regularization * wl2 / nrm : 0.f;
+            float wv = nrm > 0.f ? i_l2 * a.regularization * wl2 / nrm : 0.f;
 #pragma unroll
             for (int q = 0; q < 4; ++q) acc[q] = fmaf(wv, ov[q], acc[q]);
-            if (a.d_i_bias) accb = fmaf(a.regularization * wl2, a.d_i_bias[row], accb);
+            if (a.d_i_bias) accb = fmaf(2.f * i_l2 * a.regularization * wl2, a.d_i_bias[row], accb);
         }
     }
     float *out = partials + int64_t(x) * kp;
@@ -392,7 +403,8 @@ int lk_flexmf_sample_negatives(const lk_flexmf_sample_args *a, void *stream)
 int lk_flexmf_workspace_bytes(int32_t batch, int32_t n_neg, int32_t k, int64_t *bytes)
 {
     LK_REQUIRE(bytes != nullptr, LK_ERR_INVALID, "lk_flexmf_workspace_bytes: null result pointer");
-    LK_REQUIRE(batch >= 1 && n_neg >= 1, LK_ERR_INVALID, "lk_flexmf_workspace_bytes: batch and n_neg must be positive");
+    LK_REQUIRE(batch >= 1 && n_neg >= 0, LK_ERR_INVALID,
+               "lk_flexmf_workspace_bytes: batch must be positive and n_neg not negative");
     LK_REQUIRE(k >= 1 && k <= lk_als_max_features(), LK_ERR_UNSUPPORTED,
                "lk_flexmf_workspace_bytes: k=%d is outside 1..%d", k, lk_als_max_features());
     LK_REQUIRE(int64_t(batch) * (n_neg + 1) < (int64_t(1) << 30), LK_ERR_UNSUPPORTED,
@@ -410,8 +422,13 @@ int lk_flexmf_step(const lk_flexmf_step_args *a, void *stream)
     LK_REQUIRE(a->d_workspace != nullptr && a->workspace_bytes >= need, LK_ERR_INVALID,
                "lk_flexmf_step: the workspace has %lld bytes, the step needs %lld", (long long)a->workspace_bytes,
                (long long)need);
-    LK_REQUIRE(a->loss == LK_FLEXMF_LOGISTIC || a->loss == LK_FLEXMF_PAIRWISE, LK_ERR_INVALID,
-               "lk_flexmf_step: unknown loss %d", a->loss);
+    LK_REQUIRE(a->loss == LK_FLEXMF_LOGISTIC || a->loss == LK_FLEXMF_PAIRWISE || a->loss == LK_FLEXMF_MSE,
+               LK_ERR_INVALID, "lk_flexmf_step: unknown loss %d", a->loss);
+    const bool mse = a->loss == LK_FLEXMF_MSE;
+    LK_REQUIRE(mse == (a->n_neg == 0), LK_ERR_INVALID,
+               "lk_flexmf_step: MSE takes no negatives (n_neg = 0); the other losses take n_neg >= 1 (n_neg = %d)",
+               a->n_neg);
+    LK_REQUIRE(!mse || a->d_ratings != nullptr, LK_ERR_INVALID, "lk_flexmf_step: MSE needs the targets d_ratings");
     LK_REQUIRE(a->reg_method >= LK_FLEXMF_REG_NONE && a->reg_method <= LK_FLEXMF_REG_ADAMW, LK_ERR_INVALID,
                "lk_flexmf_step: unknown reg_method %d", a->reg_method);
     LK_REQUIRE(a->step >= 1 && a->step < (int64_t(1) << 31) && a->n_users > 0 && a->n_items > 0, LK_ERR_INVALID,
@@ -426,7 +443,7 @@ int lk_flexmf_step(const lk_flexmf_step_args *a, void *stream)
                    a->i_groups.n_uniq <= a->n_i_units,
                LK_ERR_INVALID, "lk_flexmf_step: a side has more rows than units");
     LK_REQUIRE(a->d_u_emb && a->d_u_emb_m && a->d_u_emb_v && a->d_i_emb && a->d_i_emb_m && a->d_i_emb_v &&
-                   a->d_users && a->d_pos && a->d_neg && a->d_loss,
+                   a->d_users && a->d_pos && (a->d_neg || mse) && a->d_loss,
                LK_ERR_INVALID, "lk_flexmf_step: null device pointer");
     LK_REQUIRE((a->d_u_bias == nullptr) == (a->d_u_bias_m == nullptr) &&
                    (a->d_u_bias == nullptr) == (a->d_u_bias_v == nullptr) &&

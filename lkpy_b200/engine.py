@@ -1454,10 +1454,10 @@ class SlimPlan:
 
 
 # ---------------------------------------------------------------------------
-# FlexMF implicit
+# FlexMF implicit and explicit
 # ---------------------------------------------------------------------------
 
-FLEXMF_LOSSES = {"logistic": _lib.LK_FLEXMF_LOGISTIC, "pairwise": _lib.LK_FLEXMF_PAIRWISE}
+FLEXMF_LOSSES = {"logistic": _lib.LK_FLEXMF_LOGISTIC, "pairwise": _lib.LK_FLEXMF_PAIRWISE, "mse": _lib.LK_FLEXMF_MSE}
 FLEXMF_REG_METHODS = {None: _lib.LK_FLEXMF_REG_NONE, "L2": _lib.LK_FLEXMF_REG_L2, "AdamW": _lib.LK_FLEXMF_REG_ADAMW}
 FLEXMF_MAX_ATTEMPTS = 10  # rejected draws per negative, as the reference's sampler
 FLEXMF_UNIT = 64  # occurrences of a row per gradient unit (flexmf.cu)
@@ -1529,7 +1529,8 @@ class _FlexmfGroups:
 class _FlexmfBatches:
     users: torch.Tensor
     pos: torch.Tensor
-    neg: torch.Tensor
+    neg: torch.Tensor  # [S, n]; [S, 0] for MSE
+    ratings: torch.Tensor | None  # [S] MSE targets
     u_groups: _FlexmfGroups
     i_groups: _FlexmfGroups
     n_steps: int
@@ -1537,23 +1538,29 @@ class _FlexmfBatches:
 
 class FlexMFState:
     """
-    Device state of one FlexMF implicit training run: the four parameter tables with their Adam moments, the
-    users x items CSR the sampler tests membership in, the step workspace, the optimiser step count and the sampler
-    seed.  The only caller of ``lk_flexmf_sample_negatives`` and ``lk_flexmf_step``.
+    Device state of one FlexMF training run: the four parameter tables with their Adam moments, the users x items
+    CSR the sampler tests membership in, the step workspace, the optimiser step count and the sampler seed.  The
+    only caller of ``lk_flexmf_sample_negatives`` and ``lk_flexmf_step``.
 
     ``params`` maps the reference's state-dict names (``u_bias.weight`` / ``i_bias.weight`` [n, 1], optional;
     ``u_embed.weight`` / ``i_embed.weight`` [n, k]) to f32 arrays or tensors; ``users`` / ``items`` are the training
-    interactions sorted by (user, item).
+    interactions sorted by (user, item).  ``loss="mse"`` (the explicit model) takes ``negative_count=0`` and
+    ``ratings``, the f32 target of every interaction (the centred rating), which is permuted with the samples.
     """
 
     def __init__(self, params: dict, users, items, *, loss: str, reg_method: str | None, negative_count: int = 1,
                  popular: bool = False, batch_size: int = 8192, learning_rate: float = 0.01,
-                 regularization: float = 0.01, positive_weight: float = 1.0, seed: int = 0, device=None):  # fmt: skip
+                 regularization: float = 0.01, positive_weight: float = 1.0, seed: int = 0, ratings=None,
+                 device=None):  # fmt: skip
         dev = device or _lib.require_device()
         if loss not in FLEXMF_LOSSES:
             raise ValueError(f"loss={loss!r} is not one of {sorted(FLEXMF_LOSSES)}")
         if reg_method not in FLEXMF_REG_METHODS:
             raise ValueError(f"reg_method={reg_method!r} is not one of 'AdamW', 'L2', None")
+        if (loss == "mse") != (int(negative_count) == 0):
+            raise ValueError(f"loss={loss!r} with negative_count={negative_count}: MSE takes 0 negatives, the others 1 or more")
+        if (loss == "mse") != (ratings is not None):
+            raise ValueError("ratings are the MSE targets: given with loss='mse' and only then")
         self.loss, self.reg_method, self.n_neg, self.popular = loss, reg_method, int(negative_count), bool(popular)
         self.batch_size, self.lr, self.reg = int(batch_size), float(learning_rate), float(regularization)
         self.positive_weight, self.seed = float(positive_weight), int(seed) & (2**64 - 1)
@@ -1568,6 +1575,9 @@ class FlexMFState:
         self.moments = {n: (torch.zeros_like(t), torch.zeros_like(t)) for n, t in self.params.items()}
         self.users = torch.as_tensor(users).to(dev, torch.int32).contiguous()
         self.items = torch.as_tensor(items).to(dev, torch.int32).contiguous()
+        self.ratings = None if ratings is None else torch.as_tensor(ratings).to(dev, torch.float32).contiguous()
+        if self.ratings is not None and self.ratings.shape != self.items.shape:
+            raise ValueError("one rating per interaction")
         self.ui_indptr = torch.zeros(self.n_users + 1, dtype=torch.int64, device=dev)
         torch.cumsum(torch.bincount(self.users.long(), minlength=self.n_users), 0, out=self.ui_indptr[1:])
         if self.items.numel() >= 2**31:
@@ -1613,18 +1623,28 @@ class FlexMFState:
         a.d_workspace, a.workspace_bytes = ptr(self.workspace), self.workspace.numel()
         return a
 
-    def plan_batches(self, users: torch.Tensor, pos: torch.Tensor, neg: torch.Tensor | None = None) -> "_FlexmfBatches":
+    def plan_batches(self, users: torch.Tensor, pos: torch.Tensor, neg: torch.Tensor | None = None, *,
+                     ratings: torch.Tensor | None = None) -> "_FlexmfBatches":  # fmt: skip
         """
         Everything about a run of consecutive batches (``batch_size`` samples each, the last may be short) that does
         not depend on the model: the negatives (``neg`` [S, n], default this state's sampler at the current step
-        count) and the grouping of every batch's rows.  Made once for all the steps, so an epoch pays one sampler
-        launch and two sorts instead of one of each per step.
+        count; none for MSE, which takes the targets ``ratings`` [S] instead) and the grouping of every batch's
+        rows.  Made once for all the steps, so an epoch pays one sampler launch and two sorts instead of one of each
+        per step.
         """
         dev, B, n = self.device, self.batch_size, self.n_neg
         users = users.to(dev, torch.int32).contiguous()
         pos = pos.to(dev, torch.int32).contiguous()
         S = users.numel()
-        neg = self.sample(users) if neg is None else neg.to(dev, torch.int32).contiguous()
+        if self.loss == "mse":
+            if neg is not None or ratings is None or ratings.numel() != S:
+                raise ValueError(f"MSE batches take no negatives and {S} ratings")
+            ratings = ratings.to(dev, torch.float32).contiguous()
+            neg = torch.empty((S, 0), dtype=torch.int32, device=dev)
+        else:
+            if ratings is not None:
+                raise ValueError(f"loss={self.loss!r} takes no ratings")
+            neg = self.sample(users) if neg is None else neg.to(dev, torch.int32).contiguous()
         if S == 0 or pos.numel() != S or tuple(neg.shape) != (S, n):
             raise ValueError(f"expected {S} > 0 users, as many positives and negatives of shape ({S}, {n})")
         n_steps = -(-S // B)
@@ -1635,7 +1655,7 @@ class FlexMFState:
         entries = local[:, None] * (n + 1) + torch.arange(n + 1, device=dev, dtype=torch.int32)[None, :]
         ig = _FlexmfGroups.build((step_of[:, None] * self.n_items + slots).flatten(), entries.flatten(),
                                  self.n_items, n_steps)  # fmt: skip
-        return _FlexmfBatches(users, pos, neg, ug, ig, n_steps)
+        return _FlexmfBatches(users, pos, neg, ratings, ug, ig, n_steps)
 
     def run_batches(self, plan: "_FlexmfBatches") -> torch.Tensor:
         """The steps of ``plan``, four launches each; the batch losses as a device vector, not synchronised on."""
@@ -1651,7 +1671,8 @@ class FlexMFState:
             for name, value in flexmf_adam_scalars(self.reg_method, self.lr, self.reg, a.step).items():
                 setattr(a, name, value)
             a.d_users, a.d_pos = plan.users.data_ptr() + 4 * lo, plan.pos.data_ptr() + 4 * lo
-            a.d_neg = plan.neg.data_ptr() + 4 * lo * n
+            a.d_neg = plan.neg.data_ptr() + 4 * lo * n if n > 0 else None
+            a.d_ratings = plan.ratings.data_ptr() + 4 * lo if plan.ratings is not None else None
             a.n_u_units = plan.u_groups.fill(a.u_groups, s, self.u_mark)
             a.n_i_units = plan.i_groups.fill(a.i_groups, s, self.i_mark)
             a.d_loss = losses.data_ptr() + 4 * s
@@ -1659,17 +1680,20 @@ class FlexMFState:
             self.steps_done += 1
         return losses
 
-    def train_batches(self, users: torch.Tensor, pos: torch.Tensor, neg: torch.Tensor | None = None) -> torch.Tensor:
+    def train_batches(self, users: torch.Tensor, pos: torch.Tensor, neg: torch.Tensor | None = None, *,
+                      ratings: torch.Tensor | None = None) -> torch.Tensor:  # fmt: skip
         """``run_batches(plan_batches(...))``."""
-        return self.run_batches(self.plan_batches(users, pos, neg))
+        return self.run_batches(self.plan_batches(users, pos, neg, ratings=ratings))
 
-    def step(self, users: torch.Tensor, pos: torch.Tensor, neg: torch.Tensor | None = None) -> torch.Tensor:
+    def step(self, users: torch.Tensor, pos: torch.Tensor, neg: torch.Tensor | None = None, *,
+             ratings: torch.Tensor | None = None) -> torch.Tensor:  # fmt: skip
         """One minibatch (at most ``batch_size`` samples); the loss as a device scalar."""
         if users.numel() > self.batch_size:
             raise ValueError(f"a step takes at most batch_size={self.batch_size} samples")
-        return self.train_batches(users, pos, neg)[0]
+        return self.train_batches(users, pos, neg, ratings=ratings)[0]
 
     def epoch(self, perm: torch.Tensor) -> torch.Tensor:
         """One pass over the training interactions in the order ``perm``; the batch losses (device)."""
         perm = perm.to(self.device, torch.int64)
-        return self.train_batches(self.users[perm], self.items[perm])
+        ratings = None if self.ratings is None else self.ratings[perm]
+        return self.train_batches(self.users[perm], self.items[perm], ratings=ratings)

@@ -1,8 +1,8 @@
 """
-FlexMF implicit-feedback scorer on the H100 engine — the component surface of
-``lenskit.flexmf.FlexMFImplicitScorer`` (``src/lenskit/flexmf/_implicit.py``, ``_base.py``, ``_training.py``,
-``_model.py``): matrix factorisation trained by minibatch Adam on the logistic or the pairwise (BPR) loss over
-sampled negatives.
+FlexMF scorers on the H100 engine — the component surface of ``lenskit.flexmf.FlexMFImplicitScorer`` and
+``FlexMFExplicitScorer`` (``src/lenskit/flexmf/_implicit.py``, ``_explicit.py``, ``_base.py``, ``_training.py``,
+``_model.py``): matrix factorisation trained by minibatch Adam, on the logistic or the pairwise (BPR) loss over
+sampled negatives (implicit), or on the squared error of mean-centred ratings (explicit).
 
 Same config fields, aliases, presets and defaults, the same initial parameters for a seed (torch's ``normal_`` on a
 CPU generator: user bias, item bias, user embeddings, item embeddings; rows without interactions zeroed), the same
@@ -14,8 +14,16 @@ first-epoch sample order (``rng.permutation``), and the same step mathematics to
 * ``loss="warp"`` / ``negative_strategy="misranked"`` and ``convolution_layers > 0`` (LightGCN) are rejected when the
   configuration is made.
 
-Inference is ``ub + ib + u·i``: the ALS scorers' batched scoring and fused top-n (``lk_als_recommend_batch``) with
-the item bias as the item offset and the user bias as the query offset.
+The explicit trainer draws nothing from the NumPy generator but the epoch permutations, so with the same seed its
+whole sample order is the reference's.  Its model has no bias terms: the reference's ``FlexMFModel`` keeps
+``u_bias = None`` / ``i_bias = None`` as class attributes, which shadow the ``nn.Embedding`` modules its constructor
+registers, so ``self.u_bias is not None`` is false in ``__init__`` and ``forward``.  The bias tables it creates are
+never drawn from the seeded generator, never enter a score or the L2 norm and never receive a gradient; the
+embeddings take the generator's first draws.  The explicit model here computes exactly that model, ``u·i + mu``.
+
+Inference is ``ub + ib + u·i`` (implicit) or ``u·i + mu`` (explicit): the ALS scorers' batched scoring and fused
+top-n (``lk_als_recommend_batch``) with the item bias as the item offset and the user bias (or the mean) as the query
+offset.
 """
 
 from __future__ import annotations
@@ -35,13 +43,34 @@ PRESETS = {"bpr": {"loss": "pairwise", "user_bias": False, "item_bias": False}}
 PARAM_NAMES = ("u_bias.weight", "i_bias.weight", "u_embed.weight", "i_embed.weight")
 
 
-class FlexMFImplicitConfig(BaseModel):
+class FlexMFConfigBase(BaseModel):
+    """``FlexMFConfigBase`` (``_base.py:34-95``): what the two models' configurations share."""
+
     embedding_size: PositiveInt = 64
     batch_size: PositiveInt = 8 * 1024
     learning_rate: float = 0.01
     epochs: int = 10
     regularization: float = 0.01
     reg_method: Literal["AdamW", "L2"] | None = "AdamW"
+
+    @model_validator(mode="before")
+    @classmethod
+    def apply_aliases(cls, data):
+        if isinstance(data, dict) and "embedding_size_exp" in data:  # EmbeddingSizeMixin: the size as a power of two
+            data = {k: v for k, v in data.items() if k not in ("embedding_size_exp", "embedding_size")} | {
+                "embedding_size": 2 ** data["embedding_size_exp"]
+            }
+        return data
+
+    @field_validator("embedding_size", mode="after")
+    @staticmethod
+    def check_embedding_size(k) -> int:
+        if k > engine.ALS_MAX_FEATURES:
+            raise ValueError(f"embedding_size={k} exceeds the engine limit of {engine.ALS_MAX_FEATURES}")
+        return k
+
+
+class FlexMFImplicitConfig(FlexMFConfigBase):
     preset: Literal["bpr", "warp", "lightgcn"] | None = None
     loss: Literal["logistic", "pairwise", "warp"] = "logistic"
     negative_strategy: Literal["uniform", "popular", "misranked"] | None = None
@@ -53,13 +82,9 @@ class FlexMFImplicitConfig(BaseModel):
 
     @model_validator(mode="before")
     @classmethod
-    def apply_aliases_and_preset(cls, data):
+    def apply_preset(cls, data):
         if not isinstance(data, dict):
             return data
-        if "embedding_size_exp" in data:  # EmbeddingSizeMixin: the size as a power of two
-            data = {k: v for k, v in data.items() if k not in ("embedding_size_exp", "embedding_size")} | {
-                "embedding_size": 2 ** data["embedding_size_exp"]
-            }
         preset = data.get("preset")
         if preset in ("warp", "lightgcn"):
             raise ValueError(f"preset={preset!r} is not covered by the engine (DESIGN.md §6)")
@@ -68,13 +93,6 @@ class FlexMFImplicitConfig(BaseModel):
                 raise ValueError(f"unknown preset '{preset}'")
             data = PRESETS[preset] | data
         return data
-
-    @field_validator("embedding_size", mode="after")
-    @staticmethod
-    def check_embedding_size(k) -> int:
-        if k > engine.ALS_MAX_FEATURES:
-            raise ValueError(f"embedding_size={k} exceeds the engine limit of {engine.ALS_MAX_FEATURES}")
-        return k
 
     @model_validator(mode="after")
     def check_covered(self):
@@ -91,6 +109,13 @@ class FlexMFImplicitConfig(BaseModel):
 
     def selected_user_bias(self) -> bool:
         return self.loss == "logistic" if self.user_bias is None else self.user_bias
+
+
+class FlexMFExplicitConfig(FlexMFConfigBase):
+    """``FlexMFExplicitConfig`` (``_explicit.py:25-35``): stronger regularisation, the L2 term by default."""
+
+    regularization: float = 0.1
+    reg_method: Literal["AdamW", "L2"] | None = "L2"
 
 
 def _torch_seed(rng_input) -> int | None:
@@ -134,17 +159,13 @@ def initial_parameters(n_users: int, n_items: int, k: int, user_bias: bool, item
     return out
 
 
-class FlexMFImplicitScorer(ALSBase):
-    """``FlexMFImplicitScorer``: ``train``, ``__call__``, and the batched ``score_matrix`` / ``score_batch`` /
+class FlexMFScorerBase(ALSBase):
+    """``FlexMFScorerBase`` (``_base.py:98-164``): ``__call__`` and the batched ``score_matrix`` / ``score_batch`` /
     ``recommend_batch`` (inherited from the ALS scorers, with the biases as the kernel's offsets)."""
 
-    CONFIG_CLASS = FlexMFImplicitConfig
-    config: FlexMFImplicitConfig
+    config: FlexMFConfigBase
     user_bias: np.ndarray | None = None
     item_bias: np.ndarray | None = None
-
-    def create_trainer(self, data, options):
-        return FlexMFImplicitTrainer(self, data, options)
 
     def embed_batch(self, queries):
         """Known users' embeddings; a query without a known user is unscorable (``_base.py:126-133``)."""
@@ -177,10 +198,40 @@ class FlexMFImplicitScorer(ALSBase):
         return d
 
 
-class FlexMFImplicitTrainer(ModelTrainer):
-    """``FlexMFImplicitTrainer`` (``_implicit.py:164-290`` over ``_training.py:39-258``) with device-resident state."""
+class FlexMFImplicitScorer(FlexMFScorerBase):
+    """``FlexMFImplicitScorer``: ``train`` and the scoring of :class:`FlexMFScorerBase`."""
 
-    def __init__(self, scorer: FlexMFImplicitScorer, data, options: TrainingOptions):
+    CONFIG_CLASS = FlexMFImplicitConfig
+    config: FlexMFImplicitConfig
+
+    def create_trainer(self, data, options):
+        return FlexMFImplicitTrainer(self, data, options)
+
+
+class FlexMFExplicitScorer(FlexMFScorerBase):
+    """``FlexMFExplicitScorer`` (``_explicit.py:38-55``): rating prediction ``u·i + global_bias`` (the reference's
+    model, whose bias terms are inactive: see the module docstring).  ``score_matrix`` / ``recommend_batch`` /
+    ``score_batch`` / ``__call__`` add the item offset to the dot product, then the query offset ``ub + global_bias``;
+    with the reference's model those are no item offset and ``global_bias`` rounded to f32."""
+
+    CONFIG_CLASS = FlexMFExplicitConfig
+    config: FlexMFExplicitConfig
+    global_bias: float | None = None
+
+    def create_trainer(self, data, options):
+        return FlexMFExplicitTrainer(self, data, options)
+
+    def batch_offsets(self, user_nums: np.ndarray, fold_bias):
+        ib, ub = super().batch_offsets(user_nums, fold_bias)
+        mu = np.float32(self.global_bias)
+        return ib, (np.full(len(user_nums), mu, dtype=np.float32) if ub is None else (ub + mu).astype(np.float32))
+
+
+class FlexMFTrainerBase(ModelTrainer):
+    """``FlexMFTrainerBase`` (``_training.py:39-258``) with device-resident state: the data intake, the initial
+    parameters, the epoch loop and the hand-back to the scorer.  Subclasses make the ``engine.FlexMFState``."""
+
+    def __init__(self, scorer: FlexMFScorerBase, data, options: TrainingOptions):
         from .prep import DeviceInteractions
 
         self.scorer = scorer
@@ -191,42 +242,45 @@ class FlexMFImplicitTrainer(ModelTrainer):
             scorer.users = Vocabulary(np.arange(data.n_users), "user")
             scorer.items = Vocabulary(np.arange(data.n_items), "item")
             users, items, n_users, n_items = data.users, data.items, data.n_users, data.n_items
+            ratings = data.ratings
         else:
             ds = _as_dataset(data)
             scorer.users, scorer.items = ds.users, ds.items
             it = ds.interactions
             users, items, n_users, n_items = torch.from_numpy(it.users), torch.from_numpy(it.items), it.n_users, it.n_items
+            ratings = None if it.ratings is None else torch.from_numpy(it.ratings)
         users, items = users.to(self.device), items.to(self.device)
         c = self.config
         params = initial_parameters(
-            n_users, n_items, c.embedding_size, c.selected_user_bias(), c.item_bias, torch_rng,
+            n_users, n_items, c.embedding_size, *self.biases(), torch_rng,
             torch.bincount(users.long(), minlength=n_users).cpu().numpy(),
             torch.bincount(items.long(), minlength=n_items).cpu().numpy(),
         )  # fmt: skip
-        self.state = engine.FlexMFState(
-            params, users, items, loss=c.loss, reg_method=c.reg_method, negative_count=c.negative_count,
-            popular=c.selected_negative_strategy() == "popular", batch_size=c.batch_size,
-            learning_rate=c.learning_rate, regularization=c.regularization, positive_weight=c.positive_weight,
-            device=self.device,
-        )  # fmt: skip
-        self._seeded = False
+        self.state = self.create_state(params, users, items, ratings)
         self.n_samples = int(users.numel())
         self.epochs_trained = 0  # the scorer gets its host arrays after the first epoch: until then it is not trained
 
     @property
-    def config(self) -> FlexMFImplicitConfig:
+    def config(self) -> FlexMFConfigBase:
         return self.scorer.config
+
+    def biases(self) -> tuple[bool, bool]:
+        """Whether the model has a user bias and an item bias."""
+        raise NotImplementedError
+
+    def create_state(self, params, users, items, ratings) -> engine.FlexMFState:
+        raise NotImplementedError
 
     def epoch_permutation(self) -> np.ndarray:
         """The epoch's sample order, as the reference draws it (``_training.py:205-215``)."""
         return np.require(self.rng.permutation(self.n_samples), dtype=np.int32)
 
+    def epoch_started(self) -> None:
+        """Called after the epoch's permutation is drawn, before its steps."""
+
     def train_epoch(self) -> dict[str, float]:
         perm = self.epoch_permutation()
-        if not self._seeded:
-            # after the first permutation, so that the first epoch's order is the reference's for the same seed
-            self.state.seed = int(self.rng.integers(0, 2**63))
-            self._seeded = True
+        self.epoch_started()
         losses = self.state.epoch(torch.from_numpy(perm))
         loss = float(losses.double().mean().item())  # the epoch's one read of the batch losses
         self.epochs_trained += 1
@@ -251,3 +305,51 @@ class FlexMFImplicitTrainer(ModelTrainer):
         for n, t in self.state.params.items():
             t.copy_(torch.as_tensor(state[n]).to(torch.float32).reshape(t.shape))
         self._sync_host()
+
+
+class FlexMFImplicitTrainer(FlexMFTrainerBase):
+    """``FlexMFImplicitTrainer`` (``_implicit.py:164-290``): sampled negatives, logistic or pairwise loss."""
+
+    config: FlexMFImplicitConfig
+    _seeded = False  # the sampler seed is drawn once, in the first epoch
+
+    def biases(self) -> tuple[bool, bool]:
+        return self.config.selected_user_bias(), self.config.item_bias
+
+    def create_state(self, params, users, items, ratings) -> engine.FlexMFState:
+        c = self.config
+        return engine.FlexMFState(
+            params, users, items, loss=c.loss, reg_method=c.reg_method, negative_count=c.negative_count,
+            popular=c.selected_negative_strategy() == "popular", batch_size=c.batch_size,
+            learning_rate=c.learning_rate, regularization=c.regularization, positive_weight=c.positive_weight,
+            device=self.device,
+        )  # fmt: skip
+
+    def epoch_started(self) -> None:
+        if not self._seeded:
+            # after the first permutation, so that the first epoch's order is the reference's for the same seed
+            self.state.seed = int(self.rng.integers(0, 2**63))
+            self._seeded = True
+
+
+class FlexMFExplicitTrainer(FlexMFTrainerBase):
+    """``FlexMFExplicitTrainer`` (``_explicit.py:58-125``): squared error on the ratings less their mean, no
+    negatives, and no bias terms, as in the reference's model."""
+
+    config: FlexMFExplicitConfig
+
+    def biases(self) -> tuple[bool, bool]:
+        return False, False
+
+    def create_state(self, params, users, items, ratings) -> engine.FlexMFState:
+        if ratings is None:
+            raise ValueError("FlexMFExplicitScorer trains on ratings, and the data has none")
+        # the reference's f32 torch mean on the host (_explicit.py:72-79), and the targets r - mu
+        values = ratings.cpu().to(torch.float32)
+        mean = values.mean()
+        self.scorer.global_bias = mean.item()
+        c = self.config
+        return engine.FlexMFState(
+            params, users, items, loss="mse", reg_method=c.reg_method, negative_count=0, batch_size=c.batch_size,
+            learning_rate=c.learning_rate, regularization=c.regularization, ratings=values - mean, device=self.device,
+        )  # fmt: skip

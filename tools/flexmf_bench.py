@@ -1,18 +1,20 @@
 #!/usr/bin/env python
 """
-FlexMF implicit training at the synthetic ML-25M shape (162,541 x 59,047, 25,000,095 interactions), k = 64,
-negative_count 1, on one GPU.  Per configuration and batch size:
+FlexMF training at the synthetic ML-25M shape (162,541 x 59,047, 25,000,095 interactions), k = 64, on one GPU:
+``--model implicit`` (default) with negative_count 1, or ``--model explicit``, the squared error on the generator's
+ratings less their mean, no negatives and no bias terms (the reference's explicit model).  Per configuration and
+batch size:
 
 * epoch time (host clock around a synchronise; median of ``--epochs`` epochs after one warm-up epoch), split into the
   part before the first step (``plan_batches``: sampling, sorting, grouping) and the steps (``run_batches``);
-* the same ``--steps`` steps on the device step and on the plain-torch step of ``tests/flexmf_oracle.py`` run on the
-  same device (autograd + ``torch.optim``), alternated, both fed the device sampler's negatives and neither charged
-  for the grouping; their parameters are
-  compared first (update error ‖new − want‖ / ‖want − old‖ after ``--steps`` steps, bound 1e-3: f32 rounding
+* the same ``--steps`` steps on the device step and on the plain-torch step of ``tests/flexmf_oracle.py`` (explicit:
+  ``tests/flexmf_explicit_oracle.py``) run on the same device (autograd + ``torch.optim``), alternated, both fed the
+  device sampler's negatives and neither charged for the grouping; their parameters are compared first (update error ‖new − want‖ / ‖want − old‖ after ``--steps`` steps, bound 1e-3: f32 rounding
   through that many Adam steps);
 * kernel time per step by kernel name from ``torch.profiler`` in a separate pass over the steps alone, the launch gaps
   (wall time per step with the profiler off minus that sum), and the bytes each kernel must move, from shapes, against 3.35 TB/s;
-* a NumPy rejection sampler on the host for one batch, the stand-in for what a host-side sampler costs per step.
+* implicit only: a NumPy rejection sampler on the host for one batch, the stand-in for what a host-side sampler
+  costs per step.
 
 Prints one JSON line per measurement; needs a CUDA device.
 """
@@ -33,17 +35,20 @@ import torch
 ROOT = Path(__file__).resolve().parent.parent
 sys.path[:0] = [str(ROOT), str(ROOT / "tests")]
 
+import flexmf_explicit_oracle as feo  # noqa: E402
 import flexmf_oracle as fo  # noqa: E402
 from lkpy_b200 import _lib, engine, flexmf, prep  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12  # H100 SXM data sheet
 CONFIGS = [("logistic", "AdamW", True), ("logistic", "L2", True), ("pairwise", None, False)]
+EXPLICIT_CONFIGS = [("mse", "L2", False), ("mse", "AdamW", False), ("mse", None, False)]
 
 
-def step_bytes(n_users, n_items, k, B, n, reg_method, ub, ib, uniq_u, uniq_i) -> dict[str, float]:
+def step_bytes(n_users, n_items, k, B, n, reg_method, ub, ib, uniq_u, uniq_i, targets=False) -> dict[str, float]:
     """Bytes each kernel of a step has to move, from shapes (row gathers counted once per occurrence)."""
     row = 4 * k
     fwd = B * (row + (n + 1) * row) + 4 * B * (n + 3) + 4 * B * (n + 2)  # rows, indices and biases, coef + loss out
+    fwd += 4 * B if targets else 0
     grad = B * (n + 1) * row * 2 + 4 * B * (n + 1) * 2 + (uniq_u + uniq_i) * (row + 4)  # both sides' gathers, partials
     cols = k + (1 if ub else 0), k + (1 if ib else 0)
     if reg_method == "AdamW":
@@ -62,33 +67,40 @@ def main() -> None:
     ap.add_argument("--epochs", type=int, default=3)
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--batch-sizes", type=int, nargs="+", default=[8192, 65536])
+    ap.add_argument("--model", choices=["implicit", "explicit"], default="implicit")
     a = ap.parse_args()
+    explicit = a.model == "explicit"
     dev = _lib.require_device()
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                          text=True).stdout.strip()  # fmt: skip
     print(json.dumps({"gpu": torch.cuda.get_device_name(0), "nvidia_smi_name_power_limit": smi}), flush=True)
-    users, items, _ = prep.synth_interactions_device(a.users, a.items, a.nnz, device=dev)
-    k, n = 64, 1
+    users, items, ratings = prep.synth_interactions_device(a.users, a.items, a.nnz, device=dev)
+    k, n = 64, 0 if explicit else 1
+    targets = None
+    if explicit:  # the explicit trainer's targets: ratings less their f32 mean, formed on the host
+        host_r = ratings.cpu()
+        targets = (host_r - host_r.mean()).to(dev)
+    else:
+        # host rejection sampler, one batch of 8,192
+        hu, hi = users.cpu().numpy(), items.cpu().numpy()
+        indptr = np.concatenate([[0], np.cumsum(np.bincount(hu, minlength=a.users))])
+        rows = hu[np.random.default_rng(0).integers(0, a.nnz, 8192)]
+        t0 = time.perf_counter()
+        fo.sample_negatives(indptr, hi, rows, a.items, n, seed=1)
+        print(json.dumps({"host_numpy_sampler_ms_per_8192_batch": (time.perf_counter() - t0) * 1e3}), flush=True)
 
-    # host rejection sampler, one batch of 8,192
-    hu, hi = users.cpu().numpy(), items.cpu().numpy()
-    indptr = np.concatenate([[0], np.cumsum(np.bincount(hu, minlength=a.users))])
-    rows = hu[np.random.default_rng(0).integers(0, a.nnz, 8192)]
-    t0 = time.perf_counter()
-    fo.sample_negatives(indptr, hi, rows, a.items, n, seed=1)
-    print(json.dumps({"host_numpy_sampler_ms_per_8192_batch": (time.perf_counter() - t0) * 1e3}), flush=True)
-
-    for loss, reg_method, biases in CONFIGS:
+    for loss, reg_method, biases in EXPLICIT_CONFIGS if explicit else CONFIGS:
         for B in a.batch_sizes:
-            tag = {"loss": loss, "reg_method": reg_method, "batch_size": B}
+            tag = ({"model": "explicit"} if explicit else {}) | {"loss": loss, "reg_method": reg_method, "batch_size": B}
             params = flexmf.initial_parameters(a.users, a.items, k, biases, biases, torch.Generator().manual_seed(1))
             mk = lambda: engine.FlexMFState(params, users, items, loss=loss, reg_method=reg_method, batch_size=B,  # noqa: E731
-                                            seed=5, device=dev)  # fmt: skip
+                                            negative_count=n, ratings=targets, seed=5, device=dev)  # fmt: skip
             # --- the same steps on both paths: first compared, then timed alternately
             st = mk()
             at = torch.randperm(a.nnz, device=dev, generator=torch.Generator(dev).manual_seed(3))[: a.steps * B]
             su, sp = users[at], items[at]
-            sneg = st.sample(su)
+            sneg = None if explicit else st.sample(su)
+            sr = targets[at] if explicit else None
             model = fo.Model(params, sparse=reg_method != "AdamW", device=dev)
             opt = fo.make_optimizer(model, reg_method, st.lr, st.reg)
             kw = dict(loss=loss, reg_method=reg_method, regularization=st.reg, positive_weight=1.0)
@@ -96,7 +108,10 @@ def main() -> None:
             def torch_steps():
                 for s in range(a.steps):
                     sl = slice(s * B, (s + 1) * B)
-                    out = fo.batch_loss(model, su[sl], sp[sl], sneg[sl], **kw)
+                    if explicit:
+                        out, _ = feo.mse_terms(model, su[sl], sp[sl], sr[sl], reg_method=reg_method, regularization=st.reg)
+                    else:
+                        out = fo.batch_loss(model, su[sl], sp[sl], sneg[sl], **kw)
                     out.backward()
                     opt.step()
                     opt.zero_grad()
@@ -108,7 +123,7 @@ def main() -> None:
                 torch.cuda.synchronize()
                 return out, time.perf_counter() - t0
 
-            plan, plan_s = timed(lambda: st.plan_batches(su, sp, sneg))  # sorts and grouping: not part of a step
+            plan, plan_s = timed(lambda: st.plan_batches(su, sp, sneg, ratings=sr))  # sorts and grouping: not part of a step
             st.run_batches(plan)
             torch_steps()
             errs = {}
@@ -136,8 +151,8 @@ def main() -> None:
                     name = next(nm for nm in ("forward", "loss", "grad", "update", "sample") if f"flexmf_{nm}" in e.key)
                     kern[f"flexmf_{name}_kernel"] = kern.get(f"flexmf_{name}_kernel", 0.0) + e.device_time_total / a.steps
             uq_u = float(torch.unique(su[:B]).numel())
-            uq_i = float(torch.unique(torch.cat([sp[:B], sneg[:B, 0]])).numel())
-            need = step_bytes(a.users, a.items, k, B, n, reg_method, biases, biases, uq_u, uq_i)
+            uq_i = float(torch.unique(sp[:B] if explicit else torch.cat([sp[:B], sneg[:B, 0]])).numel())
+            need = step_bytes(a.users, a.items, k, B, n, reg_method, biases, biases, uq_u, uq_i, targets=explicit)
             rows_out = {nm: {"us_per_step": us, "bytes": need.get(nm), "share_of_3.35TBps":
                              (need[nm] / HBM_BYTES_PER_S) / (us * 1e-6) if nm in need and us > 0 else None}
                         for nm, us in kern.items()}  # fmt: skip
@@ -152,7 +167,8 @@ def main() -> None:
             ep = []
             for e in range(a.epochs + 1):
                 perm = torch.from_numpy(rng.permutation(a.nnz)).to(dev)
-                plan, plan_s = timed(lambda: st.plan_batches(users[perm], items[perm]))
+                plan, plan_s = timed(lambda: st.plan_batches(users[perm], items[perm],
+                                                             ratings=targets[perm] if explicit else None))  # fmt: skip
                 losses, run_s = timed(lambda: st.run_batches(plan))
                 del plan
                 mean = float(losses.double().mean().item())
