@@ -26,6 +26,8 @@
  *   FlexMFImplicitTrainer.train_batch (autograd)  src/lenskit/flexmf/_implicit.py:253-274 lk_flexmf_step
  *   FlexMFExplicitTrainer.train_batch (autograd)  src/lenskit/flexmf/_explicit.py:108-125 lk_flexmf_step (LK_FLEXMF_MSE)
  *   FlexMFScorerBase.__call__ + TopNRanker        src/lenskit/flexmf/_base.py:117-157 lk_als_recommend_batch (biases as offsets)
+ *   TruncatedSVD sparse products (SciPy, host)    src/lenskit/sklearn/svd.py         lk_spmm
+ *   BiasedSVDScorer.__call__ + TopNRanker         src/lenskit/sklearn/svd.py         lk_als_recommend_batch (biases as offsets)
  *
  * Conventions
  *   - plain C: pointers and sizes only; no C++/torch types cross this boundary;
@@ -744,6 +746,28 @@ typedef struct lk_flexmf_step_args {
 
 LK_API int lk_flexmf_workspace_bytes(int32_t batch, int32_t n_neg, int32_t k, int64_t *bytes);
 LK_API int lk_flexmf_step(const lk_flexmf_step_args *args, void *stream);
+
+/* ------------------------------------------------------------------------
+ * Sparse x dense product (spmm.cu), the products of TruncatedSVD's randomized SVD (BiasedSVDScorer,
+ * src/lenskit/sklearn/svd.py).  Y [n_rows][W] = A D with A a CSR [n_rows x n_src] and D [n_src][W] row-major:
+ *     Y[r][c] = +0.0f;  for p in row r in stored order: Y[r][c] = Y[r][c] + val[p] * D[idx[p]][c]
+ * with the product and the sum each rounded to nearest (never one FMA).  That is SciPy's f32 `A @ D` bit for bit;
+ * `A.T @ D` and `D.T @ A` are the same walk over the transposed CSR (rows in ascending order inside a row).
+ * d_order lists every row once, longest first: the order in which rows are handed to the warps.
+ * ---------------------------------------------------------------------- */
+typedef struct lk_spmm_args {
+    int32_t n_rows, n_src;
+    int32_t width;                     /* W >= 1 */
+    int64_t nnz;                       /* < 2^31 */
+    const int32_t *d_indptr;           /* [n_rows+1] */
+    const int32_t *d_indices;          /* [nnz] in [0, n_src) */
+    const float *d_values;             /* [nnz] */
+    const int32_t *d_order;            /* [n_rows] a permutation of the rows */
+    const float *d_dense;              /* D [n_src][W] */
+    float *d_out;                      /* Y [n_rows][W], must not overlap D */
+} lk_spmm_args;
+
+LK_API int lk_spmm(const lk_spmm_args *args, void *stream);
 
 #ifdef __cplusplus
 }

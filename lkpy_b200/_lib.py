@@ -366,6 +366,21 @@ class LkFlexmfStepArgs(C.Structure):
     ]  # fmt: skip
 
 
+class LkSpmmArgs(C.Structure):
+    _fields_ = [
+        ("n_rows", C.c_int32),
+        ("n_src", C.c_int32),
+        ("width", C.c_int32),
+        ("nnz", C.c_int64),
+        ("d_indptr", vp),
+        ("d_indices", vp),
+        ("d_values", vp),
+        ("d_order", vp),
+        ("d_dense", vp),
+        ("d_out", vp),
+    ]
+
+
 #: every symbol ``include/lkpy_b200.h`` declares: name -> (restype, argtypes)
 SYMBOLS: dict[str, tuple] = {
     "lk_version": (C.c_int, []),
@@ -415,6 +430,7 @@ SYMBOLS: dict[str, tuple] = {
     "lk_flexmf_sample_negatives": (C.c_int, [C.POINTER(LkFlexmfSampleArgs), vp]),
     "lk_flexmf_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, i64p]),
     "lk_flexmf_step": (C.c_int, [C.POINTER(LkFlexmfStepArgs), vp]),
+    "lk_spmm": (C.c_int, [C.POINTER(LkSpmmArgs), vp]),
 }
 
 _lib = None

@@ -563,10 +563,15 @@ class BiasModel:
         self.damping = damping
 
     @classmethod
-    def learn(cls, it: Interactions, damping) -> "BiasModel":
+    def learn(cls, it: Interactions, damping, centered_dtype=np.float64) -> "BiasModel":
+        """``damping``: one float for both, a ``(user, item)`` tuple, or a dict ``{"user": ..., "item": ...}`` in
+        which a missing key means 0.  ``centered_dtype`` is the type of the centred ratings, which the reference
+        takes from its rating matrix: ``np.float32`` gives its statements on an f32 matrix exactly."""
+        if isinstance(damping, dict):
+            damping = (float(damping.get("user", 0.0)), float(damping.get("item", 0.0)))
         d_user, d_item = damping if isinstance(damping, tuple) else (damping, damping)
         g = float(np.mean(it.ratings))
-        centered = it.ratings.astype(np.float64) - g
+        centered = it.ratings.astype(centered_dtype) - g
         counts = np.full(it.n_items, float(d_item))
         sums = np.zeros(it.n_items)
         np.add.at(counts, it.items, 1)
@@ -581,6 +586,14 @@ class BiasModel:
         ub = np.zeros(it.n_users, dtype=np.float32)
         np.divide(sums, counts, out=ub, where=counts > 0, casting="unsafe")
         return cls(g, ib, ub, (d_user, d_item))
+
+    def batch_offsets(self, user_nums: np.ndarray, fold_bias: np.ndarray | None):
+        """``compute_for_items`` for a batch, as score offsets: global + item bias per item (f32, the global bias
+        rounded to f32 first), and per query the user's bias, or ``fold_bias`` where that is not NaN."""
+        ub = np.where(user_nums >= 0, self.user_biases[np.maximum(user_nums, 0)], 0.0).astype(np.float32)
+        if fold_bias is not None:
+            ub = np.where(np.isnan(fold_bias), ub, fold_bias).astype(np.float32)
+        return (self.item_biases + self.global_bias).astype(np.float32), ub
 
     def transform(self, it: Interactions) -> np.ndarray:
         return (it.ratings - self.global_bias - self.item_biases[it.items] - self.user_biases[it.users]).astype(
@@ -675,10 +688,7 @@ class BiasedMFScorer(ALSBase):
 
     def batch_offsets(self, user_nums: np.ndarray, fold_bias: np.ndarray | None):
         """``finalize_scores`` for a batch: global + item bias per item, user bias per query."""
-        ub = np.where(user_nums >= 0, self.bias.user_biases[np.maximum(user_nums, 0)], 0.0).astype(np.float32)
-        if fold_bias is not None:
-            ub = np.where(np.isnan(fold_bias), ub, fold_bias).astype(np.float32)
-        return (self.bias.item_biases + self.bias.global_bias).astype(np.float32), ub
+        return self.bias.batch_offsets(user_nums, fold_bias)
 
 
 class BiasedMFTrainer(ALSTrainerBase):

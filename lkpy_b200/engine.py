@@ -8,6 +8,7 @@ PyTorch is used for device memory, streams and (in ``lkpy_b200.parallel``)
 
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import threading
 from dataclasses import dataclass, field
@@ -18,7 +19,8 @@ import torch
 from . import _lib
 from ._lib import (
     LkAlsArgs, LkAlsRecArgs, LkAssocScoreArgs, LkCoocArgs, LkEaseScoreArgs, LkFlexmfSampleArgs, LkFlexmfStepArgs,
-    LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkSlimArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr,
+    LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkSlimArgs, LkSpmmArgs, LkUknnSearchArgs, check, lib, ptr,
+    stream_ptr,
 )  # fmt: skip
 from .data import InteractionCSR
 
@@ -1318,6 +1320,137 @@ class EaseState:
         """
         return _rank_launch(self._args(hist_indptr, hist_items), lib().lk_ease_score_batch, "lk_ease_score_batch", n,
                             self.n_items, hist_indptr.numel() - 1, self.weights.device, excl_indptr, excl_items)
+
+
+# ---------------------------------------------------------------------------
+# Sparse x dense products and the randomized SVD (BiasedSVD)
+# ---------------------------------------------------------------------------
+
+
+def spmm_order(m: DeviceCSR) -> torch.Tensor:
+    """The rows of ``m`` longest first (int32, ties ascending): the order ``lk_spmm`` hands rows to warps."""
+    return torch.argsort(m.indptr[1:] - m.indptr[:-1], descending=True, stable=True).to(torch.int32)
+
+
+def spmm(m: DeviceCSR, order: torch.Tensor, dense: torch.Tensor) -> torch.Tensor:
+    """
+    ``m @ dense`` (``lk_spmm``), f32 [n_rows, W]: every element one sequential sum over the row's stored entries,
+    product and sum each rounded, which is SciPy's f32 product bit for bit.  ``order`` is :func:`spmm_order` of ``m``.
+    """
+    if dense.dtype != torch.float32 or dense.dim() != 2 or dense.shape[0] != m.shape[1] or dense.shape[1] < 1:
+        raise ValueError(f"dense operand must be f32 [{m.shape[1]}, W >= 1], not {dense.dtype} {tuple(dense.shape)}")
+    dense = dense.contiguous()
+    out = torch.empty((m.shape[0], dense.shape[1]), dtype=torch.float32, device=dense.device)
+    a = LkSpmmArgs()
+    a.n_rows, a.n_src, a.width, a.nnz = m.shape[0], m.shape[1], dense.shape[1], m.nnz
+    a.d_indptr, a.d_indices, a.d_values = ptr(m.indptr), ptr(_nonempty(m.indices)), ptr(_nonempty(m.values))
+    a.d_order, a.d_dense, a.d_out = ptr(order), ptr(dense), ptr(out)
+    check(lib().lk_spmm(C.byref(a), stream_ptr()), "lk_spmm")
+    return out
+
+
+def lu_permuted_l(a: torch.Tensor) -> torch.Tensor:
+    """
+    ``scipy.linalg.lu(a, permute_l=True)[0]``, the product P L of ``a = P L U``, from ``torch.linalg.lu_factor_ex``
+    (getrf).  P is never formed: the pivots (min(m, n) row swaps, read on the host) become a row permutation that is
+    applied to L as a gather.  Shape [m, min(m, n)].
+    """
+    m, n = a.shape
+    r = min(m, n)
+    lu, piv, _info = torch.linalg.lu_factor_ex(a)  # a singular U is no error, as in SciPy
+    L = lu[:, :r].tril(-1)
+    L.diagonal().fill_(1.0)
+    perm = np.arange(m)
+    for i, t in enumerate(piv.cpu().numpy().astype(np.int64) - 1):  # LAPACK's 1-based swaps, applied in order
+        perm[i], perm[t] = perm[t], perm[i]
+    inv = np.empty(m, dtype=np.int64)
+    inv[perm] = np.arange(m)  # row perm[i] of P L is row i of L
+    return L[torch.from_numpy(inv).to(a.device)]
+
+
+@dataclass
+class SvdOperand:
+    """
+    A sparse matrix M for the randomized SVD, with Mᵀ beside it: both orientations in HBM and each one's row order
+    for ``lk_spmm``.  ``M @ D`` is ``spmm(rows)``, ``Mᵀ @ D`` is ``spmm(cols)``.
+    """
+
+    rows: DeviceCSR
+    cols: DeviceCSR
+    rows_order: torch.Tensor
+    cols_order: torch.Tensor
+
+    @classmethod
+    def create(cls, rows: DeviceCSR, cols: DeviceCSR) -> "SvdOperand":
+        return cls(rows, cols, spmm_order(rows), spmm_order(cols))
+
+    @property
+    def shape(self) -> tuple[int, int]:
+        return self.rows.shape
+
+    def mul(self, d: torch.Tensor) -> torch.Tensor:
+        return spmm(self.rows, self.rows_order, d)
+
+    def tmul(self, d: torch.Tensor) -> torch.Tensor:
+        return spmm(self.cols, self.cols_order, d)
+
+    @property
+    def T(self) -> "SvdOperand":
+        return SvdOperand(self.cols, self.rows, self.cols_order, self.rows_order)
+
+
+def randomized_svd(x: SvdOperand, q0: torch.Tensor, k: int, n_iter: int, stage=None):
+    """
+    ``TruncatedSVD(k, algorithm="randomized", n_iter=n_iter).fit`` of the f32 matrix X (scikit-learn's
+    ``_randomized_svd`` with ``flip_sign=False``, then ``svd_flip(u_based_decision=False)``) on the device: returns
+    ``(components_ [k, n_cols], singular_values_ [k])``.  M is Xᵀ when X has fewer rows than columns, else X; ``q0``
+    is the start matrix [M.shape[1], k + oversamples].  The sparse products run on ``lk_spmm`` (SciPy's bit for
+    bit); the LU (with ``n_iter > 2``), QR and SVD are torch's (cuSOLVER) in f32.  ``stage(name)``, when given, is
+    a context manager entered around each step (benchmark timing).
+    """
+    stage = stage or (lambda _name: contextlib.nullcontext())
+    with _prefer_cusolver():
+        return _randomized_svd(x, q0, k, n_iter, stage)
+
+
+@contextlib.contextmanager
+def _prefer_cusolver():
+    """torch's dense factorisations on cuSOLVER for the duration (its default may pick MAGMA's batched LU, which is
+    meant for many small matrices and says so on stdout); the caller's preference is restored after."""
+    before = torch.backends.cuda.preferred_linalg_library()
+    torch.backends.cuda.preferred_linalg_library("cusolver")
+    try:
+        yield
+    finally:
+        torch.backends.cuda.preferred_linalg_library(before)
+
+
+def _randomized_svd(x: SvdOperand, q0: torch.Tensor, k: int, n_iter: int, stage):
+    transpose = x.shape[0] < x.shape[1]
+    M = x.T if transpose else x
+    Q = q0
+    normalise = n_iter > 2  # power_iteration_normalizer="auto": LU, or nothing with n_iter <= 2
+    for _ in range(n_iter):
+        for product in (M.mul, M.tmul):
+            with stage("spmm_power"):
+                Q = product(Q)
+            if normalise:
+                with stage("lu"):
+                    Q = lu_permuted_l(Q)
+    with stage("spmm_power"):
+        Y = M.mul(Q)
+    with stage("qr"):
+        Q = torch.linalg.qr(Y, mode="reduced")[0]
+    with stage("spmm_project"):
+        B = M.tmul(Q).T  # Q.T @ M, which SciPy computes as (Mᵀ @ Q).T
+    with stage("svd"):
+        Uh, s, Vt = torch.linalg.svd(B, full_matrices=False)
+        vt = (Q @ Uh[:, :k]).T if transpose else Vt[:k]  # the right singular vectors of X
+    with stage("flip"):
+        # svd_flip(u_based_decision=False): each row's sign is that of its first entry of largest magnitude
+        pick = vt.abs().argmax(dim=1, keepdim=True)
+        vt = vt * torch.sign(torch.gather(vt, 1, pick))
+    return vt.contiguous(), s[:k].contiguous()
 
 
 # ---------------------------------------------------------------------------
