@@ -96,7 +96,10 @@ LK_API int lk_als_max_features(void);
 /*
  * Row scheduling plan (host side, once per matrix).  Rows are cut into chunks
  * of at most `chunk_nnz` nonzeros so that power-law rows neither serialise on
- * one warp nor unbalance the grid; chunks are ordered longest-row-first.  Each
+ * one warp nor unbalance the grid; chunks are ordered longest-row-first.
+ * `chunk_nnz` must be a positive multiple of 32 (else LK_ERR_INVALID); a row
+ * longer than it is cut into ceil(n / chunk_nnz) parts of 1 .. chunk_nnz
+ * nonzeros each (equal lengths rounded up to 32, the last part shorter).  Each
  * chunk record is 8 int32:
  *   {row, nnz_begin, nnz_len, n_parts, first_slot, part_index, split_index, 0}
  * n_parts == 1 for a whole row.  Rows split into several chunks accumulate

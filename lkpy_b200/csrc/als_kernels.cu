@@ -195,7 +195,8 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, AlsCfg<KP>::OCC) als_half_kern
             }
         };
 
-        issue(0, cA);
+        // an empty part must not arm a stage it never waits on (the phase bits would fall out of step)
+        if (n_it > 0) issue(0, cA);
         for (int it = 0; it < n_it; it++) {
             const int s = it & 1;
             // column indices two stages ahead
@@ -492,8 +493,10 @@ int64_t lk_als_slot_floats(int32_t k)
 static int plan_impl(const int32_t *indptr, int64_t n_rows, int32_t chunk_nnz, int64_t *n_chunks,
                      int64_t *n_split, int64_t *n_slots, int32_t *out)
 {
-    LK_REQUIRE(indptr != nullptr && n_rows >= 0 && chunk_nnz >= 32, LK_ERR_INVALID,
-               "lk_als_plan: bad arguments");
+    // chunk_nnz a multiple of 32: then plen <= chunk_nnz, so (parts - 1) * plen < n and no part is empty
+    // or longer than chunk_nnz (other lengths can round plen up far enough to leave the last part empty)
+    LK_REQUIRE(indptr != nullptr && n_rows >= 0 && chunk_nnz >= 32 && chunk_nnz % 32 == 0, LK_ERR_INVALID,
+               "lk_als_plan: bad arguments (chunk_nnz must be a positive multiple of 32)");
     std::vector<int32_t> order((size_t)n_rows);
     std::iota(order.begin(), order.end(), 0);
     std::stable_sort(order.begin(), order.end(), [&](int32_t x, int32_t y) {

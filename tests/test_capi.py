@@ -55,25 +55,49 @@ def test_no_fallback_without_device():
         accel.run_accel_task(accel.als.train_implicit_matrix(ui, p, q, np.eye(8, dtype=np.float32)))
 
 
-@pytest.mark.parametrize("chunk", [32, 64, 4096])
+def _boundary_lengths(chunk: int) -> list[int]:
+    """Row lengths where the ALS kernels change behaviour (32-row stages, 16 / 8-row MMA steps, part cuts)."""
+    base = [0, 1, 2, 7, 8, 9, 15, 16, 17, 31, 32, 33, 63, 64, 65, 95, 96, 97, 127, 128, 129, 481]
+    return base + [chunk - 1, chunk, chunk + 1, 2 * chunk, 2 * chunk + 1, 3 * chunk - 1, 40 * chunk + 1]
+
+
+@pytest.mark.parametrize("chunk", [32, 64, 96, 256, 1024, 4096])
 def test_als_plan_covers_every_nonzero_once(cuda_lib, chunk):
     inter = small_synth(3000, 500, 80000, seed=8)
     _ui, iu = data.als_implicit_matrices(inter)
-    hp = iu.indptr
+    _check_plan(cuda_lib, iu.indptr, chunk)
+
+
+@pytest.mark.parametrize("chunk", [32, 64, 96, 256, 1024, 4096])
+def test_als_plan_boundary_lengths(cuda_lib, chunk):
+    """The same plan checks on rows of the lengths where the kernels change behaviour: every boundary length of
+    every chunk size under test (so each plan also sees the others' cut points), then this chunk size's own."""
+    lens = sorted({n for c in (32, 33, 40, 48, 50, 64, 96, 100, 256, 1024) for n in _boundary_lengths(c)})
+    lens += _boundary_lengths(chunk)
+    _check_plan(cuda_lib, np.concatenate([[0], np.cumsum(lens)]).astype(np.int32), chunk)
+
+
+def _check_plan(cuda_lib, hp, chunk):
+    n_rows = len(hp) - 1
+    nnz = int(hp[-1])
     nc, ns, nslot = C.c_int64(), C.c_int64(), C.c_int64()
-    _lib.check(cuda_lib.lk_als_plan_size(hp.ctypes.data, iu.shape[0], chunk, C.byref(nc), C.byref(ns), C.byref(nslot)))
+    _lib.check(cuda_lib.lk_als_plan_size(hp.ctypes.data, n_rows, chunk, C.byref(nc), C.byref(ns), C.byref(nslot)))
     ch = np.empty((nc.value, 8), dtype=np.int32)
-    _lib.check(cuda_lib.lk_als_plan_fill(hp.ctypes.data, iu.shape[0], chunk, ch.ctypes.data))
+    _lib.check(cuda_lib.lk_als_plan_fill(hp.ctypes.data, n_rows, chunk, ch.ctypes.data))
     row, begin, ln, parts, slot0, part, split = (ch[:, i] for i in range(7))
-    assert ln.max() <= max(chunk, 32) and ln.min() >= 0
-    cover = np.zeros(iu.nnz, dtype=np.int32)
+    assert ln.max() <= chunk
+    # every part of a split row holds 1 .. chunk nonzeros, and a row has exactly ceil(n / chunk) parts
+    assert np.all(ln[parts > 1] >= 1)
+    assert np.all(parts == np.maximum(1, -(-np.diff(hp)[row] // chunk)))
+    np.testing.assert_array_equal(np.bincount(row, minlength=n_rows)[row], parts)
+    cover = np.zeros(nnz, dtype=np.int32)
     for b, l in zip(begin, ln):
         cover[b : b + l] += 1
     assert np.all(cover == 1)
     assert np.all(begin >= hp[row]) and np.all(begin + ln <= hp[row + 1])
     nnz_row = np.diff(hp)
     # every row appears; split rows have consistent part numbering and disjoint slots
-    assert set(row.tolist()) == set(range(iu.shape[0]))
+    assert set(row.tolist()) == set(range(n_rows))
     whole = parts == 1
     assert np.all(ln[whole] == nnz_row[row[whole]])
     sp = ~whole
@@ -87,7 +111,23 @@ def test_als_plan_covers_every_nonzero_once(cuda_lib, chunk):
     order = sorted(first_of_row, key=first_of_row.get)
     assert np.all(np.diff(nnz_row[order]) <= 0)
     with pytest.raises(_lib.EngineError):
-        _lib.check(cuda_lib.lk_als_plan_size(hp.ctypes.data, iu.shape[0], 8, C.byref(nc), C.byref(ns), C.byref(nslot)))
+        _lib.check(cuda_lib.lk_als_plan_size(hp.ctypes.data, n_rows, 8, C.byref(nc), C.byref(ns), C.byref(nslot)))
+
+
+@pytest.mark.parametrize("chunk", [8, 31, 33, 40, 48, 50, 100, 4095])
+def test_als_plan_rejects_chunk_not_multiple_of_32(cuda_lib, chunk):
+    """Equal parts rounded up to 32 nonzeros only stay within 1 .. chunk_nnz when chunk_nnz is a multiple of 32:
+    at 40 a row of 97 would be cut 64 + 33 + 0 (also 97 at 33 or 48, 101 at 50, 481 at 100).  Such sizes are
+    refused by both calls rather than planned with an empty or overlong part."""
+    lens = _boundary_lengths(32) + [97, 101, 481]
+    hp = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
+    nc, ns, nslot = C.c_int64(), C.c_int64(), C.c_int64()
+    with pytest.raises(_lib.EngineError, match="multiple of 32"):
+        _lib.check(cuda_lib.lk_als_plan_size(hp.ctypes.data, len(lens), chunk, C.byref(nc), C.byref(ns), C.byref(nslot)))
+    out = np.zeros((4096, 8), dtype=np.int32)
+    with pytest.raises(_lib.EngineError, match="multiple of 32"):
+        _lib.check(cuda_lib.lk_als_plan_fill(hp.ctypes.data, len(lens), chunk, out.ctypes.data))
+    assert not out.any()
 
 
 def test_knn_geometry(cuda_lib, lk_options):
