@@ -524,7 +524,9 @@ LK_API int lk_cooc_dense(int32_t n_items, const int64_t *d_indptr, const int32_t
  * r_0 .. r_{R-1} (d_ref_items in query order, repeats kept, all in [0, n_items)) and item c:
  *   agg 0 (mean, max_nbrs = None):  s = +0.0f;  for t = 0 .. R-1: s = s + A[r_t, c]  (f32 adds in query order,
  *                                   absent entries add nothing);  score = f32(f64(s) / f64(R))
- *   agg 1 (max, max_nbrs = 1):      score = max over t of A[r_t, c], absent entries 0
+ *   agg 1 (max, max_nbrs = 1):      score = max over t of A[r_t, c], absent entries 0; the max starts at +0.0f,
+ *                                   so A must be non-negative (as training makes it; NaN entries are outside
+ *                                   the contract: fmaxf drops them where np.max would propagate them)
  *   agg 2 (sum, SLIMScorer):        s as for agg 0, score = s (no divide)
  *   R == 0: every score is NaN (agg 0, 1; rank mode recommends nothing), +0.0 (agg 2; rank mode ranks the zeros).
  * A is the association CSR (int64 offsets, rows sorted by column); d_tile_ptr [n_items * (n_subtiles+1)] holds,
@@ -532,7 +534,8 @@ LK_API int lk_cooc_dense(int32_t n_items, const int64_t *d_indptr, const int32_t
  * start (lk_assoc_tile_pointers).
  *   n == 0  score mode: d_scores [n_queries][n_items].
  *   n >= 1  rank mode (n <= lk_topn_max()): argtopn over every item ascending minus the query's excluded items
- *           (ascending within a query, repeats and negative numbers skipped), ties included; outputs as
+ *           (ascending within a query, repeats and negative numbers skipped), ties included; a NaN score (+inf
+ *           and -inf at one column of two reference rows) is never offered, as argtopn skips it; outputs as
  *           lk_als_recommend_batch's rank mode.
  * n_queries * geom.n_halves < 2^31.
  * ---------------------------------------------------------------------- */

@@ -20,7 +20,7 @@
 // adds as NumPy's np.mean(axis=0) over the dense rows (absent entries add +0.0, which changes nothing).  In rank
 // mode warp 0 then offers the tile's scores in ascending item order to argtopn's heap (topn_heap.cuh), keeping
 // only count < n || s > root (exact: a full heap's root never decreases and a full heap rejects s <= root) and
-// skipping excluded items (argtopn's NaN offer).
+// skipping NaN scores (+inf and -inf in two reference rows at one column) and excluded items (argtopn's NaN offer).
 #include "tiles.cuh"
 #include "topn_heap.cuh"
 
@@ -274,7 +274,7 @@ __global__ void __launch_bounds__(CO_NT, CO_CTAS) assoc_score_kernel(const lk_as
                 for (int j0 = 0; j0 < CW; j0 += 32) {
                     const int c = h * CW + j0 + lane;
                     const float sc = acc[j0 + lane];
-                    unsigned b = __ballot_sync(FULL, c < NI && (count < n || sc > root));
+                    unsigned b = __ballot_sync(FULL, c < NI && sc == sc && (count < n || sc > root));
                     if (lane == 0) {
                         while (b) {
                             const int l = __ffs(b) - 1;
