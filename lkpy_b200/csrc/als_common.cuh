@@ -45,20 +45,232 @@ __device__ __forceinline__ float rsqrt_nr(float x)
     return r * fmaf(-h * r, r, 1.5f);
 }
 
+// a0 b0 + a1 b1 + a2 b2 + a3 b3 in one fixed expression shape: the sums of one 4-column panel
+__device__ __forceinline__ float dot4(float a0, float b0, float a1, float b1, float a2, float b2, float a3, float b3)
+{
+    return a0 * b0 + a1 * b1 + a2 * b2 + a3 * b3;
+}
+
+// One-warp systems (KP = 32, 64): the chol_solve contract below with 8-column panels.  Every lane
+// factors the 8x8 diagonal block redundantly from broadcast reads, then solves the panel entries of its
+// rows t and t + 32 into registers (x[q][0..7]), applies them to its right-hand side and updates the
+// trailing matrix in tiles 8 columns wide, so each trailing element is read and written once per 8
+// columns of the factor instead of once per 4.
+//
+// The arithmetic is that of 4-column panels, operation for operation: where the second half of a panel
+// (columns 4..7) meets the first, the first half's contribution is one dot4 subtracted before the second
+// half's own terms, exactly as a separate 4-column panel's trailing update would have left it.  The
+// trailing update subtracts the two halves' dot4s in turn, and the back substitution handles each 8-unknown
+// step as two 4-unknown ones.  So the factor, x and the status are bit-identical to a 4-column solve.  A
+// pivot row runs the same recurrence as the rows below it, which reproduces the broadcast factor's row
+// exactly (same operands in the same order); its entries right of the diagonal are stored as zero.
+template <int KP>
+__device__ __forceinline__ bool chol_solve_warp(float *As, float *ys, float *dinv, const int tid)
+{
+    constexpr int LDA = KP + 4, RPT = KP / 32, P = 8;
+    static_assert(KP % P == 0 && RPT >= 1, "one warp, whole 8-column panels");
+    bool bad = false;
+    float yv[RPT];
+#pragma unroll
+    for (int q = 0; q < RPT; q++) yv[q] = ys[tid + q * 32];
+
+    for (int j0 = 0; j0 < KP; j0 += P) {
+        // pivot block: rows j0..j0+7 of columns j0..j0+7, a diagonal block of the system (only its lower
+        // triangle is used)
+        float l[P][P], inv[P], z[P];
+#pragma unroll
+        for (int r = 0; r < P; r++)
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                if (4 * h > r) continue;
+                const float4 v = *reinterpret_cast<const float4 *>(As + (j0 + r) * LDA + j0 + 4 * h);
+                l[r][4 * h] = v.x, l[r][4 * h + 1] = v.y, l[r][4 * h + 2] = v.z, l[r][4 * h + 3] = v.w;
+            }
+        {
+            const float4 y0 = *reinterpret_cast<const float4 *>(ys + j0);
+            const float4 y1 = *reinterpret_cast<const float4 *>(ys + j0 + 4);
+            z[0] = y0.x, z[1] = y0.y, z[2] = y0.z, z[3] = y0.w, z[4] = y1.x, z[5] = y1.y, z[6] = y1.z, z[7] = y1.w;
+        }
+        // dot4 of the first half's entries of rows r and c (c >= 4)
+        auto lo4 = [&](const float(&a)[P], const float(&b)[P]) { return dot4(a[0], b[0], a[1], b[1], a[2], b[2], a[3], b[3]); };
+#pragma unroll
+        for (int r = 0; r < P; r++) {
+#pragma unroll
+            for (int c = 0; c < r; c++) {
+                float s = l[r][c];
+                if (c >= 4) s -= lo4(l[r], l[c]);
+#pragma unroll
+                for (int m = c & 4; m < c; m++) s -= l[r][m] * l[c][m];
+                l[r][c] = s * inv[c];
+            }
+            float d = l[r][r];
+            if (r >= 4) d -= lo4(l[r], l[r]);
+#pragma unroll
+            for (int m = r & 4; m < r; m++) d -= l[r][m] * l[r][m];
+            bad |= !(d > 0.0f);  // NaN included
+            inv[r] = rsqrt_nr(d);
+            l[r][r] = d * inv[r];
+            // forward substitution for the pivot rows
+            float s = z[r];
+            if (r >= 4) s -= lo4(l[r], z);
+#pragma unroll
+            for (int m = r & 4; m < r; m++) s -= l[r][m] * z[m];
+            z[r] = s * inv[r];
+        }
+        __syncwarp();  // all reads of the diagonal block / pivot rhs precede their overwrite
+
+        float x[RPT][P];
+#pragma unroll
+        for (int q = 0; q < RPT; q++) {
+            const int i = tid + q * 32;
+#pragma unroll
+            for (int c = 0; c < P; c++) x[q][c] = 0.0f;
+            if (i < j0) continue;
+            const float4 a0 = *reinterpret_cast<const float4 *>(As + i * LDA + j0);
+            const float4 a1 = *reinterpret_cast<const float4 *>(As + i * LDA + j0 + 4);
+            const float av[P] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+#pragma unroll
+            for (int c = 0; c < P; c++) {
+                float s = av[c];
+                if (c >= 4) s -= lo4(x[q], l[c]);
+#pragma unroll
+                for (int m = c & 4; m < c; m++) s -= x[q][m] * l[c][m];
+                x[q][c] = s * inv[c];
+            }
+            if (i < j0 + P) {
+                const int r = i - j0;
+                float zr = z[0], ir = inv[0];
+#pragma unroll
+                for (int c = 1; c < P; c++) {
+                    if (c == r) zr = z[c], ir = inv[c];
+                    if (c > r) x[q][c] = 0.0f;
+                }
+                yv[q] = zr;
+                dinv[i] = ir;
+            } else {
+                yv[q] -= lo4(x[q], z);
+                yv[q] -= dot4(x[q][4], z[4], x[q][5], z[5], x[q][6], z[6], x[q][7], z[7]);
+                if (i < j0 + 2 * P) ys[i] = yv[q];  // pivot rows of the next panel
+            }
+            *reinterpret_cast<float4 *>(As + i * LDA + j0) = make_float4(x[q][0], x[q][1], x[q][2], x[q][3]);
+            *reinterpret_cast<float4 *>(As + i * LDA + j0 + 4) = make_float4(x[q][4], x[q][5], x[q][6], x[q][7]);
+        }
+        __syncwarp();
+        // Trailing update A[i][cc..cc+7] -= L[i][j0..j0+7] . L[cc..cc+7][j0..j0+7]^T for every row i and every
+        // 8-column tile right of the panel, one 4-column half of the panel after the other.  Rows above a tile
+        // (i < cc) only touch the upper triangle, which is never read, so the update is applied without a
+        // per-lane branch.
+#pragma unroll 2
+        for (int cc = j0 + P; cc < KP; cc += P) {
+            float4 L[P][2];
+#pragma unroll
+            for (int c = 0; c < P; c++) {
+                L[c][0] = *reinterpret_cast<const float4 *>(As + (cc + c) * LDA + j0);
+                L[c][1] = *reinterpret_cast<const float4 *>(As + (cc + c) * LDA + j0 + 4);
+            }
+#pragma unroll
+            for (int q = 0; q < RPT; q++) {
+                if (q * 32 + 31 < cc) continue;  // this whole row group is above the tile (uniform)
+                const int i = tid + q * 32;
+                const float *xq = x[q];
+                auto upd = [&](float a, const float4(&lc)[2]) {
+                    a -= dot4(xq[0], lc[0].x, xq[1], lc[0].y, xq[2], lc[0].z, xq[3], lc[0].w);
+                    a -= dot4(xq[4], lc[1].x, xq[5], lc[1].y, xq[6], lc[1].z, xq[7], lc[1].w);
+                    return a;
+                };
+                float4 a0 = *reinterpret_cast<float4 *>(As + i * LDA + cc);
+                float4 a1 = *reinterpret_cast<float4 *>(As + i * LDA + cc + 4);
+                a0.x = upd(a0.x, L[0]), a0.y = upd(a0.y, L[1]), a0.z = upd(a0.z, L[2]), a0.w = upd(a0.w, L[3]);
+                a1.x = upd(a1.x, L[4]), a1.y = upd(a1.y, L[5]), a1.z = upd(a1.z, L[6]), a1.w = upd(a1.w, L[7]);
+                *reinterpret_cast<float4 *>(As + i * LDA + cc) = a0;
+                *reinterpret_cast<float4 *>(As + i * LDA + cc + 4) = a1;
+            }
+        }
+        __syncwarp();
+    }
+
+    // back substitution L^T x = z, eight unknowns at a time from the bottom (as two steps of four); yv holds z
+#pragma unroll
+    for (int q = 0; q < RPT; q++) {
+        const int i = tid + q * 32;
+        if (i >= KP - P) ys[i] = yv[q];
+    }
+    __syncwarp();
+    for (int j0 = KP - P; j0 >= 0; j0 -= P) {
+        float l[P][P], xs[P], di[P];
+#pragma unroll
+        for (int r = 1; r < P; r++)
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                if (4 * h >= r) continue;
+                const float4 v = *reinterpret_cast<const float4 *>(As + (j0 + r) * LDA + j0 + 4 * h);
+                l[r][4 * h] = v.x, l[r][4 * h + 1] = v.y, l[r][4 * h + 2] = v.z, l[r][4 * h + 3] = v.w;
+            }
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const float4 y = *reinterpret_cast<const float4 *>(ys + j0 + 4 * h);
+            const float4 d = *reinterpret_cast<const float4 *>(dinv + j0 + 4 * h);
+            xs[4 * h] = y.x, xs[4 * h + 1] = y.y, xs[4 * h + 2] = y.z, xs[4 * h + 3] = y.w;
+            di[4 * h] = d.x, di[4 * h + 1] = d.y, di[4 * h + 2] = d.z, di[4 * h + 3] = d.w;
+        }
+        // the lower four unknowns, then their contribution to the upper four, then those
+#pragma unroll
+        for (int h = 1; h >= 0; h--) {
+#pragma unroll
+            for (int r = 4 * h + 3; r >= 4 * h; r--) {
+                float s = xs[r];
+#pragma unroll
+                for (int m = r + 1; m < 4 * h + 4; m++) s -= l[m][r] * xs[m];
+                xs[r] = s * di[r];
+            }
+            if (h == 1) {
+#pragma unroll
+                for (int r = 0; r < 4; r++) xs[r] -= dot4(l[4][r], xs[4], l[5][r], xs[5], l[6][r], xs[6], l[7][r], xs[7]);
+            }
+        }
+        __syncwarp();
+#pragma unroll
+        for (int q = 0; q < RPT; q++) {
+            const int i = tid + q * 32;
+            if (i < j0) {
+                const float *col = As + j0 * LDA + i;  // column i of rows j0..j0+7
+                yv[q] -= dot4(col[4 * LDA], xs[4], col[5 * LDA], xs[5], col[6 * LDA], xs[6], col[7 * LDA], xs[7]);
+                yv[q] -= dot4(col[0], xs[0], col[LDA], xs[1], col[2 * LDA], xs[2], col[3 * LDA], xs[3]);
+                if (i >= j0 - P) ys[i] = yv[q];  // pivot rows of the next (upper) panel
+            } else if (i < j0 + P) {
+                const int r = i - j0;
+                float v = xs[0];
+#pragma unroll
+                for (int c = 1; c < P; c++)
+                    if (c == r) v = xs[c];
+                yv[q] = v;
+            }
+        }
+        __syncwarp();
+    }
+#pragma unroll
+    for (int q = 0; q < RPT; q++) ys[tid + q * 32] = yv[q];
+    __syncwarp();
+    return bad;
+}
+
 // Solve A x = y for a KP x KP SPD matrix held row-major in shared memory with
 // row stride KP+4 (lower triangle used), rhs in ys, scratch dinv[KP].  Executed
-// by NW warps together (NW == 1: one warp, only __syncwarp).  Thread t owns rows
-// t + q*32*NW and keeps their right-hand-side entries in registers.  On return
-// ys holds x; the result is true when a pivot was not positive (LAPACK info != 0).
+// by NW warps together.  Thread t owns rows t + q*32*NW and keeps their
+// right-hand-side entries in registers.  On return ys holds x; the result is
+// true when a pivot was not positive (LAPACK info != 0).  Only the lower
+// triangle and the diagonal 16x16 blocks are read.
 //
-// Right-looking factorisation with 4-column panels: every thread factors the 4x4
-// diagonal block redundantly from broadcast reads, solves the panel entries of its
-// own rows, applies the panel to its right-hand side (the forward substitution is
+// NW == 1 runs chol_solve_warp.  Several warps (KP = 128): right-looking
+// factorisation with 4-column panels: every thread factors the 4x4 diagonal
+// block redundantly from broadcast reads, solves the panel entries of its own
+// rows, applies the panel to its right-hand side (the forward substitution is
 // fused into the factorisation), then updates the trailing matrix in 4x4 tiles.
 // The back substitution L^T x = z runs panel by panel from the bottom.
 template <int KP, int NW>
 __device__ __forceinline__ bool chol_solve(float *As, float *ys, float *dinv, const int tid)
 {
+    if constexpr (NW == 1) return chol_solve_warp<KP>(As, ys, dinv, tid);
     constexpr int NT = NW * 32;
     constexpr int LDA = KP + 4;
     constexpr int RPT = KP / NT;

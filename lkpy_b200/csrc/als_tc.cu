@@ -106,6 +106,10 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
     using T = TcCfg<KP, ET, WEIGHTED>;
     constexpr int NW = C::NW, NT = C::NT, LDA = C::LDA, SROW = T::SROW, NS = T::NSTAGE;
     constexpr bool IMPLICIT = MODE == LK_ALS_IMPLICIT;
+    // k = 64, bf16 rows, uniform confidence v: every row's right-hand-side weight is the same v + 1, so the
+    // loop over the rows needs no shuffle of the values, and lane l accumulates features 2 l and 2 l + 1 from
+    // one 32-bit load per row
+    constexpr bool RHS_PAIR = T::BF16MMA && IMPLICIT && KP == 64;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     ET *stage0 = reinterpret_cast<ET *>(smem_raw);
     float *As = reinterpret_cast<float *>(smem_raw);
@@ -152,9 +156,7 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
         __syncthreads();
         if (ci >= a.n_chunks) break;
         const int4 c0 = __ldg(reinterpret_cast<const int4 *>(a.d_chunks) + 2 * ci);
-        const int4 c1 = __ldg(reinterpret_cast<const int4 *>(a.d_chunks) + 2 * ci + 1);
         const int row = c0.x, begin = c0.y, len = c0.z, nparts = c0.w;
-        const int slot0 = c1.x, part = c1.y, split_idx = c1.z;
         float *thisrow = a.d_this + (size_t)row * k;
 
         if (len == 0 && nparts == 1) {
@@ -178,17 +180,22 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
         float yacc[C::YPT];
 #pragma unroll
         for (int q = 0; q < C::YPT; q++) yacc[q] = 0.0f;
+        float ypair[2] = {0.0f, 0.0f};  // RHS_PAIR: y[2 lane], y[2 lane + 1]
+        const float wu = a.uniform_val + 1.0f;
 
         const int n_it = (len + 31) >> 5;
         const int32_t *cols = a.d_cols + begin;
         const float *vals = a.d_vals + begin;
         // column index of this lane's row in stages it .. it + NS (cq[0]: stage it), value in stages it, it + 1
+        // (RHS_PAIR reads no values: they all equal the uniform confidence)
         int cq[NS + 1];
-        float vq[2];
+        float vq[2] = {0.f, 0.f};
 #pragma unroll
         for (int j = 0; j < NS; j++) cq[j] = j * 32 + lane < len ? __ldg(cols + j * 32 + lane) : -1;
+        if constexpr (!RHS_PAIR) {
 #pragma unroll
-        for (int j = 0; j < 2; j++) vq[j] = j * 32 + lane < len ? __ldg(vals + j * 32 + lane) : 0.f;
+            for (int j = 0; j < 2; j++) vq[j] = j * 32 + lane < len ? __ldg(vals + j * 32 + lane) : 0.f;
+        }
 
         auto issue = [&](int it, int c) {
             const int s = it % NS;
@@ -209,19 +216,27 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
             const int nxt = (it + NS) * 32 + lane;
             cq[NS] = nxt < len ? __ldg(cols + nxt) : -1;
             const int vnxt = (it + 2) * 32 + lane;
-            const float vn = vnxt < len ? __ldg(vals + vnxt) : 0.f;
+            const float vn = !RHS_PAIR && vnxt < len ? __ldg(vals + vnxt) : 0.f;
             if (it + NS - 1 < n_it) issue(it + NS - 1, cq[NS - 1]);
             mbar_wait(&bars[s], (phases >> s) & 1u);
             phases ^= (1u << s);
             const int nrows = min(32, len - it * 32);
             const ET *st = stage0 + s * T::STAGE_ELTS;
 
-            // right-hand side, as the SIMT kernel computes it
-            for (int r = 0; r < nrows; r++) {
-                const float v = __shfl_sync(FULL, vq[0], r);
-                const float w = IMPLICIT ? v + 1.0f : v;
+            // right-hand side, as the SIMT kernel computes it: y = fma(o_r, w_r, y) over the rows in order
+            if constexpr (RHS_PAIR) {
+                for (int r = 0; r < nrows; r++) {
+                    const uint32_t u = *reinterpret_cast<const uint32_t *>(st + r * SROW + 2 * lane);
+                    ypair[0] = fmaf(__uint_as_float(u << 16), wu, ypair[0]);
+                    ypair[1] = fmaf(__uint_as_float(u & 0xffff0000u), wu, ypair[1]);
+                }
+            } else {
+                for (int r = 0; r < nrows; r++) {
+                    const float v = __shfl_sync(FULL, vq[0], r);
+                    const float w = IMPLICIT ? v + 1.0f : v;
 #pragma unroll
-                for (int q = 0; q < C::YPT; q++) yacc[q] = fmaf(tc_elt(st[r * SROW + tid + q * NT]), w, yacc[q]);
+                    for (int q = 0; q < C::YPT; q++) yacc[q] = fmaf(tc_elt(st[r * SROW + tid + q * NT]), w, yacc[q]);
+                }
             }
 
             if constexpr (T::BF16MMA) {
@@ -291,6 +306,16 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
             vq[1] = vn;
         }
 
+        if constexpr (RHS_PAIR) {
+            // to the general layout: lane l holds y[l + 32 q], which lane (l >> 1) + 16 q holds in ypair[l & 1]
+#pragma unroll
+            for (int q = 0; q < C::YPT; q++) {
+                const float y0 = __shfl_sync(FULL, ypair[0], (lane >> 1) + 16 * q);
+                const float y1 = __shfl_sync(FULL, ypair[1], (lane >> 1) + 16 * q);
+                yacc[q] = (lane & 1) ? y1 : y0;
+            }
+        }
+
         // accumulator (mi, nj, r) holds G[qi + 16 mi + g + 8 (r / 2)][qj + 8 nj + 2 t + r % 2]
         if (scale != 1.0f) {
 #pragma unroll
@@ -304,6 +329,9 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
 
         // ---- rows split over several chunks: park the partial, last part reduces
         if (nparts > 1) {
+            // read here rather than with c0, so that it is not held through the Gram
+            const int4 c1 = __ldg(reinterpret_cast<const int4 *>(a.d_chunks) + 2 * ci + 1);
+            const int slot0 = c1.x, part = c1.y, split_idx = c1.z;
             float *slot = a.d_partials + (size_t)(slot0 + part) * C::SLOTF;
 #pragma unroll
             for (int mi = 0; mi < 4; mi++)
