@@ -28,6 +28,8 @@
  *   FlexMFScorerBase.__call__ + TopNRanker        src/lenskit/flexmf/_base.py:117-157 lk_als_recommend_batch (biases as offsets)
  *   TruncatedSVD sparse products (SciPy, host)    src/lenskit/sklearn/svd.py         lk_spmm
  *   BiasedSVDScorer.__call__ + TopNRanker         src/lenskit/sklearn/svd.py         lk_als_recommend_batch (biases as offsets)
+ *   NMFScorer.train (scikit-learn _update_cdnmf_fast) src/lenskit/sklearn/nmf.py     lk_nmf_cd_sweep + lk_f32_seq_sum (+ lk_spmm)
+ *   NMFScorer.__call__ + TopNRanker               src/lenskit/sklearn/nmf.py         lk_als_recommend_batch
  *
  * Conventions
  *   - plain C: pointers and sizes only; no C++/torch types cross this boundary;
@@ -774,6 +776,40 @@ typedef struct lk_spmm_args {
 } lk_spmm_args;
 
 LK_API int lk_spmm(const lk_spmm_args *args, void *stream);
+
+/* ------------------------------------------------------------------------
+ * NMF coordinate descent (nmf.cu), scikit-learn's solver="cd" behind NMFScorer (src/lenskit/sklearn/nmf.py).
+ *
+ * lk_nmf_cd_sweep is one `_update_cdnmf_fast(W, HHt, XHt, arange(k))` bit for bit: for each component t in
+ * order and each row i,
+ *     grad = -XHt[i][t];  for r in 0..k-1: grad = grad + HHt[t][r] * W[i][r]      (product and sum each rounded)
+ *     pg = W[i][t] == 0 ? min(0, grad) : grad;   d_pg[t][i] = |pg|
+ *     if HHt[t][t] != 0: W[i][t] = max(W[i][t] - grad / HHt[t][t], 0)
+ * W is updated in place.  The sweep's violation is the left-to-right f32 sum of d_pg in its [k][n] order, which
+ * lk_f32_seq_sum computes.  k in 1..128, else LK_ERR_UNSUPPORTED.
+ * ---------------------------------------------------------------------- */
+typedef struct lk_nmf_cd_sweep_args {
+    int32_t n;                         /* rows of W */
+    int32_t k;                         /* components, 1..128 */
+    float *d_w;                        /* W [n][k] row-major, in place */
+    const float *d_hht;                /* HHt [k][k] row-major, l2 already on the diagonal */
+    const float *d_xht;                /* XHt [n][k] row-major, l1 already subtracted */
+    float *d_pg;                       /* [k][n] out: |projected gradient|, component-major */
+} lk_nmf_cd_sweep_args;
+
+LK_API int lk_nmf_cd_sweep(const lk_nmf_cd_sweep_args *args, void *stream);
+
+/* lk_f32_seq_sum: `count` (1..8) independent sums, run concurrently, one CTA each.  Sum i is
+ *     s = +0.0f;  for j in 0..n-1: s = s + x[j]      (each addition rounded to nearest even)
+ * over non-negative values (inf and NaN propagate as in that loop), which is np.cumsum(x, dtype=float32)[-1]
+ * bit for bit, written to *d_out.  It needs no workspace: each sum is scanned one tile at a time within its CTA. */
+typedef struct lk_f32_seq_sum_args {
+    int64_t n;
+    const float *d_x;                  /* [n] */
+    float *d_out;                      /* [1] */
+} lk_f32_seq_sum_args;
+
+LK_API int lk_f32_seq_sum(const lk_f32_seq_sum_args *sums, int32_t count, void *stream);
 
 #ifdef __cplusplus
 }

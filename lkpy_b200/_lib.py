@@ -381,6 +381,25 @@ class LkSpmmArgs(C.Structure):
     ]
 
 
+class LkNmfCdSweepArgs(C.Structure):
+    _fields_ = [
+        ("n", C.c_int32),
+        ("k", C.c_int32),
+        ("d_w", vp),
+        ("d_hht", vp),
+        ("d_xht", vp),
+        ("d_pg", vp),
+    ]
+
+
+class LkF32SeqSumArgs(C.Structure):
+    _fields_ = [
+        ("n", C.c_int64),
+        ("d_x", vp),
+        ("d_out", vp),
+    ]
+
+
 #: every symbol ``include/lkpy_b200.h`` declares: name -> (restype, argtypes)
 SYMBOLS: dict[str, tuple] = {
     "lk_version": (C.c_int, []),
@@ -431,6 +450,8 @@ SYMBOLS: dict[str, tuple] = {
     "lk_flexmf_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, i64p]),
     "lk_flexmf_step": (C.c_int, [C.POINTER(LkFlexmfStepArgs), vp]),
     "lk_spmm": (C.c_int, [C.POINTER(LkSpmmArgs), vp]),
+    "lk_nmf_cd_sweep": (C.c_int, [C.POINTER(LkNmfCdSweepArgs), vp]),
+    "lk_f32_seq_sum": (C.c_int, [C.POINTER(LkF32SeqSumArgs), C.c_int32, vp]),
 }
 
 _lib = None

@@ -19,8 +19,8 @@ import torch
 from . import _lib
 from ._lib import (
     LkAlsArgs, LkAlsRecArgs, LkAssocScoreArgs, LkCoocArgs, LkEaseScoreArgs, LkFlexmfSampleArgs, LkFlexmfStepArgs,
-    LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkSlimArgs, LkSpmmArgs, LkUknnSearchArgs, check, lib, ptr,
-    stream_ptr,
+    LkF32SeqSumArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkNmfCdSweepArgs, LkSlimArgs, LkSpmmArgs,
+    LkUknnSearchArgs, check, lib, ptr, stream_ptr,
 )  # fmt: skip
 from .data import InteractionCSR
 
@@ -1425,7 +1425,30 @@ def _prefer_cusolver():
         torch.backends.cuda.preferred_linalg_library(before)
 
 
-def _randomized_svd(x: SvdOperand, q0: torch.Tensor, k: int, n_iter: int, stage):
+def randomized_svd_usv(x: SvdOperand, q0: torch.Tensor, k: int, n_iter: int, stage=None):
+    """
+    scikit-learn's ``_randomized_svd(X, k, n_iter=n_iter)`` with ``flip_sign=True`` on the device, as NMF's
+    ``nndsvda`` initialisation calls it: returns ``(U [n_rows, k], s [k], Vt [k, n_cols])`` of the f32 matrix X.
+    Each component's sign makes the entry of largest magnitude (the first such) of X's left singular vector
+    positive: ``svd_flip(U, Vt)`` without transposition, ``svd_flip(..., u_based_decision=False)`` on Xᵀ's factors
+    with it.  ``q0`` and the products, LU, QR and SVD are as in :func:`randomized_svd`.
+    """
+    stage = stage or (lambda _name: contextlib.nullcontext())
+    with _prefer_cusolver():
+        transpose, Q, Uh, s, Vt = _randomized_basis(x, q0, n_iter, stage)
+        with stage("svd"):
+            left = (Q @ Uh[:, :k], Vt[:k].T)  # M's left singular vectors, and its right ones
+            u, vt = (left[1], left[0].T) if transpose else (left[0], left[1].T)
+        with stage("flip"):
+            pick = u.abs().argmax(dim=0, keepdim=True)
+            sign = torch.sign(torch.gather(u, 0, pick))
+            u, vt = u * sign, vt * sign.T
+    return u.contiguous(), s[:k].contiguous(), vt.contiguous()
+
+
+def _randomized_basis(x: SvdOperand, q0: torch.Tensor, n_iter: int, stage):
+    """The range finder and the small SVD of ``_randomized_svd``: ``(transpose, Q, Uh, s, Vt)`` with M = Xᵀ when
+    ``transpose``, else X, and ``Q.T @ M = Uh diag(s) Vt``."""
     transpose = x.shape[0] < x.shape[1]
     M = x.T if transpose else x
     Q = q0
@@ -1445,12 +1468,132 @@ def _randomized_svd(x: SvdOperand, q0: torch.Tensor, k: int, n_iter: int, stage)
         B = M.tmul(Q).T  # Q.T @ M, which SciPy computes as (Mᵀ @ Q).T
     with stage("svd"):
         Uh, s, Vt = torch.linalg.svd(B, full_matrices=False)
+    return transpose, Q, Uh, s, Vt
+
+
+def _randomized_svd(x: SvdOperand, q0: torch.Tensor, k: int, n_iter: int, stage):
+    transpose, Q, Uh, s, Vt = _randomized_basis(x, q0, n_iter, stage)
+    with stage("svd"):
         vt = (Q @ Uh[:, :k]).T if transpose else Vt[:k]  # the right singular vectors of X
     with stage("flip"):
         # svd_flip(u_based_decision=False): each row's sign is that of its first entry of largest magnitude
         pick = vt.abs().argmax(dim=1, keepdim=True)
         vt = vt * torch.sign(torch.gather(vt, 1, pick))
     return vt.contiguous(), s[:k].contiguous()
+
+
+# ---------------------------------------------------------------------------
+# NMF coordinate descent (NMFScorer)
+# ---------------------------------------------------------------------------
+
+
+def nmf_gram(q: torch.Tensor) -> torch.Tensor:
+    """``Q.T @ Q`` [k, k]: in f64, rounded once to f32 (scikit-learn's is an f32 sgemm; see DESIGN.md §4.17)."""
+    q = q.double()
+    return (q.T @ q).float().contiguous()
+
+
+def nmf_cd_sweep(w: torch.Tensor, hht: torch.Tensor, xht: torch.Tensor, pg: torch.Tensor) -> None:
+    """One ``_update_cdnmf_fast(W, HHt, XHt, arange(k))`` (``lk_nmf_cd_sweep``): W [n, k] updated in place, every
+    |projected gradient| written to ``pg`` [k, n]."""
+    n, k = w.shape
+    for t, shape in ((w, (n, k)), (hht, (k, k)), (xht, (n, k)), (pg, (k, n))):
+        if t.dtype != torch.float32 or tuple(t.shape) != shape or not t.is_contiguous():
+            raise ValueError(f"NMF sweep operands must be contiguous f32 of shapes W [n, k], HHt [k, k], XHt [n, k], "
+                             f"pg [k, n]; got {tuple(t.shape)} for {shape}")  # fmt: skip
+    a = LkNmfCdSweepArgs()
+    a.n, a.k = n, k
+    a.d_w, a.d_hht, a.d_xht, a.d_pg = ptr(w), ptr(hht), ptr(xht), ptr(pg)
+    check(lib().lk_nmf_cd_sweep(C.byref(a), stream_ptr()), "lk_nmf_cd_sweep")
+
+
+def f32_seq_sum(xs: list[torch.Tensor]) -> torch.Tensor:
+    """The left-to-right f32 sums ``np.cumsum(x, dtype=float32)[-1]`` of the non-negative f32 tensors ``xs`` (at
+    most 8), computed concurrently by ``lk_f32_seq_sum``: a device tensor [len(xs)]."""
+    out = torch.empty(len(xs), dtype=torch.float32, device=xs[0].device)
+    sums = (LkF32SeqSumArgs * len(xs))()
+    for i, x in enumerate(xs):
+        if x.dtype != torch.float32 or not x.is_contiguous():
+            raise ValueError("f32_seq_sum needs contiguous f32 tensors")
+        sums[i].n, sums[i].d_x, sums[i].d_out = x.numel(), ptr(x), out.data_ptr() + 4 * i
+    check(lib().lk_f32_seq_sum(sums, len(xs), stream_ptr()), "lk_f32_seq_sum")
+    return out
+
+
+@dataclass
+class NmfDescent:
+    """
+    ``_fit_coordinate_descent`` on the device for the indicator matrix X (both orientations in ``x``): W [n_rows, k]
+    and Ht [n_cols, k] in HBM, updated in place by :meth:`iteration`, and the two |pg| buffers of the sweeps.
+    """
+
+    x: SvdOperand
+    W: torch.Tensor
+    Ht: torch.Tensor
+    l1_W: float = 0.0
+    l1_H: float = 0.0
+    l2_W: float = 0.0
+    l2_H: float = 0.0
+    pg_W: torch.Tensor = field(init=False)
+    pg_H: torch.Tensor = field(init=False)
+
+    def __post_init__(self):
+        k = self.W.shape[1]
+        self.pg_W = torch.empty((k, self.W.shape[0]), dtype=torch.float32, device=self.W.device)
+        self.pg_H = torch.empty((k, self.Ht.shape[0]), dtype=torch.float32, device=self.W.device)
+
+    def half(self, product, w, ht, l1: float, l2: float, pg, stage) -> None:
+        """``_update_coordinate_descent(X, W, Ht, l1, l2)`` without its violation sum: Gram, product, sweep."""
+        with stage("gram"):
+            hht = nmf_gram(ht)
+            if l2 != 0.0:
+                hht.diagonal().add_(l2)  # in f32, as NumPy adds a Python float to an f32 array
+        with stage("spmm"):
+            xht = product(ht)
+            if l1 != 0.0:
+                xht.sub_(l1)
+        with stage("sweep"):
+            nmf_cd_sweep(w, hht, xht, pg)
+
+    def iteration(self, stage=None) -> tuple[float, float]:
+        """One iteration: the W sweep, the H sweep, then both violations (f32, returned as Python floats)."""
+        stage = stage or (lambda _name: contextlib.nullcontext())
+        self.half(self.x.mul, self.W, self.Ht, self.l1_W, self.l2_W, self.pg_W, stage)
+        self.half(self.x.tmul, self.Ht, self.W, self.l1_H, self.l2_H, self.pg_H, stage)
+        with stage("sum"):
+            v = f32_seq_sum([self.pg_W.view(-1), self.pg_H.view(-1)]).cpu().numpy()
+        return float(v[0]), float(v[1])
+
+
+def nndsvd(u: torch.Tensor, s: torch.Tensor, vt: torch.Tensor, fill: float) -> tuple[torch.Tensor, torch.Tensor]:
+    """
+    The NNDSVD step of scikit-learn's ``_initialize_nmf`` (``init="nndsvda"``) on the device: W [n_rows, k] and
+    H [k, n_cols] from X's SVD, entries below 1e-6 set to 0 and then every 0 to ``fill`` (``X.mean()``).  The norms
+    are square roots of f32 sums of squares taken in f64, and the products of norms are f64, as there; f32 sums in
+    another order than BLAS's, so W and H agree with scikit-learn's to rounding.
+    """
+    W = torch.zeros_like(u)
+    H = torch.zeros_like(vt)
+    W[:, 0] = torch.sqrt(s[0]) * u[:, 0].abs()
+    H[0, :] = torch.sqrt(s[0]) * vt[0, :].abs()
+    if u.shape[1] > 1:
+        x, y = u[:, 1:], vt[1:, :].T  # one column per component
+        xp, yp = x.clamp(min=0), y.clamp(min=0)
+        xn, yn = x.clamp(max=0).abs(), y.clamp(max=0).abs()
+        nrm = lambda a: (a * a).sum(dim=0).double().sqrt()  # noqa: E731
+        xpn, ypn, xnn, ynn = nrm(xp), nrm(yp), nrm(xn), nrm(yn)
+        mp, mn = xpn * ypn, xnn * ynn
+        pos = mp > mn
+        uu = torch.where(pos, xp / xpn.float(), xn / xnn.float())
+        vv = torch.where(pos, yp / ypn.float(), yn / ynn.float())
+        lbd = torch.sqrt(s[1:] * torch.where(pos, mp, mn).float())
+        W[:, 1:] = lbd * uu
+        H[1:, :] = (lbd * vv).T
+    W[W < 1e-6] = 0
+    H[H < 1e-6] = 0
+    W[W == 0] = fill
+    H[H == 0] = fill
+    return W.contiguous(), H.contiguous()
 
 
 # ---------------------------------------------------------------------------
