@@ -30,6 +30,8 @@
  *   BiasedSVDScorer.__call__ + TopNRanker         src/lenskit/sklearn/svd.py         lk_als_recommend_batch (biases as offsets)
  *   NMFScorer.train (scikit-learn _update_cdnmf_fast) src/lenskit/sklearn/nmf.py     lk_nmf_cd_sweep + lk_f32_seq_sum (+ lk_spmm)
  *   NMFScorer.__call__ + TopNRanker               src/lenskit/sklearn/nmf.py         lk_als_recommend_batch
+ *   BiasModel.learn (NumPy, host)                 src/lenskit/basic/bias.py:84-150   lk_bias_learn
+ *   BiasScorer / PopScorer __call__ + TopNRanker  src/lenskit/basic/bias.py, popularity.py lk_offset_score_batch
  *
  * Conventions
  *   - plain C: pointers and sizes only; no C++/torch types cross this boundary;
@@ -810,6 +812,64 @@ typedef struct lk_f32_seq_sum_args {
 } lk_f32_seq_sum_args;
 
 LK_API int lk_f32_seq_sum(const lk_f32_seq_sum_args *sums, int32_t count, void *stream);
+
+/* ------------------------------------------------------------------------
+ * Bias model and offset scoring (basic.cu), behind BiasScorer and PopScorer (src/lenskit/basic/bias.py,
+ * popularity.py).
+ *
+ * lk_bias_learn is BiasModel.learn (bias.py:84-150) bit for bit, on ratings r in (user, item) COO order:
+ *     g = f32(f64(+0.0f + pairwise(r)) / nnz)          np.mean of the f32 ratings (NumPy's pairwise order)
+ *     c = r - g                                        f32, or f64(r) - g with centered_f64
+ *   item pass:  cnt = d_item; s = 0.0; for each rating of the item by ascending user: cnt += 1.0; s += f64(c)
+ *               ib[i] = cnt > 0 ? f32(s / cnt) : 0;  then c = c - ib[item]   (in c's type)
+ *   user pass:  the same over each user's ratings in COO order, ub[u] = cnt > 0 ? f32(s / cnt) : 0
+ * Every add is a rounded f64 add in that order (np.add.at); the counts too, unless d is an integer, when they are
+ * exactly d + n.  A pass left out (d_item_bias or d_user_bias NULL) is skipped; without the item pass the user
+ * pass sums r - g.  The mean is a parallel walk of the pairwise tree; each entity's sum is one warp, with entities
+ * handed out in the caller's order (longest first keeps the longest chains from starting last).
+ * ---------------------------------------------------------------------- */
+typedef struct lk_bias_learn_args {
+    int64_t nnz;                       /* 1 .. 2^31 - 1 */
+    int32_t n_users, n_items;
+    const float *d_ratings;            /* [nnz] COO order, sorted by (user, item) */
+    const int32_t *d_items;            /* [nnz] COO item numbers */
+    const int32_t *d_user_indptr;      /* [n_users + 1] offsets of each user's ratings in COO order */
+    const int32_t *d_item_indptr;      /* [n_items + 1] offsets into d_item_ratings */
+    const float *d_item_ratings;       /* [nnz] the ratings item-major, ascending user within an item */
+    const int32_t *d_user_order;       /* [n_users] every user once: the order users are handed to warps */
+    const int32_t *d_item_order;       /* [n_items] every item once */
+    int32_t centered_f64;              /* 0: c in f32 (an f32 rating matrix), 1: c in f64 */
+    double damping_user, damping_item; /* >= 0 */
+    void *d_workspace;                 /* lk_bias_learn_workspace_bytes() bytes */
+    float *d_mean;                     /* [1] out: g */
+    float *d_item_bias;                /* [n_items] out, or NULL: no item pass */
+    float *d_user_bias;                /* [n_users] out, or NULL: no user pass */
+} lk_bias_learn_args;
+
+LK_API int64_t lk_bias_learn_workspace_bytes(void);
+LK_API int lk_bias_learn(const lk_bias_learn_args *args, void *stream);
+
+/*
+ * lk_offset_score_batch: s(q, i) = f32(f64(base[i]) + offset[q]) for every item i and query q (offset NULL: 0).
+ * With the offset in f64 that is NumPy's `f32 scores += f64 user bias` (computed in f64, rounded once) and, for an
+ * f32 offset, the f32 sum itself.  n == 0: score mode, d_scores [B][n_items] row-major.  n in 1..lk_topn_max():
+ * rank mode, argtopn over every item in ascending order (topn_heap.cuh's output contract), the query's exclusions
+ * (ascending within each query, in range) and NaN scores never offered.  One thread per query.
+ */
+typedef struct lk_offset_score_args {
+    int32_t n_items, n_queries;
+    const float *d_base;               /* [n_items] */
+    const double *d_offset;            /* [n_queries] or NULL */
+    int32_t n;
+    float *d_scores;                   /* score mode */
+    const int64_t *d_excl_indptr;      /* rank mode: [B + 1] or NULL */
+    const int32_t *d_excl_items;
+    int32_t *d_out_idx;                /* [B][n] */
+    float *d_out_val;                  /* [B][n] */
+    int32_t *d_out_cnt;                /* [B] */
+} lk_offset_score_args;
+
+LK_API int lk_offset_score_batch(const lk_offset_score_args *args, void *stream);
 
 #ifdef __cplusplus
 }

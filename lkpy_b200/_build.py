@@ -18,7 +18,7 @@ CSRC = Path(__file__).resolve().parent / "csrc"
 LIB = CSRC / "liblkpy_b200.so"
 SOURCES = ["capi.cu", "als_kernels.cu", "als_tc.cu", "knn_build.cu", "knn_score.cu", "knn_user.cu", "topn.cu", "prep.cu",
            "als_recommend.cu", "cooc.cu", "ease.cu", "slim.cu", "flexmf.cu",
-           "spmm.cu", "nmf.cu"]
+           "spmm.cu", "nmf.cu", "basic.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17", "--extended-lambda",
@@ -38,7 +38,7 @@ def _stale() -> bool:
         return True
     t = LIB.stat().st_mtime
     deps = [CSRC / s for s in SOURCES] + [
-        CSRC / "common.cuh", CSRC / "als_common.cuh", CSRC / "topn_heap.cuh", CSRC / "tiles.cuh",
+        CSRC / "common.cuh", CSRC / "als_common.cuh", CSRC / "topn_heap.cuh", CSRC / "tiles.cuh", CSRC / "pairwise.cuh",
     ]  # fmt: skip
     deps.append(CSRC.parent.parent / "include" / "lkpy_b200.h")
     return any(d.stat().st_mtime > t for d in deps)

@@ -400,6 +400,44 @@ class LkF32SeqSumArgs(C.Structure):
     ]
 
 
+class LkBiasLearnArgs(C.Structure):
+    _fields_ = [
+        ("nnz", C.c_int64),
+        ("n_users", C.c_int32),
+        ("n_items", C.c_int32),
+        ("d_ratings", vp),
+        ("d_items", vp),
+        ("d_user_indptr", vp),
+        ("d_item_indptr", vp),
+        ("d_item_ratings", vp),
+        ("d_user_order", vp),
+        ("d_item_order", vp),
+        ("centered_f64", C.c_int32),
+        ("damping_user", C.c_double),
+        ("damping_item", C.c_double),
+        ("d_workspace", vp),
+        ("d_mean", vp),
+        ("d_item_bias", vp),
+        ("d_user_bias", vp),
+    ]
+
+
+class LkOffsetScoreArgs(C.Structure):
+    _fields_ = [
+        ("n_items", C.c_int32),
+        ("n_queries", C.c_int32),
+        ("d_base", vp),
+        ("d_offset", vp),
+        ("n", C.c_int32),
+        ("d_scores", vp),
+        ("d_excl_indptr", vp),
+        ("d_excl_items", vp),
+        ("d_out_idx", vp),
+        ("d_out_val", vp),
+        ("d_out_cnt", vp),
+    ]
+
+
 #: every symbol ``include/lkpy_b200.h`` declares: name -> (restype, argtypes)
 SYMBOLS: dict[str, tuple] = {
     "lk_version": (C.c_int, []),
@@ -452,6 +490,9 @@ SYMBOLS: dict[str, tuple] = {
     "lk_spmm": (C.c_int, [C.POINTER(LkSpmmArgs), vp]),
     "lk_nmf_cd_sweep": (C.c_int, [C.POINTER(LkNmfCdSweepArgs), vp]),
     "lk_f32_seq_sum": (C.c_int, [C.POINTER(LkF32SeqSumArgs), C.c_int32, vp]),
+    "lk_bias_learn_workspace_bytes": (C.c_int64, []),
+    "lk_bias_learn": (C.c_int, [C.POINTER(LkBiasLearnArgs), vp]),
+    "lk_offset_score_batch": (C.c_int, [C.POINTER(LkOffsetScoreArgs), vp]),
 }
 
 _lib = None

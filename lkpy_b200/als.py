@@ -563,28 +563,32 @@ class BiasModel:
         self.damping = damping
 
     @classmethod
-    def learn(cls, it: Interactions, damping, centered_dtype=np.float64) -> "BiasModel":
+    def learn(cls, it: Interactions, damping, centered_dtype=np.float64, entities=("user", "item")) -> "BiasModel":
         """``damping``: one float for both, a ``(user, item)`` tuple, or a dict ``{"user": ..., "item": ...}`` in
         which a missing key means 0.  ``centered_dtype`` is the type of the centred ratings, which the reference
-        takes from its rating matrix: ``np.float32`` gives its statements on an f32 matrix exactly."""
+        takes from its rating matrix: ``np.float32`` gives its statements on an f32 matrix exactly.  ``entities``
+        names the biases to learn; one left out is None."""
         if isinstance(damping, dict):
             damping = (float(damping.get("user", 0.0)), float(damping.get("item", 0.0)))
         d_user, d_item = damping if isinstance(damping, tuple) else (damping, damping)
         g = float(np.mean(it.ratings))
         centered = it.ratings.astype(centered_dtype) - g
-        counts = np.full(it.n_items, float(d_item))
-        sums = np.zeros(it.n_items)
-        np.add.at(counts, it.items, 1)
-        np.add.at(sums, it.items, centered)
-        ib = np.zeros(it.n_items, dtype=np.float32)
-        np.divide(sums, counts, out=ib, where=counts > 0, casting="unsafe")
-        centered = centered - ib[it.items]
-        counts = np.full(it.n_users, float(d_user))
-        sums = np.zeros(it.n_users)
-        np.add.at(counts, it.users, 1)
-        np.add.at(sums, it.users, centered)
-        ub = np.zeros(it.n_users, dtype=np.float32)
-        np.divide(sums, counts, out=ub, where=counts > 0, casting="unsafe")
+        ib = ub = None
+        if "item" in entities:
+            counts = np.full(it.n_items, float(d_item))
+            sums = np.zeros(it.n_items)
+            np.add.at(counts, it.items, 1)
+            np.add.at(sums, it.items, centered)
+            ib = np.zeros(it.n_items, dtype=np.float32)
+            np.divide(sums, counts, out=ib, where=counts > 0, casting="unsafe")
+            centered = centered - ib[it.items]
+        if "user" in entities:
+            counts = np.full(it.n_users, float(d_user))
+            sums = np.zeros(it.n_users)
+            np.add.at(counts, it.users, 1)
+            np.add.at(sums, it.users, centered)
+            ub = np.zeros(it.n_users, dtype=np.float32)
+            np.divide(sums, counts, out=ub, where=counts > 0, casting="unsafe")
         return cls(g, ib, ub, (d_user, d_item))
 
     def batch_offsets(self, user_nums: np.ndarray, fold_bias: np.ndarray | None):

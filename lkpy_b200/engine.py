@@ -18,9 +18,9 @@ import torch
 
 from . import _lib
 from ._lib import (
-    LkAlsArgs, LkAlsRecArgs, LkAssocScoreArgs, LkCoocArgs, LkEaseScoreArgs, LkFlexmfSampleArgs, LkFlexmfStepArgs,
-    LkF32SeqSumArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkNmfCdSweepArgs, LkSlimArgs, LkSpmmArgs,
-    LkUknnSearchArgs, check, lib, ptr, stream_ptr,
+    LkAlsArgs, LkAlsRecArgs, LkAssocScoreArgs, LkBiasLearnArgs, LkCoocArgs, LkEaseScoreArgs, LkFlexmfSampleArgs,
+    LkFlexmfStepArgs, LkF32SeqSumArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkNmfCdSweepArgs,
+    LkOffsetScoreArgs, LkSlimArgs, LkSpmmArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr,
 )  # fmt: skip
 from .data import InteractionCSR
 
@@ -1973,3 +1973,82 @@ class FlexMFState:
         perm = perm.to(self.device, torch.int64)
         ratings = None if self.ratings is None else self.ratings[perm]
         return self.train_batches(self.users[perm], self.items[perm], ratings=ratings)
+
+
+# ---------------------------------------------------------------------------
+# Bias model and offset scoring (BiasScorer, PopScorer)
+# ---------------------------------------------------------------------------
+
+
+def longest_first(indptr: torch.Tensor) -> torch.Tensor:
+    """The rows of a CSR offset array longest first (int32, ties ascending)."""
+    return torch.argsort(indptr[1:] - indptr[:-1], descending=True, stable=True).to(torch.int32)
+
+
+def bias_learn(
+    ratings: torch.Tensor, items: torch.Tensor, user_indptr: torch.Tensor, item_indptr: torch.Tensor,
+    item_ratings: torch.Tensor, damping: tuple[float, float], *, item_pass: bool = True, user_pass: bool = True,
+    centered_f64: bool = False,
+):  # fmt: skip
+    """
+    ``BiasModel.learn`` on the device (``lk_bias_learn``), bit for bit with the host statements: returns the global
+    mean (f32 [1]) and the item and user biases (f32 [n_items] and [n_users], or None for a pass left out).
+    ``ratings`` and ``items`` are the COO arrays sorted by (user, item), ``user_indptr`` their user offsets, and
+    ``item_ratings`` the ratings item-major (ascending user within an item) with offsets ``item_indptr`` (int32).
+    ``damping`` is ``(user, item)``; ``centered_f64`` centres in f64 (an f64 rating matrix) instead of f32.
+    """
+    dev = ratings.device
+    n_users, n_items = user_indptr.numel() - 1, item_indptr.numel() - 1
+    a = LkBiasLearnArgs()
+    a.nnz, a.n_users, a.n_items = ratings.numel(), n_users, n_items
+    a.d_ratings, a.d_items = ptr(ratings), ptr(items)
+    a.d_user_indptr, a.d_item_indptr, a.d_item_ratings = ptr(user_indptr), ptr(item_indptr), ptr(item_ratings)
+    user_order, item_order = longest_first(user_indptr), longest_first(item_indptr)
+    a.d_user_order, a.d_item_order = ptr(user_order), ptr(item_order)
+    a.centered_f64 = int(centered_f64)
+    a.damping_user, a.damping_item = float(damping[0]), float(damping[1])
+    ws = torch.empty(int(lib().lk_bias_learn_workspace_bytes()), dtype=torch.uint8, device=dev)
+    mean = torch.empty(1, dtype=torch.float32, device=dev)
+    ib = torch.empty(n_items, dtype=torch.float32, device=dev) if item_pass else None
+    ub = torch.empty(n_users, dtype=torch.float32, device=dev) if user_pass else None
+    a.d_workspace, a.d_mean = ptr(ws), ptr(mean)
+    a.d_item_bias, a.d_user_bias = ptr(_nonempty_or_none(ib)), ptr(_nonempty_or_none(ub))
+    check(lib().lk_bias_learn(C.byref(a), stream_ptr()), "lk_bias_learn")
+    return mean, ib, ub
+
+
+def _nonempty_or_none(t: torch.Tensor | None) -> torch.Tensor | None:
+    return None if t is None else _nonempty(t)
+
+
+def offset_scores(
+    base: torch.Tensor, n_queries: int, offset: torch.Tensor | None = None, n: int | None = None,
+    excl_indptr: torch.Tensor | None = None, excl_items: torch.Tensor | None = None,
+):  # fmt: skip
+    """
+    Scores ``s(q, i) = f32(f64(base[i]) + offset[q])`` (``lk_offset_score_batch``) for ``n_queries`` queries:
+    ``base`` f32 [n_items], ``offset`` f64 [n_queries] or None for 0.  ``n=None`` (score mode) returns
+    ``S [B, n_items]``.  An integer ``n`` (rank mode) returns ``(idx [B, n] int32, -1 padding; val [B, n] f32, NaN
+    padding; cnt [B] int32)``: ``argtopn`` over every item minus ``excl_items[excl_indptr[q]:excl_indptr[q+1]]``
+    (any order; repeats, negative and unknown numbers are ignored), ties included.
+    """
+    _lib.require_device()
+    dev = base.device
+    base = base.to(torch.float32).contiguous()
+    n_items = base.numel()
+    if n_items >= 2**31:
+        raise _lib.EngineError("offset scoring with 2**31 or more items is not supported")
+    if offset is not None:
+        offset = offset.to(device=dev, dtype=torch.float64).contiguous()
+        if offset.numel() != n_queries:
+            raise ValueError(f"offset has {offset.numel()} entries for {n_queries} queries")
+    a = LkOffsetScoreArgs()
+    a.n_items, a.n_queries = n_items, n_queries
+    a.d_base, a.d_offset = ptr(base), ptr(offset)
+    if n is None:
+        S = torch.empty((n_queries, n_items), dtype=torch.float32, device=dev)
+        a.n, a.d_scores = 0, ptr(S)
+        check(lib().lk_offset_score_batch(C.byref(a), stream_ptr()), "lk_offset_score_batch")
+        return S
+    return _rank_launch(a, lib().lk_offset_score_batch, "lk_offset_score_batch", n, n_items, n_queries, dev,
+                        excl_indptr, excl_items)  # fmt: skip

@@ -86,8 +86,9 @@ def query_bias(bias: BiasModel, items, query: RecQuery) -> float | None:
     if ratings is None:
         return None
     uoff = ratings - bias.global_bias
-    nums = query.query_items.numbers(vocabulary=items, missing="negative")
-    uoff[nums >= 0] -= bias.item_biases[nums[nums >= 0]]
+    if bias.item_biases is not None:
+        nums = query.query_items.numbers(vocabulary=items, missing="negative")
+        uoff[nums >= 0] -= bias.item_biases[nums[nums >= 0]]
     ub = np.sum(uoff) / (np.sum(np.isfinite(uoff)) + bias.damping[0])
     return 0.0 if np.isnan(ub) else float(ub)
 
