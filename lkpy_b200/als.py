@@ -22,28 +22,22 @@ from typing import Literal
 
 import numpy as np
 import torch
-from pydantic import AliasChoices, BaseModel, Field, PositiveFloat, PositiveInt, field_validator
+from pydantic import AliasChoices, BaseModel, Field, PositiveFloat, PositiveInt
 
 from . import _lib, engine
-from .components import Component, Dataset, ItemList, ModelTrainer, RecQuery, TrainingOptions, UsesTrainer
-from .data import InteractionCSR, Interactions
+from .basic import BiasModel
+from .components import Dataset, ItemList, ModelTrainer, RecQuery, TrainingOptions, UsesTrainer, _as_dataset
+from .data import InteractionCSR
+from .factors import EmbeddingSize, FactorScorer
 
 
 class ALSConfig(BaseModel):
-    embedding_size: PositiveInt = Field(default=64, validation_alias=AliasChoices("embedding_size", "features"))
+    embedding_size: EmbeddingSize = Field(default=64, validation_alias=AliasChoices("embedding_size", "features"))
     epochs: PositiveInt = 10
     regularization: PositiveFloat | tuple[PositiveFloat, PositiveFloat] = 0.1
     user_embeddings: bool | Literal["prefer"] = True
     gather_dtype: Literal["float32", "bfloat16"] = "float32"
     "Engine option: storage type of the gathered (opposite) factor rows."
-
-    @field_validator("embedding_size", mode="after")
-    @staticmethod
-    def check_embedding_size(k) -> int:
-        # engine limit (the reference has none), reported at configuration time
-        if k > engine.ALS_MAX_FEATURES:
-            raise ValueError(f"embedding_size={k} exceeds the engine limit of {engine.ALS_MAX_FEATURES}")
-        return k
 
     @property
     def user_reg(self) -> float:
@@ -65,24 +59,9 @@ class BiasedMFConfig(ALSConfig):
     damping: float | tuple[float, float] = 5.0
 
 
-def _as_dataset(data) -> Dataset:
-    if isinstance(data, Dataset):
-        return data
-    if isinstance(data, Interactions):
-        return Dataset(data)
-    raise TypeError("expected a Dataset or Interactions")
-
-
-class ALSBase(UsesTrainer, Component):
-    """``ALSBase`` (als/_common.py:113-192)."""
-
-    users = None
-    items = None
-    user_embeddings: np.ndarray | None = None
-    item_embeddings: np.ndarray | None = None
-
-    def is_trained(self) -> bool:
-        return self.item_embeddings is not None
+class ALSBase(FactorScorer, UsesTrainer):
+    """``ALSBase`` (als/_common.py:113-192): the reference's ``__call__``, and the batched path of
+    :class:`FactorScorer` with fold-in rows (``_implicit.py:77-130``) solved on the device by the training kernel."""
 
     def new_user_embedding(self, user_num, items: ItemList):  # pragma: no cover
         raise NotImplementedError
@@ -113,29 +92,8 @@ class ALSBase(UsesTrainer, Component):
         scores[mask] = self.item_embeddings[item_nums[mask], :] @ u_feat
         return self.finalize_scores(user_num, ItemList(items, scores=scores), u_offset)
 
-    # ------------------------------------------------------------------------------------------
-    # Batched inference on the device (SURVEY.md §8f N1 + N2): what the reference does one query at
-    # a time — ALSBase.__call__ (als/_common.py:133-175), fold-in (_implicit.py:77-130), TopNRanker
-    # → ItemList.top_n → argtopn (basic/topn.py:32-69, data/_items.py:942-998,
-    # src/accel/data/sorting.rs:131-170) — for a whole batch of queries with the factors resident
-    # in HBM: fold-in rows by the training kernel, scores by one library GEMM (Q · Xᵀ, item-major so
-    # the selection kernel's scan is coalesced), top-N by lk_topn_columns.
-    # ------------------------------------------------------------------------------------------
-
-    def _device_items(self) -> torch.Tensor:
-        dev = _lib.require_device()
-        cached = self.__dict__.get("_d_items_cache")
-        if cached is None or cached[0] is not self.item_embeddings:
-            t = torch.from_numpy(np.ascontiguousarray(self.item_embeddings, dtype=np.float32)).to(dev)
-            self.__dict__["_d_items_cache"] = cached = (self.item_embeddings, t)
-        return cached[1]
-
     def fold_in_batch(self, histories: list[ItemList]) -> torch.Tensor:  # pragma: no cover
         raise NotImplementedError
-
-    def batch_offsets(self, user_nums: np.ndarray, fold_bias: np.ndarray | None):
-        """(per-item offset [n_items] or None, per-query offset [B] or None) added to Q · Xᵀ."""
-        return None, None
 
     def embed_batch(self, queries) -> tuple[torch.Tensor, np.ndarray, np.ndarray, np.ndarray | None]:
         """
@@ -174,66 +132,43 @@ class ALSBase(UsesTrainer, Component):
             scorable |= known
         return X, scorable, user_nums, fold_bias
 
-    def _offsets(self, user_nums, fold_bias, dev):
-        item_off, query_off = self.batch_offsets(user_nums, fold_bias)
-        if item_off is not None:
-            item_off = torch.from_numpy(np.ascontiguousarray(item_off, dtype=np.float32)).to(dev)
-        if query_off is not None:
-            query_off = torch.from_numpy(np.ascontiguousarray(query_off, dtype=np.float32)).to(dev)
-        return item_off, query_off
-
-    def score_matrix(self, queries) -> torch.Tensor:
-        """
-        Scores of every item for every query, item-major: [n_items, B] f32, NaN columns for unscorable queries.
-        Each score is one fp32 FMA chain over ascending d, then the item offset and the query offset (f32 adds):
-        ``engine.als_recommend``'s score mode.
-        """
-        X, scorable, user_nums, fold_bias = self.embed_batch(queries)
-        item_off, query_off = self._offsets(user_nums, fold_bias, X.device)
-        S = engine.als_recommend(self._device_items(), X, None, item_off, query_off)
-        if not scorable.all():
-            S[:, torch.from_numpy(np.flatnonzero(~scorable)).to(S.device)] = float("nan")
-        return S
-
-    def recommend_batch(self, queries, n: int, *, exclude: Literal["query"] | None = None) -> list[ItemList]:
-        """
-        Top-``n`` items for every query, scored and selected on the device in one launch (``engine.als_recommend``'s
-        rank mode; memory O(B·n), no score matrix): for each query the result of the candidate selector, the
-        scores of :meth:`score_matrix` and ``TopNRanker``, bit for bit.  ``exclude="query"`` leaves the query's
-        own items (``query.query_items`` known to the model) out of the candidates, as
-        ``TrainingItemsCandidateSelector`` does; the default ``None`` ranks every item.  (The kNN scorers'
-        ``recommend_batch`` defaults to ``"query"``.)  An unscorable query gets an empty list.  The kernel sweeps
-        every item once per 64 queries, so batch widely.
-        """
-        from .batch import check_exclude, empty_list, history_csr, rank_size, ranked_lists
-
-        check_exclude(exclude)
-        queries = [RecQuery.create(q) for q in queries]
-        n_eff = rank_size(n, self.item_embeddings.shape[0])
-        if n_eff == 0:
-            return [empty_list(self.items) for _ in queries]
-        X, scorable, user_nums, fold_bias = self.embed_batch(queries)
-        at = np.flatnonzero(scorable)
-        if len(at) == 0:
-            return [empty_list(self.items) for _ in queries]
-        dev = X.device
-        item_off, query_off = self._offsets(user_nums, fold_bias, dev)
-        excl = (None, None)
-        if exclude == "query":
-            excl = history_csr([queries[b] for b in at], self.items, dev)[1:]
-        sel = torch.from_numpy(at).to(dev)
-        idx, val, cnt = engine.als_recommend(
-            self._device_items(), X[sel].contiguous(), n_eff, item_off,
-            query_off[sel] if query_off is not None else None, *excl,
-        )  # fmt: skip
-        return ranked_lists(self.items, len(queries), at, idx, val, cnt)
-
 
 def _solve_cholesky(A: np.ndarray, y: np.ndarray) -> np.ndarray:
     """``lenskit.math.solve.solve_cholesky`` (math/solve.py:17-41); host fold-in only."""
     from scipy.linalg import cho_factor, cho_solve
 
     return np.require(cho_solve(cho_factor(A), y), dtype=A.dtype)
+
+
+def _solve_fold_in(d_items: torch.Tensor, rows: list[tuple[np.ndarray, np.ndarray]], mode: int, **solve):
+    """
+    Fold-in embeddings [len(rows), k] for a batch of histories: row b of a CSR matrix holds history b's
+    ``(columns, values)``, its columns in ascending order as the CSR container wants, and ONE checked
+    ``lk_als_half_epoch`` in ``mode`` (the training kernel, fp32 item table ``d_items``) solves them all.  ``solve``
+    passes the half-epoch's ``otor`` or ``reg``.  An empty history stays 0 (``_explicit.py:134-135``).
+    """
+    cols, vals, indptr = [], [], [0]
+    for c, v in rows:
+        c = c.astype(np.int32)
+        order = np.argsort(c, kind="stable")
+        cols.append(c[order])
+        vals.append(np.asarray(v, dtype=np.float32)[order])
+        indptr.append(indptr[-1] + len(c))
+    n_items, k = d_items.shape
+    csr = InteractionCSR(
+        np.asarray(indptr, dtype=np.int32),
+        np.concatenate(cols) if cols else np.empty(0, np.int32),
+        np.concatenate(vals) if vals else np.empty(0, np.float32),
+        (len(rows), n_items),
+    )
+    plan = engine.ALSHalfPlan.create(engine.DeviceCSR.from_host(csr, d_items.device), k)
+    x = torch.zeros((len(rows), k), dtype=torch.float32, device=d_items.device)
+    plan.sqdelta.zero_()
+    plan.status.zero_()
+    engine.als_half_epoch(plan, mode, x, d_items, **solve)
+    if int(plan.status.item()):
+        raise RuntimeError("ALS solve error: a fold-in system is not positive definite")
+    return x
 
 
 class ALSTrainerBase(ModelTrainer):
@@ -455,17 +390,20 @@ class ImplicitMFScorer(ALSBase):
     def create_trainer(self, data, options):
         return ImplicitMFTrainer(self, data, options)
 
+    def _confidences(self, items: ItemList, known: np.ndarray) -> np.ndarray:
+        """The fold-in values of a history's ``known`` items: ``rating × weight`` with ``use_ratings``, else
+        ``weight`` (``_implicit.py:84-90``)."""
+        if self.config.use_ratings:
+            ratings = items.field("rating")
+            if ratings is None:
+                raise ValueError("no ratings in user items")
+            return ratings[known] * self.config.weight
+        return np.full(int(known.sum()), self.config.weight)
+
     def new_user_embedding(self, user_num, user_items: ItemList):
         ri = user_items.numbers(vocabulary=self.items, missing="negative")
         good = ri >= 0
-        if self.config.use_ratings:
-            ratings = user_items.field("rating")
-            if ratings is None:
-                raise ValueError("no ratings in user items")
-            val = ratings[good] * self.config.weight
-        else:
-            val = np.full((int(good.sum()),), self.config.weight)
-        val = val.astype(self.item_embeddings.dtype)
+        val = self._confidences(user_items, good).astype(self.item_embeddings.dtype)
         M = self.item_embeddings[ri[good], :]
         A = self._OtOr + (M.T * val) @ M
         y = M.T @ (val + 1.0)
@@ -473,46 +411,18 @@ class ImplicitMFScorer(ALSBase):
 
     def fold_in_batch(self, histories: list[ItemList]):
         """
-        ``new_user_embedding`` for a batch of histories on the device: the histories become the rows
-        of a CSR matrix and one ``lk_als_half_epoch`` (the training kernel, fp32 item table) solves
-        them all — same math as ``_train_new_row`` (``_implicit.py:109-130``).
+        ``new_user_embedding`` for a batch of histories on the device, one implicit half-epoch — same math as
+        ``_train_new_row`` (``_implicit.py:109-130``).
         """
-        dev = _lib.require_device()
-        k = self.item_embeddings.shape[1]
-        cols, vals, indptr = [], [], [0]
+        rows = []
         for h in histories:
             ri = h.numbers(vocabulary=self.items, missing="negative")
             good = ri >= 0
-            if self.config.use_ratings:
-                ratings = h.field("rating")
-                if ratings is None:
-                    raise ValueError("no ratings in user items")
-                v = np.asarray(ratings)[good] * self.config.weight
-            else:
-                v = np.full(int(good.sum()), self.config.weight)
-            c = ri[good].astype(np.int32)
-            order = np.argsort(c, kind="stable")  # the CSR container wants ascending columns
-            cols.append(c[order])
-            vals.append(np.asarray(v, dtype=np.float32)[order])
-            indptr.append(indptr[-1] + len(c))
-        csr = InteractionCSR(
-            np.asarray(indptr, dtype=np.int32),
-            np.concatenate(cols) if cols else np.empty(0, np.int32),
-            np.concatenate(vals) if vals else np.empty(0, np.float32),
-            (len(histories), self.item_embeddings.shape[0]),
-        )
-        dm = engine.DeviceCSR.from_host(csr, dev)
-        plan = engine.ALSHalfPlan.create(dm, k)
+            rows.append((ri[good], self._confidences(h, good)))
         d_items = self._device_items()
-        ws = engine.OtorWorkspace.create(k, dev)
+        ws = engine.OtorWorkspace.create(d_items.shape[1], d_items.device)
         otor = engine.als_otor(d_items, float(self.config.user_reg), ws, None)
-        x = torch.zeros((len(histories), k), dtype=torch.float32, device=dev)
-        plan.sqdelta.zero_()
-        plan.status.zero_()
-        engine.als_half_epoch(plan, _lib.LK_ALS_IMPLICIT, x, d_items, otor=otor)
-        if int(plan.status.item()):
-            raise RuntimeError("ALS solve error: a fold-in system is not positive definite")
-        return x, None
+        return _solve_fold_in(d_items, rows, _lib.LK_ALS_IMPLICIT, otor=otor), None
 
 
 class ImplicitMFTrainer(ALSTrainerBase):
@@ -553,58 +463,6 @@ class ImplicitMFTrainer(ALSTrainerBase):
 # ---------------------------------------------------------------------------
 
 
-class BiasModel:
-    """The part of ``lenskit.basic.BiasModel`` (basic/bias.py:84-150) BiasedMF needs."""
-
-    def __init__(self, global_bias, item_biases, user_biases, damping):
-        self.global_bias = global_bias
-        self.item_biases = item_biases
-        self.user_biases = user_biases
-        self.damping = damping
-
-    @classmethod
-    def learn(cls, it: Interactions, damping, centered_dtype=np.float64, entities=("user", "item")) -> "BiasModel":
-        """``damping``: one float for both, a ``(user, item)`` tuple, or a dict ``{"user": ..., "item": ...}`` in
-        which a missing key means 0.  ``centered_dtype`` is the type of the centred ratings, which the reference
-        takes from its rating matrix: ``np.float32`` gives its statements on an f32 matrix exactly.  ``entities``
-        names the biases to learn; one left out is None."""
-        if isinstance(damping, dict):
-            damping = (float(damping.get("user", 0.0)), float(damping.get("item", 0.0)))
-        d_user, d_item = damping if isinstance(damping, tuple) else (damping, damping)
-        g = float(np.mean(it.ratings))
-        centered = it.ratings.astype(centered_dtype) - g
-        ib = ub = None
-        if "item" in entities:
-            counts = np.full(it.n_items, float(d_item))
-            sums = np.zeros(it.n_items)
-            np.add.at(counts, it.items, 1)
-            np.add.at(sums, it.items, centered)
-            ib = np.zeros(it.n_items, dtype=np.float32)
-            np.divide(sums, counts, out=ib, where=counts > 0, casting="unsafe")
-            centered = centered - ib[it.items]
-        if "user" in entities:
-            counts = np.full(it.n_users, float(d_user))
-            sums = np.zeros(it.n_users)
-            np.add.at(counts, it.users, 1)
-            np.add.at(sums, it.users, centered)
-            ub = np.zeros(it.n_users, dtype=np.float32)
-            np.divide(sums, counts, out=ub, where=counts > 0, casting="unsafe")
-        return cls(g, ib, ub, (d_user, d_item))
-
-    def batch_offsets(self, user_nums: np.ndarray, fold_bias: np.ndarray | None):
-        """``compute_for_items`` for a batch, as score offsets: global + item bias per item (f32, the global bias
-        rounded to f32 first), and per query the user's bias, or ``fold_bias`` where that is not NaN."""
-        ub = np.where(user_nums >= 0, self.user_biases[np.maximum(user_nums, 0)], 0.0).astype(np.float32)
-        if fold_bias is not None:
-            ub = np.where(np.isnan(fold_bias), ub, fold_bias).astype(np.float32)
-        return (self.item_biases + self.global_bias).astype(np.float32), ub
-
-    def transform(self, it: Interactions) -> np.ndarray:
-        return (it.ratings - self.global_bias - self.item_biases[it.items] - self.user_biases[it.users]).astype(
-            np.float32
-        )
-
-
 class BiasedMFScorer(ALSBase):
     """``BiasedMFScorer`` (als/_explicit.py:32-91)."""
 
@@ -615,16 +473,18 @@ class BiasedMFScorer(ALSBase):
     def create_trainer(self, data, options):
         return BiasedMFTrainer(self, data, options)
 
+    def _fold_in_bias(self, item_nums: np.ndarray, ratings: np.ndarray) -> float:
+        """The user bias of a query's rated items (:meth:`BiasModel.user_bias_for_items`), where BiasedMF counts an
+        infinite one, as well as NaN, as 0."""
+        u_bias = self.bias.user_bias_for_items(item_nums, ratings)
+        return u_bias if np.isfinite(u_bias) else 0.0
+
     def new_user_embedding(self, user_num, items: ItemList):
         inums = items.numbers(vocabulary=self.items, missing="negative")
         ratings = items.field("rating")
         assert ratings is not None
         mask = (inums >= 0) & np.isfinite(ratings)
-        uoff = ratings - self.bias.global_bias
-        uoff[inums >= 0] -= self.bias.item_biases[inums[inums >= 0]]
-        u_bias = float(np.sum(uoff) / (np.sum(np.isfinite(uoff)) + self.bias.damping[0]))
-        if not np.isfinite(u_bias):  # BiasModel.compute_for_items zeroes a NaN user bias (basic/bias.py)
-            u_bias = 0.0
+        u_bias = self._fold_in_bias(inums, ratings)
         biases = np.full(len(items), self.bias.global_bias, dtype=np.float32)
         biases[inums >= 0] += self.bias.item_biases[inums[inums >= 0]]
         rv = (ratings - biases - u_bias)[mask].astype(np.float32)
@@ -647,47 +507,23 @@ class BiasedMFScorer(ALSBase):
     def fold_in_batch(self, histories: list[ItemList]):
         """
         ``new_user_embedding`` for a batch of histories on the device: the bias-removed ratings of every
-        history become one row of a CSR matrix and ONE explicit half-epoch (``lk_als_half_epoch`` mode 1,
+        history become one row of ONE explicit half-epoch (``lk_als_half_epoch`` mode 1,
         ``A = MᵀM + reg·n·I``, ``b = Mᵀr`` — the math of ``_train_bias_row_cholesky``,
-        ``_explicit.py:121-147``) solves them all.  The user offsets follow ``BiasModel.compute_for_items``
-        (a non-finite offset counts as 0); ratings that are not finite are left out of the row.
+        ``_explicit.py:121-147``), with the user offsets of :meth:`_fold_in_bias` on the f32 ratings; ratings
+        that are not finite are left out of the row.
         """
-        dev = _lib.require_device()
-        k = self.item_embeddings.shape[1]
-        cols, vals, indptr, offs = [], [], [0], []
+        rows, offs = [], []
         for h in histories:
             inums = h.numbers(vocabulary=self.items, missing="negative")
             ratings = h.field("rating")
             assert ratings is not None
             ratings = np.asarray(ratings, dtype=np.float32)
-            known = inums >= 0
-            uoff = ratings - self.bias.global_bias
-            uoff[known] -= self.bias.item_biases[inums[known]]
-            u_bias = float(np.sum(uoff) / (np.sum(np.isfinite(uoff)) + self.bias.damping[0]))
-            if not np.isfinite(u_bias):
-                u_bias = 0.0
+            u_bias = self._fold_in_bias(inums, ratings)
             offs.append(u_bias)
-            mask = known & np.isfinite(ratings)
+            mask = (inums >= 0) & np.isfinite(ratings)
             biases = self.bias.global_bias + self.bias.item_biases[inums[mask]]
-            rv = (ratings[mask] - biases - u_bias).astype(np.float32)
-            c = inums[mask].astype(np.int32)
-            order = np.argsort(c, kind="stable")  # the CSR container wants ascending columns
-            cols.append(c[order])
-            vals.append(rv[order])
-            indptr.append(indptr[-1] + len(c))
-        csr = InteractionCSR(
-            np.asarray(indptr, dtype=np.int32),
-            np.concatenate(cols) if cols else np.empty(0, np.int32),
-            np.concatenate(vals) if vals else np.empty(0, np.float32),
-            (len(histories), self.item_embeddings.shape[0]),
-        )
-        plan = engine.ALSHalfPlan.create(engine.DeviceCSR.from_host(csr, dev), k)
-        x = torch.zeros((len(histories), k), dtype=torch.float32, device=dev)  # empty histories stay 0 (:134-135)
-        plan.sqdelta.zero_()
-        plan.status.zero_()
-        engine.als_half_epoch(plan, _lib.LK_ALS_EXPLICIT, x, self._device_items(), reg=float(self.config.user_reg))
-        if int(plan.status.item()):
-            raise RuntimeError("ALS solve error: a fold-in system is not positive definite")
+            rows.append((inums[mask], (ratings[mask] - biases - u_bias).astype(np.float32)))
+        x = _solve_fold_in(self._device_items(), rows, _lib.LK_ALS_EXPLICIT, reg=float(self.config.user_reg))
         return x, np.asarray(offs, dtype=np.float32)
 
     def batch_offsets(self, user_nums: np.ndarray, fold_bias: np.ndarray | None):

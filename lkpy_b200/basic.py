@@ -3,8 +3,9 @@ Bias and popularity scorers on the H100 engine — the component surface of ``le
 ``PopScorer`` (``src/lenskit/basic/bias.py``, ``popularity.py``): the two baselines that run beside most models.
 
 Same configs (``BiasConfig.entities`` / ``damping``, ``PopConfig.score``), the same trained attributes
-(``BiasScorer.model``, an :class:`als.BiasModel`; ``PopScorer.items`` and ``item_scores``) and the same
-``__call__``; plus ``score_batch`` and ``recommend_batch``.
+(``BiasScorer.model``, a :class:`BiasModel`; ``PopScorer.items`` and ``item_scores``) and the same
+``__call__``; plus ``score_batch`` and ``recommend_batch``.  :class:`BiasModel` is also the bias model of BiasedMF
+and BiasedSVD.
 
 ``BiasScorer.train`` is ``BiasModel.learn`` on the device (``lk_bias_learn``), bit for bit with the host statements
 on the f32 rating matrix: NumPy's pairwise mean, then each entity's ``np.add.at`` sum in COO order and the f64
@@ -15,7 +16,7 @@ Both score ``s(q, i) = f32(f64(base[i]) + offset[q])`` on ``lk_offset_score_batc
 through argtopn's heap (ties included) without a score matrix:
 
 * ``BiasScorer``: ``base = f32(g) + ib`` (f32), the offset the user's bias, the bias of the query's ratings
-  (``compute_for_items``' statements, NaN counted as 0) or 0 for an unknown user.  That is the reference's
+  (:meth:`BiasModel.user_bias_for_items`, NaN counted as 0) or 0 for an unknown user.  That is the reference's
   ``scores += user_bias``: an f64 bias is added in f64 and rounded once, an f32 one gives the f32 sum.  An item
   the model does not know scores ``f32(g)`` plus the offset, as in the reference, not NaN.
 * ``PopScorer``: ``base = item_scores`` and no offset; an unknown item scores NaN.
@@ -31,13 +32,79 @@ import torch
 from pydantic import BaseModel, NonNegativeFloat, PlainSerializer
 
 from . import _lib, engine
-from .als import BiasModel, _as_dataset
 from .batch import check_exclude, empty_list, history_csr, rank_size, ranked_lists, target_scores
-from .components import Component, ItemList, RecQuery, Trainable, TrainingOptions
+from .components import Component, ItemList, RecQuery, Trainable, TrainingOptions, _as_dataset
+from .data import Interactions
 from .prep import coo_to_csr_pair
-from .svd import query_bias
 
 ENTITIES = frozenset({"user", "item"})
+
+
+class BiasModel:
+    """The part of ``lenskit.basic.BiasModel`` (basic/bias.py:84-150, 216-230) the bias, BiasedMF and BiasedSVD
+    scorers need.  :meth:`learn` is the host statement of :func:`learn`, and its oracle."""
+
+    def __init__(self, global_bias, item_biases, user_biases, damping):
+        self.global_bias = global_bias
+        self.item_biases = item_biases
+        self.user_biases = user_biases
+        self.damping = damping
+
+    @classmethod
+    def learn(cls, it: Interactions, damping, centered_dtype=np.float64, entities=("user", "item")) -> "BiasModel":
+        """``damping``: one float for both, a ``(user, item)`` tuple, or a dict ``{"user": ..., "item": ...}`` in
+        which a missing key means 0.  ``centered_dtype`` is the type of the centred ratings, which the reference
+        takes from its rating matrix: ``np.float32`` gives its statements on an f32 matrix exactly.  ``entities``
+        names the biases to learn; one left out is None."""
+        if isinstance(damping, dict):
+            damping = (float(damping.get("user", 0.0)), float(damping.get("item", 0.0)))
+        d_user, d_item = damping if isinstance(damping, tuple) else (damping, damping)
+        g = float(np.mean(it.ratings))
+        centered = it.ratings.astype(centered_dtype) - g
+        ib = ub = None
+        if "item" in entities:
+            counts = np.full(it.n_items, float(d_item))
+            sums = np.zeros(it.n_items)
+            np.add.at(counts, it.items, 1)
+            np.add.at(sums, it.items, centered)
+            ib = np.zeros(it.n_items, dtype=np.float32)
+            np.divide(sums, counts, out=ib, where=counts > 0, casting="unsafe")
+            centered = centered - ib[it.items]
+        if "user" in entities:
+            counts = np.full(it.n_users, float(d_user))
+            sums = np.zeros(it.n_users)
+            np.add.at(counts, it.users, 1)
+            np.add.at(sums, it.users, centered)
+            ub = np.zeros(it.n_users, dtype=np.float32)
+            np.divide(sums, counts, out=ub, where=counts > 0, casting="unsafe")
+        return cls(g, ib, ub, (d_user, d_item))
+
+    def user_bias_for_items(self, item_nums: np.ndarray | None, ratings: np.ndarray) -> float:
+        """
+        The user bias ``compute_for_items`` takes from a query's rated items (basic/bias.py:216-230): the damped mean
+        of ``rating - g - ib[item]``, with ``ib`` subtracted for the known items (``item_nums >= 0``; ``item_nums``
+        may be None for a model without item biases).  Ratings that are not finite are left out of the count, and a
+        NaN result counts as 0.  The arithmetic is in the dtype of ``ratings``, which the caller chooses.
+        """
+        uoff = ratings - self.global_bias
+        if self.item_biases is not None:
+            known = item_nums >= 0
+            uoff[known] -= self.item_biases[item_nums[known]]
+        ub = np.sum(uoff) / (np.sum(np.isfinite(uoff)) + self.damping[0])
+        return 0.0 if np.isnan(ub) else float(ub)
+
+    def batch_offsets(self, user_nums: np.ndarray, fold_bias: np.ndarray | None):
+        """``compute_for_items`` for a batch, as score offsets: global + item bias per item (f32, the global bias
+        rounded to f32 first), and per query the user's bias, or ``fold_bias`` where that is not NaN."""
+        ub = np.where(user_nums >= 0, self.user_biases[np.maximum(user_nums, 0)], 0.0).astype(np.float32)
+        if fold_bias is not None:
+            ub = np.where(np.isnan(fold_bias), ub, fold_bias).astype(np.float32)
+        return (self.item_biases + self.global_bias).astype(np.float32), ub
+
+    def transform(self, it: Interactions) -> np.ndarray:
+        return (it.ratings - self.global_bias - self.item_biases[it.items] - self.user_biases[it.users]).astype(
+            np.float32
+        )
 
 
 def damping_pair(damping) -> tuple[float, float]:
@@ -55,7 +122,7 @@ def damping_pair(damping) -> tuple[float, float]:
 
 def learn(data, damping=0.0, *, entities=ENTITIES, centered_dtype=np.float32) -> BiasModel:
     """
-    ``BiasModel.learn(data, damping, entities=...)`` on the device, bit for bit with :meth:`als.BiasModel.learn` on
+    ``BiasModel.learn(data, damping, entities=...)`` on the device, bit for bit with :meth:`BiasModel.learn` on
     the same ``centered_dtype`` (``np.float32``: the reference's f32 rating matrix; ``np.float64``: BiasedMF's
     centring).  A bias left out of ``entities`` is None.
     """
@@ -180,9 +247,11 @@ class BiasScorer(_OffsetScorer):
         if m.user_biases is None:
             return out
         for b, q in enumerate(queries):
-            fold = query_bias(m, self.items, q)
-            if fold is not None:
-                out[b] = fold
+            rated = q.query_items
+            ratings = None if rated is None else rated.field("rating")
+            if ratings is not None:
+                nums = None if m.item_biases is None else rated.numbers(vocabulary=self.items, missing="negative")
+                out[b] = m.user_bias_for_items(nums, ratings)
             elif q.user_id is not None:
                 uno = self.users.number(q.user_id, missing="none")
                 if uno is not None:

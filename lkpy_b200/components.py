@@ -22,6 +22,8 @@ from typing import Any, Literal
 
 import numpy as np
 
+from .data import Interactions
+
 
 class Vocabulary:
     """Sorted id <-> number map."""
@@ -249,3 +251,11 @@ class Dataset:
         it = self.interactions
         lo, hi = np.searchsorted(it.users, [user_num, user_num + 1])
         return ItemList(item_nums=it.items[lo:hi], vocabulary=self.items, rating=it.ratings[lo:hi])
+
+
+def _as_dataset(data) -> Dataset:
+    if isinstance(data, Dataset):
+        return data
+    if isinstance(data, Interactions):
+        return Dataset(data)
+    raise TypeError("expected a Dataset or Interactions")

@@ -26,8 +26,7 @@ import torch
 from pydantic import BaseModel, PositiveFloat
 
 from . import _lib, engine
-from .als import _as_dataset
-from .components import Component, ItemList, Trainable, TrainingOptions
+from .components import Component, ItemList, Trainable, TrainingOptions, _as_dataset
 from .batch import check_exclude, empty_list, history_csr, rank_size, ranked_lists, target_scores
 
 MIN_SCIPY_VERSION = "1.17"

@@ -21,9 +21,9 @@ registers, so ``self.u_bias is not None`` is false in ``__init__`` and ``forward
 never drawn from the seeded generator, never enter a score or the L2 norm and never receive a gradient; the
 embeddings take the generator's first draws.  The explicit model here computes exactly that model, ``u·i + mu``.
 
-Inference is ``ub + ib + u·i`` (implicit) or ``u·i + mu`` (explicit): the ALS scorers' batched scoring and fused
-top-n (``lk_als_recommend_batch``) with the item bias as the item offset and the user bias (or the mean) as the query
-offset.
+Inference is ``ub + ib + u·i`` (implicit) or ``u·i + mu`` (explicit): the known-user scoring and fused top-n of
+:class:`factors.KnownUserScorer` (``lk_als_recommend_batch``) with the item bias as the item offset and the user bias
+(or the mean) as the query offset.
 """
 
 from __future__ import annotations
@@ -32,42 +32,25 @@ from typing import Literal
 
 import numpy as np
 import torch
-from pydantic import BaseModel, NonNegativeInt, PositiveFloat, PositiveInt, field_validator, model_validator
+from pydantic import NonNegativeInt, PositiveFloat, PositiveInt, model_validator
 
 from . import _lib, engine
-from .als import ALSBase, _as_dataset
-from .batch import target_scores
-from .components import ItemList, ModelTrainer, RecQuery, TrainingOptions, Vocabulary
+from .components import ModelTrainer, TrainingOptions, UsesTrainer, Vocabulary, _as_dataset
+from .factors import EmbeddingSize, EmbeddingSizeExp, KnownUserScorer
 
 PRESETS = {"bpr": {"loss": "pairwise", "user_bias": False, "item_bias": False}}
 PARAM_NAMES = ("u_bias.weight", "i_bias.weight", "u_embed.weight", "i_embed.weight")
 
 
-class FlexMFConfigBase(BaseModel):
+class FlexMFConfigBase(EmbeddingSizeExp):
     """``FlexMFConfigBase`` (``_base.py:34-95``): what the two models' configurations share."""
 
-    embedding_size: PositiveInt = 64
+    embedding_size: EmbeddingSize = 64
     batch_size: PositiveInt = 8 * 1024
     learning_rate: float = 0.01
     epochs: int = 10
     regularization: float = 0.01
     reg_method: Literal["AdamW", "L2"] | None = "AdamW"
-
-    @model_validator(mode="before")
-    @classmethod
-    def apply_aliases(cls, data):
-        if isinstance(data, dict) and "embedding_size_exp" in data:  # EmbeddingSizeMixin: the size as a power of two
-            data = {k: v for k, v in data.items() if k not in ("embedding_size_exp", "embedding_size")} | {
-                "embedding_size": 2 ** data["embedding_size_exp"]
-            }
-        return data
-
-    @field_validator("embedding_size", mode="after")
-    @staticmethod
-    def check_embedding_size(k) -> int:
-        if k > engine.ALS_MAX_FEATURES:
-            raise ValueError(f"embedding_size={k} exceeds the engine limit of {engine.ALS_MAX_FEATURES}")
-        return k
 
 
 class FlexMFImplicitConfig(FlexMFConfigBase):
@@ -159,43 +142,20 @@ def initial_parameters(n_users: int, n_items: int, k: int, user_bias: bool, item
     return out
 
 
-class FlexMFScorerBase(ALSBase):
-    """``FlexMFScorerBase`` (``_base.py:98-164``): ``__call__`` and the batched ``score_matrix`` / ``score_batch`` /
-    ``recommend_batch`` (inherited from the ALS scorers, with the biases as the kernel's offsets)."""
+class FlexMFScorerBase(KnownUserScorer, UsesTrainer):
+    """``FlexMFScorerBase`` (``_base.py:98-164``): the known-user scoring of :class:`KnownUserScorer`
+    (``__call__`` and the batched ``score_matrix`` / ``score_batch`` / ``recommend_batch``) with the biases as the
+    kernel's offsets."""
 
     config: FlexMFConfigBase
     user_bias: np.ndarray | None = None
     item_bias: np.ndarray | None = None
-
-    def embed_batch(self, queries):
-        """Known users' embeddings; a query without a known user is unscorable (``_base.py:126-133``)."""
-        dev = _lib.require_device()
-        queries = [RecQuery.create(q) for q in queries]
-        nums = [None if q.user_id is None else self.users.number(q.user_id, missing=None) for q in queries]
-        user_nums = np.array([-1 if u is None else u for u in nums], dtype=np.int64)
-        scorable = user_nums >= 0
-        X = np.zeros((len(queries), self.item_embeddings.shape[1]), dtype=np.float32)
-        X[scorable] = self.user_embeddings[user_nums[scorable]]
-        return torch.from_numpy(X).to(dev), scorable, user_nums, None
 
     def batch_offsets(self, user_nums: np.ndarray, fold_bias):
         ub = None
         if self.user_bias is not None:
             ub = np.where(user_nums >= 0, self.user_bias[np.maximum(user_nums, 0)], 0.0).astype(np.float32)
         return self.item_bias, ub
-
-    def score_batch(self, queries, targets: list[ItemList]) -> list[ItemList]:
-        """Score ``targets[i]`` for ``queries[i]``: columns of :meth:`score_matrix` picked out on the device.
-        Unknown items, and every item of a query without a known user, score NaN."""
-        return target_scores(self.score_matrix(queries).T, targets, self.items)
-
-    def __call__(self, query, items: ItemList) -> ItemList:
-        return self.score_batch([query], [items])[0]
-
-    def __getstate__(self):
-        d = dict(self.__dict__)
-        d.pop("_d_items_cache", None)  # host arrays are the pickled state
-        return d
 
 
 class FlexMFImplicitScorer(FlexMFScorerBase):

@@ -21,9 +21,8 @@ import torch
 from pydantic import AliasChoices, BaseModel, Field, PositiveFloat, PositiveInt, field_validator
 
 from . import _lib, engine
-from .als import _as_dataset
 from .batch import check_exclude, empty_list, rank_size, ranked_lists
-from .components import Component, ItemList, RecQuery, Trainable, TrainingOptions
+from .components import Component, ItemList, RecQuery, Trainable, TrainingOptions, _as_dataset
 from .data import InteractionCSR, knn_item_matrices
 
 

@@ -36,8 +36,7 @@ from pydantic import AliasChoices, BaseModel, Field, PositiveFloat, PositiveInt,
 from scipy.sparse import csr_array
 
 from . import _lib, engine
-from .als import _as_dataset
-from .components import Component, ItemList, RecQuery, Trainable, TrainingOptions
+from .components import Component, ItemList, RecQuery, Trainable, TrainingOptions, _as_dataset
 from .data import InteractionCSR
 from .batch import check_exclude, empty_list, history_csr, rank_size, ranked_lists
 

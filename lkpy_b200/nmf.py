@@ -21,9 +21,9 @@ Training follows scikit-learn (``solver="cd"``, ``init=None``, ``tol=1e-4``, no 
 The SVD of the initialisation is cuSOLVER's instead of LAPACK's and the Grams are rounded once, so the factors agree
 with the reference's to rounding, not bit for bit (DESIGN.md §4.17).
 
-Scoring is the ALS scorers' batched path (``lk_als_recommend_batch``) over ``user_components`` and
-``item_components`` with no offsets: one f32 FMA chain per score, where the reference takes an f32 product and returns
-it as f64.
+Scoring is the known-user path of :class:`factors.KnownUserScorer` (``lk_als_recommend_batch``) over
+``user_components`` and ``item_components`` with no offsets: one f32 FMA chain per score, where the reference takes an
+f32 product and returns it as f64.
 """
 
 from __future__ import annotations
@@ -34,12 +34,11 @@ from typing import Literal
 import numpy as np
 import scipy.sparse as sps
 import torch
-from pydantic import AliasChoices, BaseModel, Field, PositiveInt, field_validator, model_validator
+from pydantic import AliasChoices, Field, PositiveInt, field_validator
 
 from . import _lib, engine
-from .als import _as_dataset
-from .components import Trainable, TrainingOptions
-from .flexmf import FlexMFScorerBase
+from .components import Trainable, TrainingOptions, _as_dataset
+from .factors import EmbeddingSizeExp, KnownUserScorer, within_engine_limit
 from .prep import coo_to_csr_pair
 
 try:
@@ -55,7 +54,7 @@ N_OVERSAMPLES = 10
 TOL = 1e-4
 
 
-class NMFConfig(BaseModel, extra="forbid"):
+class NMFConfig(EmbeddingSizeExp, extra="forbid"):
     beta_loss: Literal["frobenius", "kullback-leibler", "itakura-saito"] = "frobenius"
     max_iter: PositiveInt = Field(default=200, validation_alias=AliasChoices("max_iter", "epochs"))
     embedding_size: PositiveInt | None = Field(
@@ -66,23 +65,12 @@ class NMFConfig(BaseModel, extra="forbid"):
     l1_ratio: float = 0.0
     method: Literal["full", "minibatch"] = "full"
 
-    @model_validator(mode="before")
-    @classmethod
-    def apply_aliases(cls, data):
-        if isinstance(data, dict) and "embedding_size_exp" in data:  # EmbeddingSizeMixin: the size as a power of two
-            data = {k: v for k, v in data.items() if k not in ("embedding_size_exp", "embedding_size", "n_components")} | {
-                "embedding_size": 2 ** data["embedding_size_exp"]
-            }
-        return data
-
     @field_validator("embedding_size", mode="after")
     @staticmethod
     def check_embedding_size(k) -> int:
         if k is None:
             raise ValueError("embedding_size=None (scikit-learn's n_features) is not covered by the engine")
-        if k > engine.ALS_MAX_FEATURES:
-            raise ValueError(f"embedding_size={k} exceeds the engine limit of {engine.ALS_MAX_FEATURES}")
-        return k
+        return within_engine_limit(k)
 
     @field_validator("beta_loss", mode="after")
     @staticmethod
@@ -163,9 +151,9 @@ def factorize(x: engine.SvdOperand, config: NMFConfig, stage=None) -> tuple[torc
     return d.W, d.Ht.T, n_iter
 
 
-class NMFScorer(FlexMFScorerBase, Trainable):
+class NMFScorer(KnownUserScorer, Trainable):
     """
-    ``NMFScorer``: ``train`` on the device, and the known-user scoring of :class:`FlexMFScorerBase`
+    ``NMFScorer``: ``train`` on the device, and the known-user scoring of :class:`KnownUserScorer`
     (``score_matrix`` / ``score_batch`` / ``__call__`` / ``recommend_batch``) with no offsets.  A query whose user
     is unknown scores NaN and gets an empty list.
     """
@@ -193,4 +181,3 @@ class NMFScorer(FlexMFScorerBase, Trainable):
         self.users, self.items = ds.users, ds.items
         self.user_embeddings = self.user_components
         self.item_embeddings = self.item_components
-        self.__dict__.pop("_d_items_cache", None)

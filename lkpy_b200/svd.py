@@ -21,11 +21,11 @@ Training follows the reference on the device:
 
 ``algorithm="arpack"`` (SciPy's ``svds``) is rejected when the configuration is made.
 
-Scoring is the ALS scorers' batched path (``lk_als_recommend_batch``): the user's component row against
-``components_.T``, with ``f32(g) + ib`` as the item offset and the user bias as the query offset, or the bias of the
-query's ratings when the query carries rated items (``BiasModel.compute_for_items``).  Each score is one f32 FMA
-chain over the components followed by two f32 adds; the reference computes ``user_components[u] @ components_`` as an
-f32 product and adds the biases in f64, returning f64 scores, so the two agree to f32 rounding.
+Scoring is the known-user path of :class:`factors.KnownUserScorer` (``lk_als_recommend_batch``): the user's component
+row against ``components_.T``, with ``f32(g) + ib`` as the item offset and the user bias as the query offset, or the
+bias of the query's ratings when the query carries rated items (:meth:`basic.BiasModel.user_bias_for_items`). Each
+score is one f32 FMA chain over the components followed by two f32 adds; the reference computes ``user_components[u] @
+components_`` as an f32 product and adds the biases in f64, returning f64 scores, so the two agree to f32 rounding.
 """
 
 from __future__ import annotations
@@ -34,40 +34,23 @@ from typing import Literal
 
 import numpy as np
 import torch
-from pydantic import AliasChoices, BaseModel, Field, NonNegativeFloat, NonNegativeInt, PositiveInt, field_validator
-from pydantic import model_validator
+from pydantic import AliasChoices, Field, NonNegativeFloat, NonNegativeInt, field_validator
 
 from . import _lib, engine
-from .als import BiasModel, _as_dataset
-from .components import RecQuery, Trainable, TrainingOptions
-from .flexmf import FlexMFScorerBase
+from .basic import BiasModel
+from .components import RecQuery, Trainable, TrainingOptions, _as_dataset
+from .factors import EmbeddingSize, EmbeddingSizeExp, KnownUserScorer
 from .prep import coo_to_csr_pair
 
 #: scikit-learn's ``TruncatedSVD`` default ``n_oversamples``
 N_OVERSAMPLES = 10
 
 
-class BiasedSVDConfig(BaseModel, extra="forbid"):
-    embedding_size: PositiveInt = Field(default=64, validation_alias=AliasChoices("embedding_size", "features"))
+class BiasedSVDConfig(EmbeddingSizeExp, extra="forbid"):
+    embedding_size: EmbeddingSize = Field(default=64, validation_alias=AliasChoices("embedding_size", "features"))
     damping: NonNegativeFloat | dict[Literal["user", "item"], NonNegativeFloat] = 5
     algorithm: Literal["arpack", "randomized"] = "randomized"
     n_iter: NonNegativeInt = 5
-
-    @model_validator(mode="before")
-    @classmethod
-    def apply_aliases(cls, data):
-        if isinstance(data, dict) and "embedding_size_exp" in data:  # EmbeddingSizeMixin: the size as a power of two
-            data = {k: v for k, v in data.items() if k not in ("embedding_size_exp", "embedding_size", "features")} | {
-                "embedding_size": 2 ** data["embedding_size_exp"]
-            }
-        return data
-
-    @field_validator("embedding_size", mode="after")
-    @staticmethod
-    def check_embedding_size(k) -> int:
-        if k > engine.ALS_MAX_FEATURES:
-            raise ValueError(f"embedding_size={k} exceeds the engine limit of {engine.ALS_MAX_FEATURES}")
-        return k
 
     @field_validator("algorithm", mode="after")
     @staticmethod
@@ -77,25 +60,9 @@ class BiasedSVDConfig(BaseModel, extra="forbid"):
         return algorithm
 
 
-def query_bias(bias: BiasModel, items, query: RecQuery) -> float | None:
-    """The user bias ``BiasModel.compute_for_items`` takes from the query's rated items, or None when the query has
-    no ``rating`` field (the user's trained bias applies then).  A NaN bias counts as 0."""
-    if query.query_items is None:
-        return None
-    ratings = query.query_items.field("rating")
-    if ratings is None:
-        return None
-    uoff = ratings - bias.global_bias
-    if bias.item_biases is not None:
-        nums = query.query_items.numbers(vocabulary=items, missing="negative")
-        uoff[nums >= 0] -= bias.item_biases[nums[nums >= 0]]
-    ub = np.sum(uoff) / (np.sum(np.isfinite(uoff)) + bias.damping[0])
-    return 0.0 if np.isnan(ub) else float(ub)
-
-
-class BiasedSVDScorer(FlexMFScorerBase, Trainable):
+class BiasedSVDScorer(KnownUserScorer, Trainable):
     """
-    ``BiasedSVDScorer``: ``train`` on the device, and the known-user scoring of :class:`FlexMFScorerBase`
+    ``BiasedSVDScorer``: ``train`` on the device, and the known-user scoring of :class:`KnownUserScorer`
     (``score_matrix`` / ``score_batch`` / ``__call__`` / ``recommend_batch``) with the biases as the kernel's offsets.
     A query whose user is unknown scores NaN and gets an empty list.
     """
@@ -134,12 +101,17 @@ class BiasedSVDScorer(FlexMFScorerBase, Trainable):
         # the scoring path's tables: user rows, and item rows [n_items, k]
         self.user_embeddings = self.user_components
         self.item_embeddings = np.ascontiguousarray(self.components_.T)
-        self.__dict__.pop("_d_items_cache", None)
 
     def embed_batch(self, queries):
+        """Known users' embeddings, and as the user offset the bias of the query's ratings where it has them."""
+        queries = [RecQuery.create(q) for q in queries]
         X, scorable, user_nums, _ = super().embed_batch(queries)
-        fold = [query_bias(self.bias, self.items, RecQuery.create(q)) for q in queries]
-        fold_bias = np.array([np.nan if b is None else b for b in fold], dtype=np.float32)
+        fold_bias = np.full(len(queries), np.nan, dtype=np.float32)
+        for b, q in enumerate(queries):
+            ratings = None if q.query_items is None else q.query_items.field("rating")
+            if ratings is not None:
+                nums = q.query_items.numbers(vocabulary=self.items, missing="negative")
+                fold_bias[b] = self.bias.user_bias_for_items(nums, ratings)
         return X, scorable, user_nums, fold_bias
 
     def batch_offsets(self, user_nums: np.ndarray, fold_bias):

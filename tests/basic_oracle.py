@@ -3,7 +3,8 @@ Host restatements for the bias model and the offset scorers (tests/test_basic*.p
 
 * NumPy's pairwise f32 sum, and the global mean the way ``lk_bias_learn`` evaluates it — the tree cut at
   ``MEAN_DEPTH``, each subtree summed on its own, the inner nodes above combined level by level;
-* ``BiasModel.compute_for_items`` (basic/bias.py), statement for statement, for one query;
+* ``BiasModel.compute_for_items`` (basic/bias.py), statement for statement, for one query: the user bias of its rated
+  items (the oracle of ``basic.BiasModel.user_bias_for_items``) and the scores;
 * the host composition a batched ranking must reproduce: scores, exclusions as NaN, ``argtopn``.
 """
 
@@ -88,7 +89,7 @@ def kernel_mean(r: np.ndarray) -> np.float32:
 
 def bias_scores(model, users, items, query, targets) -> np.ndarray:
     """``BiasScorer.__call__``: ``model.compute_for_items(targets, query.user_id, query.query_items)``'s scores,
-    with the reference's statements on ``lkpy_b200.als.BiasModel`` (``damping`` as ``(user, item)``)."""
+    with the reference's statements on ``lkpy_b200.basic.BiasModel`` (``damping`` as ``(user, item)``)."""
     scores = np.full(len(targets), model.global_bias, dtype=np.float32)
     if model.item_biases is not None:
         idxes = targets.numbers(vocabulary=items, missing="negative")
@@ -98,20 +99,25 @@ def bias_scores(model, users, items, query, targets) -> np.ndarray:
     ratings = None if user_items is None else user_items.field("rating")
     if model.user_biases is not None:
         if ratings is not None:
-            uoff = ratings - model.global_bias
-            if model.item_biases is not None:
-                r_idxes = user_items.numbers(vocabulary=items, missing="negative")
-                r_mask = r_idxes >= 0
-                uoff[r_mask] -= model.item_biases[r_idxes[r_mask]]
-            user_bias = np.sum(uoff) / (np.sum(np.isfinite(uoff)) + model.damping[0])
-            if np.isnan(user_bias):
-                user_bias = 0
-            scores += user_bias
+            scores += rated_user_bias(model, items, user_items)
         elif query.user_id is not None:
             uno = users.number(query.user_id, missing="none")
             if uno is not None:
                 scores += model.user_biases[uno]
     return scores
+
+
+def rated_user_bias(model, items, user_items):
+    """``compute_for_items``' user bias from the rated items ``user_items`` (they have a ``rating`` field)."""
+    uoff = user_items.field("rating") - model.global_bias
+    if model.item_biases is not None:
+        r_idxes = user_items.numbers(vocabulary=items, missing="negative")
+        r_mask = r_idxes >= 0
+        uoff[r_mask] -= model.item_biases[r_idxes[r_mask]]
+    user_bias = np.sum(uoff) / (np.sum(np.isfinite(uoff)) + model.damping[0])
+    if np.isnan(user_bias):
+        user_bias = 0
+    return user_bias
 
 
 def ranked(scores: np.ndarray, excluded, n: int) -> tuple[np.ndarray, np.ndarray]:

@@ -229,6 +229,9 @@ def test_components_pickle_round_trip(cuda_lib, ml_small):
     for m in models:
         before = m.recommend_batch(queries, 50, exclude="query")
         m2 = pickle.loads(pickle.dumps(m))
+        # the device item table stays out of the pickle: it loads without a GPU
+        state = [x for v in m2.__dict__.values() for x in (v if isinstance(v, tuple) else (v,))]
+        assert not any(isinstance(x, torch.Tensor) for x in state)
         after = m2.recommend_batch(queries, 50, exclude="query")
         for r0, r1 in zip(before, after):
             assert np.array_equal(r0.numbers(vocabulary=m.items), r1.numbers(vocabulary=m2.items))

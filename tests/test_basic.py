@@ -19,8 +19,7 @@ import basic_oracle as bo
 import basic_ref_sandbox as brs
 import ref_sandbox
 from lkpy_b200 import _lib
-from lkpy_b200.als import BiasModel
-from lkpy_b200.basic import BiasConfig, BiasScorer, PopConfig, PopScorer, damping_pair
+from lkpy_b200.basic import BiasConfig, BiasModel, BiasScorer, PopConfig, PopScorer, damping_pair
 from lkpy_b200.components import Dataset, ItemList, RecQuery
 from test_flexmf import test_ctypes_structs_match_header as _layout_check
 
@@ -141,7 +140,7 @@ def our_queries(ml_small, vocab_items):
 
 @pytest.mark.parametrize("name", list(brs.BIAS_CONFIGS))
 def test_host_bias_statements_are_the_reference(ml_small, name):
-    """``als.BiasModel.learn`` (the oracle of ``lk_bias_learn``) on the f32 ratings and ``compute_for_items``'
+    """``basic.BiasModel.learn`` (the oracle of ``lk_bias_learn``) on the f32 ratings and ``compute_for_items``'
     statements reproduce the reference BiasScorer's model and scores bit for bit."""
     g = reference_golden(f"basic_bias_{name}", ml_small)
     cfg = BiasConfig(**brs.BIAS_CONFIGS[name])
@@ -156,6 +155,29 @@ def test_host_bias_statements_are_the_reference(ml_small, name):
     for q, want in zip(our_queries(ml_small, ds.items), g["scores"]):
         got = bo.bias_scores(m, ds.users, ds.items, q, targets)
         assert np.array_equal(got.view(np.int32), want.view(np.int32))
+
+
+def test_user_bias_for_items_is_compute_for_items(ml_small):
+    """``BiasModel.user_bias_for_items`` against ``compute_for_items``' statements, in the ratings' dtype: unknown
+    items, NaN ratings, an all-NaN query, infinite ratings (an infinite bias stays infinite, as in the reference), and a
+    model without item biases."""
+    ds = Dataset(ml_small)
+    ids = ds.items.ids()
+    cases = [([ids[0], ids[5], -7], [4.0, 3.5, 2.0]), ([ids[1], ids[2], ids[3]], [np.nan, 5.0, 1.0]),
+             ([ids[1], ids[2]], [np.nan, np.nan]), ([ids[4], ids[9]], [np.inf, 3.0]),
+             ([ids[4], ids[9]], [-np.inf, 3.0]), ([ids[4], ids[9]], [np.inf, -np.inf])]  # fmt: skip
+    for entities in (("user", "item"), ("user",)):
+        m = BiasModel.learn(ml_small, (2.5, 1.0), np.float32, entities)
+        for item_ids, ratings in cases:
+            for dtype in (np.float32, np.float64):
+                q = ItemList(item_ids=item_ids, rating=np.array(ratings, dtype=dtype))
+                got = m.user_bias_for_items(q.numbers(vocabulary=ds.items, missing="negative"), q.field("rating"))
+                want = bo.rated_user_bias(m, ds.items, q)
+                assert np.float64(got).view(np.int64) == np.float64(want).view(np.int64), (entities, ratings, dtype)
+        q = ItemList(item_ids=[ids[4], ids[9]], rating=[np.inf, 3.0])
+        assert m.user_bias_for_items(q.numbers(vocabulary=ds.items), q.field("rating")) == np.inf
+        q = ItemList(item_ids=[ids[1], ids[2]], rating=[np.nan, np.nan])
+        assert m.user_bias_for_items(q.numbers(vocabulary=ds.items), q.field("rating")) == 0.0
 
 
 @pytest.mark.parametrize("mode", brs.POP_SCORES)

@@ -1,6 +1,6 @@
 """
 BiasScorer and PopScorer on the device: ``lk_bias_learn`` bit for bit against the host statements
-(``als.BiasModel.learn``), ``lk_offset_score_batch`` rankings against the host composition (``__call__``, exclusion,
+(``basic.BiasModel.learn``), ``lk_offset_score_batch`` rankings against the host composition (``__call__``, exclusion,
 ``argtopn``), and the trained scorers against the recordings of the reference's own classes.
 """
 
@@ -12,7 +12,7 @@ import pytest
 import basic_oracle as bo
 import basic_ref_sandbox as brs
 from lkpy_b200 import basic, engine
-from lkpy_b200.als import BiasModel
+from lkpy_b200.basic import BiasModel
 from lkpy_b200.basic import BiasScorer, PopScorer
 from lkpy_b200.components import Dataset, ItemList, RecQuery, TrainingOptions
 from lkpy_b200.data import Interactions

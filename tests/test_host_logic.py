@@ -92,6 +92,33 @@ def test_solve_cholesky_property():
         assert F @ x == approx(y, rel=2.0e-6, abs=5.0e-9)
 
 
+def test_biased_mf_fold_in_zeroes_an_infinite_user_bias():
+    """BiasedMF's fold-in counts a user bias that is not finite as 0: NaN, as the reference's ``compute_for_items``
+    does, and also an infinite one, which ``BiasModel.user_bias_for_items`` (the reference's rule) keeps."""
+    from lkpy_b200.als import BiasedMFScorer, _solve_cholesky
+    from lkpy_b200.basic import BiasModel
+    from lkpy_b200.components import ItemList, Vocabulary
+
+    rng = np.random.default_rng(7)
+    m = BiasedMFScorer(embedding_size=8)
+    m.items = Vocabulary(np.arange(20), "item")
+    m.item_embeddings = rng.standard_normal((20, 8)).astype(np.float32)
+    m.bias = BiasModel(3.5, (rng.standard_normal(20) * 0.1).astype(np.float32), np.zeros(4, np.float32), (5.0, 5.0))
+    items = np.array([2, 7, 11])
+    for ratings, rule in (([np.inf, 4.0, 3.0], np.inf), ([-np.inf, 4.0, 3.0], -np.inf), ([np.inf, -np.inf, 3.0], 0.0)):
+        for dtype in (np.float32, np.float64):
+            q = ItemList(item_ids=items, rating=np.array(ratings, dtype=dtype))
+            assert m.bias.user_bias_for_items(items, q.field("rating")) == rule
+            emb, u_bias = m.new_user_embedding(None, q)
+            assert u_bias == 0.0
+            rated = items[np.isfinite(ratings)]
+            M = m.item_embeddings[rated]
+            rv = (np.asarray(ratings)[np.isfinite(ratings)] - 3.5 - m.bias.item_biases[rated]).astype(np.float32)
+            want = _solve_cholesky(M.T @ M + np.eye(8, dtype=np.float32) * 0.1 * len(rated), M.T @ rv)
+            assert np.allclose(emb, want, rtol=1e-5, atol=1e-6)
+            assert np.isfinite(m(q, ItemList(item_ids=[1, 2, 3])).scores()).all()
+
+
 def test_accel_mirror_signatures_match_reference_stubs():
     """Every function the reference's typed stubs declare for the two hot paths (`_accel/als.pyi`,
     `_accel/knn.pyi`, recorded in tests/golden/accel_stub_signatures.json) exists in lkpy_b200.accel with

@@ -23,7 +23,7 @@ import ref_sandbox
 import svd_oracle as so
 import svd_ref_sandbox as srs
 from lkpy_b200 import _lib
-from lkpy_b200.als import BiasModel
+from lkpy_b200.basic import BiasModel
 from lkpy_b200.components import Dataset
 from lkpy_b200.svd import BiasedSVDConfig, BiasedSVDScorer
 
@@ -90,7 +90,7 @@ def test_restatement_is_truncated_svd(ml_small, n_iter, transposed):
 
 @pytest.mark.parametrize("k", GOLDEN_K)
 def test_restatement_is_the_reference(ml_small, k):
-    """The restatement, with the bias model of ``lkpy_b200.als`` and the start matrix drawn after
+    """The restatement, with the bias model of ``lkpy_b200.basic`` and the start matrix drawn after
     ``np.random.seed``, reproduces the reference's recording (the biases bit for bit) and leaves the global state
     where it did."""
     g = reference_golden(ml_small, k)

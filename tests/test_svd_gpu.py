@@ -11,12 +11,13 @@ import pytest
 import scipy.sparse as sps
 import torch
 
+import basic_oracle as bo
 import oracle
 import svd_oracle as so
 import svd_ref_sandbox as srs
 import test_svd as host
 from lkpy_b200 import engine, svd
-from lkpy_b200.als import BiasModel
+from lkpy_b200.basic import BiasModel
 from lkpy_b200.components import Dataset, ItemList, RecQuery
 from lkpy_b200.data import InteractionCSR, Interactions
 from lkpy_b200.svd import BiasedSVDScorer
@@ -146,7 +147,7 @@ def test_reference_three_by_three_case():
     assert np.isnan(m(50, ItemList(item_ids=[3])).scores()).all()
 
 
-def test_scorer_batched_interface(ml_small):
+def test_scorer_batched_interface_against_host_bias(ml_small):
     ds = Dataset(ml_small)
     np.random.seed(3)
     m = BiasedSVDScorer(embedding_size=16)
@@ -179,7 +180,7 @@ def test_scorer_batched_interface(ml_small):
     # the score chain: user components . item components (f32 FMA chain), + (f32(g) + ib), + user bias
     ib = (m.bias.item_biases + m.bias.global_bias).astype(np.float32)
     for b, u in ((0, 0), (2, 77)):
-        ub = m.bias.user_biases[u] if b == 0 else svd.query_bias(m.bias, m.items, queries[b])
+        ub = m.bias.user_biases[u] if b == 0 else bo.rated_user_bias(m.bias, m.items, queries[b].query_items)
         want = (m.components_.T.astype(np.float64) @ m.user_components[u] + ib) + np.float32(ub)
         assert np.allclose(S[:, b], want, rtol=1e-5, atol=1e-5)
     m2 = pickle.loads(pickle.dumps(m))

@@ -31,7 +31,7 @@ sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 
 import oracle  # noqa: E402
 from lkpy_b200 import _lib, basic, data, engine  # noqa: E402
-from lkpy_b200.als import BiasModel  # noqa: E402
+from lkpy_b200.basic import BiasModel  # noqa: E402
 from lkpy_b200.components import Dataset, ItemList, RecQuery  # noqa: E402
 from lkpy_b200.prep import coo_to_csr_pair  # noqa: E402
 

@@ -33,7 +33,7 @@ import torch
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 
 from lkpy_b200 import _lib, data, engine, svd  # noqa: E402
-from lkpy_b200.als import BiasModel  # noqa: E402
+from lkpy_b200.basic import BiasModel  # noqa: E402
 from lkpy_b200.components import Dataset, ItemList, RecQuery  # noqa: E402
 
 
