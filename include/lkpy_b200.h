@@ -32,6 +32,9 @@
  *   NMFScorer.__call__ + TopNRanker               src/lenskit/sklearn/nmf.py         lk_als_recommend_batch
  *   BiasModel.learn (NumPy, host)                 src/lenskit/basic/bias.py:84-150   lk_bias_learn
  *   BiasScorer / PopScorer __call__ + TopNRanker  src/lenskit/basic/bias.py, popularity.py lk_offset_score_batch
+ *   StochasticTopNRanker.__call__ (_compute_keys + ItemList.top_n)
+ *                                                 src/lenskit/stochastic/_ranker.py:89-156,
+ *                                                 src/lenskit/data/_items.py:942-998 lk_stochastic_topn
  *
  * Conventions
  *   - plain C: pointers and sizes only; no C++/torch types cross this boundary;
@@ -870,6 +873,66 @@ typedef struct lk_offset_score_args {
 } lk_offset_score_args;
 
 LK_API int lk_offset_score_batch(const lk_offset_score_args *args, void *stream);
+
+/* ------------------------------------------------------------------------
+ * Stochastic top-n (stochastic.cu), behind StochasticTopNRanker (src/lenskit/stochastic/_ranker.py:89-156).
+ *
+ * Each of B rows holds n_items f32 scores at d_scores[q * row_stride + i * item_stride] (a contiguous [B][L]
+ * matrix, or the transpose of an item-major [L][B] one, without a copy).  Position i of row q is valid when its score
+ * is finite and i is not among the row's exclusions (ascending, in range; topn_excluded's semantics).  With N valid
+ * positions, numbered in list order, and s = f32(score * scale):
+ *   LK_STOCH_SOFTMAX  e = f32(exp(f64(s - max s)));  w = e / (+0.0f + pairwise(e))               (f32)
+ *   LK_STOCH_LINEAR   r = f64(max s) - f64(min s); t = (s - min s) / f32(r); w = t / (+0.0f + pairwise(t));
+ *                     w = 1.0f / f32(N) when !(r > 0) or !(sum > 0)                              (f32)
+ *   LK_STOCH_NONE     w = s
+ *   key = log(u) / f64(max(w, FLT_MIN))   (f64), u = (raw >> 11) * 2^-53 the k-th draw of the query's stream for
+ *   the k-th valid position, raw = XSL-RR of the PCG64 state after the draw's step (NumPy's PCG64: the 128-bit LCG
+ *   state = state * M + inc, then the output of the new state).  pairwise is NumPy's order (pairwise.cuh) over
+ *   the valid values in list order.  A row with nothing valid draws nothing.
+ * Streams: d_state holds (state_hi, state_lo, inc_hi, inc_lo).  shared_stream = 0: row q draws from its own state
+ *   d_state[4q .. 4q+3] from its start.  shared_stream = 1: every row draws from d_state[0 .. 3], row q starting
+ *   after the draws of rows 0 .. q-1 and *d_position draws in; *d_position is advanced by the batch's draws, so a
+ *   batch split into calls continues one stream, and the caller reads the total from it once.
+ * d_jump: lk_stochastic_jump_words() u64, built by the caller: entries 0..32 are (M^j, G_j) and entries 33..96 are
+ *   (M^(2^t), G_(2^t)), each as (mul_hi, mul_lo, add_hi, add_lo), where G_j = sum_{k<j} M^k: j steps take s to
+ *   M^j s + G_j inc (mod 2^128).
+ * n in 1..lk_topn_max(): rank mode, argtopn over the keys with the valid positions offered in list order
+ *   (topn_heap.cuh's contract): d_out_idx [B][n] positions (-1 padding), d_out_val [B][n] the original scores (NaN
+ *   padding), d_out_key [B][n] the keys (NaN padding; may be NULL), d_out_cnt [B] the list lengths.
+ * n == 0: key mode, d_keys [B][n_items] row-major, the key of every valid position and NaN elsewhere; d_out_cnt [B]
+ *   the valid counts.
+ * The workspace is lk_stochastic_workspace_bytes(B, n_items, transform) bytes: 20 per row, plus 4 * B * n_items for
+ * the compacted values that softmax and linear sum.  Callers split large batches to bound it.
+ * ---------------------------------------------------------------------- */
+#define LK_STOCH_NONE 0
+#define LK_STOCH_SOFTMAX 1
+#define LK_STOCH_LINEAR 2
+#define LK_STOCH_JUMP_WORDS (4 * (33 + 64))
+
+typedef struct lk_stochastic_args {
+    int32_t n_queries, n_items;        /* B rows of n_items positions (n_items < 2^31 - 64) */
+    const float *d_scores;
+    int64_t row_stride, item_stride;   /* in elements */
+    const int64_t *d_excl_indptr;      /* [B + 1] or NULL */
+    const int32_t *d_excl_items;
+    int32_t transform;                 /* LK_STOCH_* */
+    float scale;
+    int32_t shared_stream;             /* 0: a state per row, 1: one stream through the rows */
+    int32_t n;                         /* 0: key mode, 1..lk_topn_max(): rank mode */
+    const uint64_t *d_state;           /* [B][4], or [1][4] with shared_stream */
+    const uint64_t *d_jump;            /* [LK_STOCH_JUMP_WORDS] */
+    int64_t *d_position;               /* shared_stream: [1] in/out, draws consumed */
+    void *d_workspace;
+    int64_t workspace_bytes;
+    int32_t *d_out_idx;                /* rank mode [B][n] */
+    float *d_out_val;                  /* rank mode [B][n] */
+    double *d_out_key;                 /* rank mode [B][n], or NULL */
+    int32_t *d_out_cnt;                /* [B] */
+    double *d_keys;                    /* key mode [B][n_items] */
+} lk_stochastic_args;
+
+LK_API int64_t lk_stochastic_workspace_bytes(int64_t n_queries, int64_t n_items, int32_t transform);
+LK_API int lk_stochastic_topn(const lk_stochastic_args *args, void *stream);
 
 #ifdef __cplusplus
 }

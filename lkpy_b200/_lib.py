@@ -20,6 +20,8 @@ LK_MAX_REPLICAS = 8
 LK_COOC_COUNT, LK_ASSOC_PROBABILITY, LK_ASSOC_LIFT = 0, 1, 2
 LK_FLEXMF_LOGISTIC, LK_FLEXMF_PAIRWISE, LK_FLEXMF_MSE = 0, 1, 2
 LK_FLEXMF_REG_NONE, LK_FLEXMF_REG_L2, LK_FLEXMF_REG_ADAMW = 0, 1, 2
+LK_STOCH_NONE, LK_STOCH_SOFTMAX, LK_STOCH_LINEAR = 0, 1, 2
+LK_STOCH_JUMP_WORDS = 4 * (33 + 64)
 
 i32p = C.POINTER(C.c_int32)
 i64p = C.POINTER(C.c_int64)
@@ -438,6 +440,32 @@ class LkOffsetScoreArgs(C.Structure):
     ]
 
 
+class LkStochasticArgs(C.Structure):
+    _fields_ = [
+        ("n_queries", C.c_int32),
+        ("n_items", C.c_int32),
+        ("d_scores", vp),
+        ("row_stride", C.c_int64),
+        ("item_stride", C.c_int64),
+        ("d_excl_indptr", vp),
+        ("d_excl_items", vp),
+        ("transform", C.c_int32),
+        ("scale", C.c_float),
+        ("shared_stream", C.c_int32),
+        ("n", C.c_int32),
+        ("d_state", vp),
+        ("d_jump", vp),
+        ("d_position", vp),
+        ("d_workspace", vp),
+        ("workspace_bytes", C.c_int64),
+        ("d_out_idx", vp),
+        ("d_out_val", vp),
+        ("d_out_key", vp),
+        ("d_out_cnt", vp),
+        ("d_keys", vp),
+    ]
+
+
 #: every symbol ``include/lkpy_b200.h`` declares: name -> (restype, argtypes)
 SYMBOLS: dict[str, tuple] = {
     "lk_version": (C.c_int, []),
@@ -493,6 +521,8 @@ SYMBOLS: dict[str, tuple] = {
     "lk_bias_learn_workspace_bytes": (C.c_int64, []),
     "lk_bias_learn": (C.c_int, [C.POINTER(LkBiasLearnArgs), vp]),
     "lk_offset_score_batch": (C.c_int, [C.POINTER(LkOffsetScoreArgs), vp]),
+    "lk_stochastic_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64, C.c_int32]),
+    "lk_stochastic_topn": (C.c_int, [C.POINTER(LkStochasticArgs), vp]),
 }
 
 _lib = None

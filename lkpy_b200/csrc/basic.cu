@@ -30,30 +30,15 @@ constexpr int MEAN_THREADS = 256;
 constexpr int BIAS_THREADS = 256;   // 8 warps, one entity each at a time
 constexpr int BIAS_CHUNKS = 4;      // 32-value chunks each lane holds: 128 values per step of the chain
 
-// Descend the mean's pairwise tree (over r[0 .. nnz)) along the d leading bits of path p.  Returns false when the
-// path runs into a leaf above depth d with path bits left that are not all zero: no such node exists.  A node at
-// depth d with path p keeps its value in slot p << (MEAN_DEPTH - d).
-__device__ __forceinline__ bool mean_node(const int64_t nnz, const int d, const uint32_t p, int64_t &lo, int64_t &n)
-{
-    lo = 0, n = nnz;
-    for (int k = 0; k < d; k++) {
-        if (n <= 128) return (p & ((1u << (d - k)) - 1u)) == 0u;
-        const int64_t n2 = pairwise_split(n);
-        if ((p >> (d - 1 - k)) & 1u)
-            lo += n2, n -= n2;
-        else
-            n = n2;
-    }
-    return true;
-}
-
+// The mean's pairwise tree over r[0 .. nnz) is cut at MEAN_DEPTH (pairwise_node): a node at depth d with path p
+// keeps its value in slot p << (MEAN_DEPTH - d).
 __global__ void __launch_bounds__(MEAN_THREADS) mean_subtrees_kernel(const float *__restrict__ r, const int64_t nnz,
                                                                      float *__restrict__ part)
 {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (1u << MEAN_DEPTH)) return;
     int64_t lo, n;
-    if (!mean_node(nnz, MEAN_DEPTH, t, lo, n)) return;
+    if (!pairwise_node(nnz, MEAN_DEPTH, t, lo, n)) return;
     part[t] = pairwise_sum<F32Ops>([&](int64_t p) { return __ldg(r + p); }, lo, n);
 }
 
@@ -64,7 +49,7 @@ __global__ void __launch_bounds__(1024) mean_combine_kernel(const int64_t nnz, f
         for (int d = MEAN_DEPTH - 1; d >= 0; d--) {
             for (uint32_t p = threadIdx.x; p < (1u << d); p += blockDim.x) {
                 int64_t lo, n;
-                if (!mean_node(nnz, d, p, lo, n) || n <= 128) continue;  // absent, or a leaf: its slot is final
+                if (!pairwise_node(nnz, d, p, lo, n) || n <= 128) continue;  // absent, or a leaf: its slot is final
                 const uint32_t s = p << (MEAN_DEPTH - d);
                 part[s] = __fadd_rn(part[s], part[s + (1u << (MEAN_DEPTH - d - 1))]);
             }

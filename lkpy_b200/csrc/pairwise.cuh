@@ -1,5 +1,5 @@
-// pairwise.cuh — NumPy's float reduction order on the device, shared by prep.cu (per-column sums) and basic.cu
-// (the global mean of the bias model).
+// pairwise.cuh — NumPy's float reduction order on the device, shared by prep.cu (per-column sums), basic.cu
+// (the global mean of the bias model) and stochastic.cu (the softmax and linear normalisers).
 //
 // NumPy's reduction of a segment is first + pairwise(rest), where pairwise(a, n) adds sequentially for n < 8,
 // keeps eight interleaved partial sums for n <= 128 (combined as ((r0+r1)+(r2+r3)) + ((r4+r5)+(r6+r7)), then the
@@ -26,6 +26,25 @@ __host__ __device__ __forceinline__ int64_t pairwise_split(const int64_t n)
 {
     const int64_t n2 = n / 2;
     return n2 - n2 % 8;
+}
+
+// Descend the pairwise tree over n_total values along the d leading bits of path p (a set bit takes the right
+// child), giving the node's range [lo, lo + n).  Returns false when the path runs into a leaf above depth d with path
+// bits left that are not all zero: no such node exists.  Cutting the tree at depth d this way hands its 2^d subtrees
+// to parallel walkers (basic.cu's mean, stochastic.cu's normaliser).
+__host__ __device__ __forceinline__ bool pairwise_node(const int64_t n_total, const int d, const uint32_t p,
+                                                       int64_t &lo, int64_t &n)
+{
+    lo = 0, n = n_total;
+    for (int k = 0; k < d; k++) {
+        if (n <= 128) return (p & ((1u << (d - k)) - 1u)) == 0u;
+        const int64_t n2 = pairwise_split(n);
+        if ((p >> (d - 1 - k)) & 1u)
+            lo += n2, n -= n2;
+        else
+            n = n2;
+    }
+    return true;
 }
 
 // leaf of the pairwise tree (n <= 128)

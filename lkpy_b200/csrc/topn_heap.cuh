@@ -1,6 +1,6 @@
 // topn_heap.cuh — the one device copy of argtopn's indirect min-heap (src/accel/indirect/heap.rs,
 // src/accel/data/sorting.rs:131-170) and of its output contract, shared by every batched top-n kernel: topn.cu,
-// the ranking mode of knn_score.cu, als_recommend.cu, cooc.cu and ease.cu.
+// the ranking mode of knn_score.cu, als_recommend.cu, cooc.cu, ease.cu, basic.cu and stochastic.cu (f64 keys).
 //
 // The contract: candidates are offered in ascending item order, an excluded item counts as a NaN offer (never
 // accepted), and each query's row of n is written in descending score order, padded with -1 items and NaN scores,
@@ -8,8 +8,9 @@
 //
 // The heap is reached through a storage policy H so that each kernel keeps its own layout (per-thread local
 // arrays, shared memory, a strided workspace) and its own payload:
-//     typename H::Ent         the entry: a float score `v` and whatever rides along with it
-//     float H::val(int pos)   the score at pos
+//     typename H::Ent         the entry: a score `v` (float, or double for stochastic.cu's f64 keys) and whatever
+//                             rides along with it
+//     V     H::val(int pos)   the score at pos, of the type of `v`
 //     Ent   H::get(int pos)   the entry at pos
 //     void  H::put(int pos, Ent e)
 // Both sifts move a hole instead of swapping, which leaves exactly the arrangement the reference's swaps leave.
@@ -40,10 +41,10 @@ __device__ __forceinline__ void topn_heap_down(H &h, int pos, const int lim)
     const typename H::Ent e = h.get(pos);
     for (;;) {
         int mn = pos;
-        float mv = e.v;
+        auto mv = e.v;
         const int left = 2 * pos + 1, right = 2 * pos + 2;
         if (left < lim) {
-            const float lv = h.val(left);
+            const auto lv = h.val(left);
             if (lv < mv) {
                 mn = left;
                 mv = lv;
@@ -59,9 +60,9 @@ __device__ __forceinline__ void topn_heap_down(H &h, int pos, const int lim)
 
 // argtopn's offer of a non-NaN entry (the caller drops NaN, sorting.rs:142): heap.rs:41-45 push + upheap while
 // the heap has room, else heap.rs:46-52 replace the root if strictly greater and downheap.  `root` mirrors the
-// root's score once the heap holds an entry.
-template <class H>
-__device__ __forceinline__ void topn_heap_offer(H &h, int &count, float &root, const int n,
+// root's score once the heap holds an entry; V is the score type.
+template <class H, typename V>
+__device__ __forceinline__ void topn_heap_offer(H &h, int &count, V &root, const int n,
                                                 const typename H::Ent e)
 {
     if (count < n) {

@@ -20,7 +20,7 @@ from . import _lib
 from ._lib import (
     LkAlsArgs, LkAlsRecArgs, LkAssocScoreArgs, LkBiasLearnArgs, LkCoocArgs, LkEaseScoreArgs, LkFlexmfSampleArgs,
     LkFlexmfStepArgs, LkF32SeqSumArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkNmfCdSweepArgs,
-    LkOffsetScoreArgs, LkSlimArgs, LkSpmmArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr,
+    LkOffsetScoreArgs, LkSlimArgs, LkSpmmArgs, LkStochasticArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr,
 )  # fmt: skip
 from .data import InteractionCSR
 
@@ -2052,3 +2052,132 @@ def offset_scores(
         return S
     return _rank_launch(a, lib().lk_offset_score_batch, "lk_offset_score_batch", n, n_items, n_queries, dev,
                         excl_indptr, excl_items)  # fmt: skip
+
+
+# ---------------------------------------------------------------------------
+# stochastic top-n (StochasticTopNRanker)
+# ---------------------------------------------------------------------------
+
+#: NumPy's PCG64 multiplier (PCG_DEFAULT_MULTIPLIER_128)
+PCG64_MULT = 0x2360ED051FC65DA44385DF649FCCF645
+_M64, _M128 = (1 << 64) - 1, (1 << 128) - 1
+#: the bytes one split of a stochastic batch may take for its workspace, and in key mode for its key matrix
+STOCHASTIC_SPLIT_BYTES = 1 << 30
+_STOCH_TRANSFORMS = {None: _lib.LK_STOCH_NONE, "softmax": _lib.LK_STOCH_SOFTMAX, "linear": _lib.LK_STOCH_LINEAR}
+
+
+def pcg64_jump(j: int) -> tuple[int, int]:
+    """``(M^j, G_j) mod 2^128`` with ``G_j = sum(M^k for k < j)``: ``j`` PCG64 steps take a state ``s`` to
+    ``M^j s + G_j inc``.  Square-and-multiply on Python ints."""
+    mul, add, m, g = 1, 0, PCG64_MULT, 1
+    while j:
+        if j & 1:
+            mul, add = (m * mul) & _M128, (m * add + g) & _M128
+        m, g = (m * m) & _M128, (m * g + g) & _M128
+        j >>= 1
+    return mul, add
+
+
+def pcg64_words(state: int, inc: int) -> list[int]:
+    """A PCG64 ``(state, inc)`` as the four u64 words ``lk_stochastic_topn`` takes."""
+    return [state >> 64, state & _M64, inc >> 64, inc & _M64]
+
+
+def stochastic_jump_table() -> np.ndarray:
+    """``lk_stochastic_topn``'s ``d_jump``: ``(M^j, G_j)`` for j = 0..32, then for j = 2^t, t = 0..63."""
+    rows = [pcg64_jump(j) for j in range(33)] + [pcg64_jump(1 << t) for t in range(64)]
+    return np.array([pcg64_words(m, g) for m, g in rows], dtype=np.uint64).reshape(-1)
+
+
+_jump_tables: dict = {}
+
+
+def _device_jump_table(dev) -> torch.Tensor:
+    t = _jump_tables.get(dev)
+    if t is None:
+        t = _jump_tables[dev] = torch.from_numpy(stochastic_jump_table().view(np.int64)).to(dev)
+    return t
+
+
+def stochastic_topn(
+    scores: torch.Tensor, n: int | None, *, transform: str | None, scale: float, states: np.ndarray, shared: bool,
+    excl_indptr: torch.Tensor | None = None, excl_items: torch.Tensor | None = None, with_keys: bool = False,
+):  # fmt: skip
+    """
+    Plackett–Luce top-``n`` of every row of ``scores`` [B, L] (f32, any strides: a contiguous matrix or the
+    transpose of an item-major one) by exponential keys (``lk_stochastic_topn``, include/lkpy_b200.h has the
+    arithmetic).  Position i of row b is valid when its score is finite and it is not among
+    ``excl_items[excl_indptr[b]:excl_indptr[b+1]]`` (any order; repeats and out-of-range numbers are ignored).
+    ``states`` holds PCG64 states as u64 words ``[B, 4]`` (each row its own stream) or, with ``shared``, ``[1, 4]``
+    (one stream through the rows in order).
+
+    Returns ``(idx [B, w] int32 positions, -1 padding; val [B, w] f32 scores, NaN padding; key [B, w] f64 or None;
+    cnt [B] int32 list lengths; drawn)``, where ``w`` is ``n``, or ``L`` for ``n=None`` (every valid position) and
+    ``drawn`` a device int64 [1] holding the draws of a shared stream.  ``n`` in 1..``lk_topn_max()`` is the rank
+    mode; ``None`` and larger ``n`` take every key (key mode) and sort each row's keys on the device, truncated to
+    ``n``.  Equal keys may then come out in any order, as the reference's unstable sort allows.  Batches are split
+    so that each launch's workspace and keys stay within ``STOCHASTIC_SPLIT_BYTES``.
+    """
+    _lib.require_device()
+    if scores.dtype != torch.float32 or scores.dim() != 2:
+        raise TypeError("scores must be a 2-D float32 tensor")
+    if transform not in _STOCH_TRANSFORMS:
+        raise ValueError(f"unknown transform {transform!r}")
+    tcode = _STOCH_TRANSFORMS[transform]
+    dev = scores.device
+    B, L = scores.shape
+    if L > 2**31 - 65:
+        raise _lib.EngineError("stochastic ranking of 2**31 - 64 or more positions is not supported")
+    if n is not None and n < 1:
+        raise ValueError("n must be positive or None")
+    rank = n is not None and n <= int(lib().lk_topn_max())
+    width = n if rank else (L if n is None else min(n, L))
+    states = np.ascontiguousarray(states, dtype=np.uint64).reshape(-1, 4)
+    if states.shape[0] != (1 if shared else B):
+        raise ValueError(f"states must have {1 if shared else B} rows")
+    d_states = torch.from_numpy(states.view(np.int64)).to(dev)
+    drawn = torch.zeros(1, dtype=torch.int64, device=dev)
+    idx = torch.full((B, width), -1, dtype=torch.int32, device=dev)
+    val = torch.full((B, width), float("nan"), dtype=torch.float32, device=dev)
+    key = torch.full((B, width), float("nan"), dtype=torch.float64, device=dev) if with_keys or not rank else None
+    cnt = torch.zeros(max(B, 1), dtype=torch.int32, device=dev)
+    if B == 0 or L == 0:
+        return idx, val, key if with_keys else None, cnt[:B], drawn
+    if excl_indptr is not None:
+        excl_indptr, excl_items = _sorted_exclusions(excl_indptr, excl_items, L, B, dev)
+    per_row = int(lib().lk_stochastic_workspace_bytes(1, L, tcode)) + (0 if rank else 8 * L)
+    chunk = max(1, min(B, STOCHASTIC_SPLIT_BYTES // per_row))
+    ws_bytes = int(lib().lk_stochastic_workspace_bytes(chunk, L, tcode))
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    keys = None if rank else torch.empty((chunk, L), dtype=torch.float64, device=dev)
+    jump = _device_jump_table(dev)
+    for c0 in range(0, B, chunk):
+        c1 = min(B, c0 + chunk)
+        a = LkStochasticArgs()
+        a.n_queries, a.n_items = c1 - c0, L
+        a.d_scores, a.row_stride, a.item_stride = ptr(scores[c0:c1]), scores.stride(0), scores.stride(1)
+        if excl_indptr is not None:
+            a.d_excl_indptr, a.d_excl_items = ptr(excl_indptr[c0:]), ptr(excl_items)
+        a.transform, a.scale, a.shared_stream = tcode, float(scale), int(shared)
+        a.d_state, a.d_jump, a.d_position = ptr(d_states if shared else d_states[c0:c1]), ptr(jump), ptr(drawn)
+        a.d_workspace, a.workspace_bytes = ptr(ws), ws_bytes
+        a.d_out_cnt = ptr(cnt[c0:c1])
+        if rank:
+            a.n = n
+            a.d_out_idx, a.d_out_val = ptr(idx[c0:c1]), ptr(val[c0:c1])
+            a.d_out_key = ptr(key[c0:c1]) if with_keys else None
+        else:
+            a.n, a.d_keys = 0, ptr(keys)
+        check(lib().lk_stochastic_topn(C.byref(a), stream_ptr()), "lk_stochastic_topn")
+        if not rank:
+            # a sort of each row's keys, invalid positions (NaN) last; the valid count cuts the row
+            k = torch.nan_to_num(keys[: c1 - c0], nan=float("-inf"))
+            sk, order = torch.sort(k, dim=1, descending=True)
+            c = cnt[c0:c1].clamp(max=width)
+            keep = torch.arange(width, device=dev)[None, :] < c[:, None]
+            take = order[:, :width]
+            idx[c0:c1] = torch.where(keep, take, -1).to(torch.int32)
+            val[c0:c1] = torch.where(keep, scores[c0:c1].gather(1, take), float("nan"))
+            key[c0:c1] = torch.where(keep, sk[:, :width], float("nan"))
+            cnt[c0:c1] = c
+    return idx, val, key if with_keys else None, cnt[:B], drawn
