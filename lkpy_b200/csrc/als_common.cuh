@@ -51,11 +51,50 @@ __device__ __forceinline__ float dot4(float a0, float b0, float a1, float b1, fl
     return a0 * b0 + a1 * b1 + a2 * b2 + a3 * b3;
 }
 
+// Trailing update of one of chol_solve_warp's last two tiles, cc = KP - 16 (W = 4) or KP - 8 (W = 2).  Only its
+// N = KP - cc = 4 W rows i >= cc are below the diagonal, all in the last row group, so a whole-warp pass over
+// them would leave 16 or 24 lanes idle.  Here 8 / W lanes share each row, each updating W of the tile's 8
+// columns, and read the row's panel entries back from As (the panel step stored exactly the values it holds
+// in registers).  Every element gets the same two dot4 subtractions, in the same order, as in the general
+// tile loop, so the factor's bits do not change.  Rows above the tile are not touched: that part of the
+// upper triangle is never read.
+template <int KP, int W>
+__device__ __forceinline__ void chol_tile_shared(float *As, const int tid, const int j0, const int cc)
+{
+    constexpr int LDA = KP + 4, N = 4 * W;
+    static_assert(W == 2 || W == 4, "16 rows x 4 columns or 8 rows x 2 columns per lane pair / quad");
+    const int lane = tid & 31;
+    const int i = cc + lane % N, c0 = (lane / N) * W;
+    const float4 x0 = *reinterpret_cast<const float4 *>(As + i * LDA + j0);
+    const float4 x1 = *reinterpret_cast<const float4 *>(As + i * LDA + j0 + 4);
+    float *ap = As + i * LDA + cc + c0;
+    float a[W];
+    if constexpr (W == 4) {
+        const float4 v = *reinterpret_cast<const float4 *>(ap);
+        a[0] = v.x, a[1] = v.y, a[2] = v.z, a[3] = v.w;
+    } else {
+        const float2 v = *reinterpret_cast<const float2 *>(ap);
+        a[0] = v.x, a[1] = v.y;
+    }
+#pragma unroll
+    for (int c = 0; c < W; c++) {
+        const float4 l0 = *reinterpret_cast<const float4 *>(As + (cc + c0 + c) * LDA + j0);
+        const float4 l1 = *reinterpret_cast<const float4 *>(As + (cc + c0 + c) * LDA + j0 + 4);
+        a[c] -= dot4(x0.x, l0.x, x0.y, l0.y, x0.z, l0.z, x0.w, l0.w);
+        a[c] -= dot4(x1.x, l1.x, x1.y, l1.y, x1.z, l1.z, x1.w, l1.w);
+    }
+    if constexpr (W == 4)
+        *reinterpret_cast<float4 *>(ap) = make_float4(a[0], a[1], a[2], a[3]);
+    else
+        *reinterpret_cast<float2 *>(ap) = make_float2(a[0], a[1]);
+}
+
 // One-warp systems (KP = 32, 64): the chol_solve contract below with 8-column panels.  Every lane
 // factors the 8x8 diagonal block redundantly from broadcast reads, then solves the panel entries of its
 // rows t and t + 32 into registers (x[q][0..7]), applies them to its right-hand side and updates the
 // trailing matrix in tiles 8 columns wide, so each trailing element is read and written once per 8
-// columns of the factor instead of once per 4.
+// columns of the factor instead of once per 4.  The last two tiles, which have only 16 and 8 rows in the
+// lower triangle, spread those rows' columns over the whole warp (chol_tile_shared).
 //
 // The arithmetic is that of 4-column panels, operation for operation: where the second half of a panel
 // (columns 4..7) meets the first, the first half's contribution is one dot4 subtracted before the second
@@ -161,7 +200,7 @@ __device__ __forceinline__ bool chol_solve_warp(float *As, float *ys, float *din
         // (i < cc) only touch the upper triangle, which is never read, so the update is applied without a
         // per-lane branch.
 #pragma unroll 2
-        for (int cc = j0 + P; cc < KP; cc += P) {
+        for (int cc = j0 + P; cc < KP - 2 * P; cc += P) {
             float4 L[P][2];
 #pragma unroll
             for (int c = 0; c < P; c++) {
@@ -186,6 +225,8 @@ __device__ __forceinline__ bool chol_solve_warp(float *As, float *ys, float *din
                 *reinterpret_cast<float4 *>(As + i * LDA + cc + 4) = a1;
             }
         }
+        if (j0 + P <= KP - 2 * P) chol_tile_shared<KP, 4>(As, tid, j0, KP - 2 * P);
+        if (j0 + P <= KP - P) chol_tile_shared<KP, 2>(As, tid, j0, KP - P);
         __syncwarp();
     }
 
