@@ -35,6 +35,8 @@
  *   StochasticTopNRanker.__call__ (_compute_keys + ItemList.top_n)
  *                                                 src/lenskit/stochastic/_ranker.py:89-156,
  *                                                 src/lenskit/data/_items.py:942-998 lk_stochastic_topn
+ *   FAIRReranker.__call__ (and TopNRanker + FAIRReranker)
+ *                                                 src/lenskit/reranking/fair.py      lk_fair_rerank
  *
  * Conventions
  *   - plain C: pointers and sizes only; no C++/torch types cross this boundary;
@@ -933,6 +935,50 @@ typedef struct lk_stochastic_args {
 
 LK_API int64_t lk_stochastic_workspace_bytes(int64_t n_queries, int64_t n_items, int32_t transform);
 LK_API int lk_stochastic_topn(const lk_stochastic_args *args, void *stream);
+
+/* ------------------------------------------------------------------------
+ * FA*IR re-ranking (fair.cu), behind FAIRReranker.__call__ (src/lenskit/reranking/fair.py).
+ *
+ * The merge of one ranked list of L positions with protected flags f[0 .. L) and a length len <= L: with P the
+ * queue of protected positions and U the queue of the others, both ascending, and c the protected count so far,
+ * for i = 0 .. len-1 take the head of P when c < d_m[i] and P is not empty, else the smaller head of P and U (the
+ * head of whichever is not empty).  Scores are never read by the merge.
+ *
+ * mode LK_FAIR_LISTS: B lists, list b the positions d_list_indptr[b] .. d_list_indptr[b+1] of d_list_protected
+ *   (one byte per position, nonzero = protected), merged to length d_list_len[b] (0 .. min(n, list length)).
+ *   Output: d_out_idx [B][n] the chosen positions within each list, -1 padding; d_out_cnt [B] = d_list_len.
+ * mode LK_FAIR_SCORES: B rows of n_items f32 scores at d_scores[q * row_stride + i * item_stride], one protected
+ *   byte per item (d_item_protected [n_items]), optional exclusions (d_excl_indptr [B + 1] and d_excl_items,
+ *   ascending and in range within each row, topn_excluded's semantics).  Each row's list is argtopn's top
+ *   n_candidates (1 .. lk_topn_max()) of its scores, an excluded item offered as NaN (topn_heap.cuh's contract),
+ *   and the merge runs over that list to length min(n, its length).  Output in argtopn's contract: d_out_idx [B][n]
+ *   item numbers (-1 padding), d_out_val [B][n] their scores (NaN padding; may be NULL), d_out_cnt [B].
+ * n in 1 .. lk_topn_max(); d_m holds at least n entries (the trained m_list).
+ * ---------------------------------------------------------------------- */
+#define LK_FAIR_LISTS 0
+#define LK_FAIR_SCORES 1
+
+typedef struct lk_fair_args {
+    int32_t mode;                      /* LK_FAIR_* */
+    int32_t n_queries;                 /* B */
+    int32_t n;                         /* output width, 1..lk_topn_max() */
+    int32_t n_candidates;              /* scores: N, 1..lk_topn_max() */
+    const int32_t *d_m;                /* [n] minimum protected counts of the prefixes 1..n */
+    const int64_t *d_list_indptr;      /* lists: [B + 1] */
+    const uint8_t *d_list_protected;   /* lists: one flag per position */
+    const int32_t *d_list_len;         /* lists: [B] output lengths */
+    int32_t n_items;                   /* scores */
+    const float *d_scores;             /* scores */
+    int64_t row_stride, item_stride;   /* scores, in elements */
+    const uint8_t *d_item_protected;   /* scores: [n_items] */
+    const int64_t *d_excl_indptr;      /* scores: [B + 1] or NULL */
+    const int32_t *d_excl_items;
+    int32_t *d_out_idx;                /* [B][n] */
+    float *d_out_val;                  /* scores: [B][n] or NULL */
+    int32_t *d_out_cnt;                /* [B] */
+} lk_fair_args;
+
+LK_API int lk_fair_rerank(const lk_fair_args *args, void *stream);
 
 #ifdef __cplusplus
 }

@@ -22,6 +22,7 @@ LK_FLEXMF_LOGISTIC, LK_FLEXMF_PAIRWISE, LK_FLEXMF_MSE = 0, 1, 2
 LK_FLEXMF_REG_NONE, LK_FLEXMF_REG_L2, LK_FLEXMF_REG_ADAMW = 0, 1, 2
 LK_STOCH_NONE, LK_STOCH_SOFTMAX, LK_STOCH_LINEAR = 0, 1, 2
 LK_STOCH_JUMP_WORDS = 4 * (33 + 64)
+LK_FAIR_LISTS, LK_FAIR_SCORES = 0, 1
 
 i32p = C.POINTER(C.c_int32)
 i64p = C.POINTER(C.c_int64)
@@ -466,6 +467,29 @@ class LkStochasticArgs(C.Structure):
     ]
 
 
+class LkFairArgs(C.Structure):
+    _fields_ = [
+        ("mode", C.c_int32),
+        ("n_queries", C.c_int32),
+        ("n", C.c_int32),
+        ("n_candidates", C.c_int32),
+        ("d_m", vp),
+        ("d_list_indptr", vp),
+        ("d_list_protected", vp),
+        ("d_list_len", vp),
+        ("n_items", C.c_int32),
+        ("d_scores", vp),
+        ("row_stride", C.c_int64),
+        ("item_stride", C.c_int64),
+        ("d_item_protected", vp),
+        ("d_excl_indptr", vp),
+        ("d_excl_items", vp),
+        ("d_out_idx", vp),
+        ("d_out_val", vp),
+        ("d_out_cnt", vp),
+    ]
+
+
 #: every symbol ``include/lkpy_b200.h`` declares: name -> (restype, argtypes)
 SYMBOLS: dict[str, tuple] = {
     "lk_version": (C.c_int, []),
@@ -523,6 +547,7 @@ SYMBOLS: dict[str, tuple] = {
     "lk_offset_score_batch": (C.c_int, [C.POINTER(LkOffsetScoreArgs), vp]),
     "lk_stochastic_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64, C.c_int32]),
     "lk_stochastic_topn": (C.c_int, [C.POINTER(LkStochasticArgs), vp]),
+    "lk_fair_rerank": (C.c_int, [C.POINTER(LkFairArgs), vp]),
 }
 
 _lib = None

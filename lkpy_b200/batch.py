@@ -28,6 +28,17 @@ def empty_list(vocabulary) -> ItemList:
     )  # fmt: skip
 
 
+def take(items: ItemList, pos: np.ndarray, *, ordered: bool | None = None, **extra) -> ItemList:
+    """The entries ``pos`` of ``items``, with every field, plus ``extra`` fields."""
+    fields = {k: v[pos] for k, v in items._fields.items()}
+    fields.update(extra)
+    scores = fields.pop("score", None)
+    return ItemList(
+        item_ids=None if items._ids is None else items._ids[pos], item_nums=None if items._nums is None else items._nums[pos],
+        vocabulary=items._vocab, scores=scores, ordered=ordered, **fields,
+    )  # fmt: skip
+
+
 def rank_size(n: int, n_items: int) -> int:
     """The list length a kernel is asked for: ``min(n, n_items)``, or 0 when every list is empty.  Raises
     ``ValueError`` past the engine limit ``lk_topn_max()``."""

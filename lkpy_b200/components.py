@@ -73,11 +73,15 @@ class Vocabulary:
 
 
 class ItemList:
-    """Items identified by id and/or number, with named fields (``rating``, ``score`` …)."""
+    """Items identified by id and/or number, with named fields (``rating``, ``score`` …).  ``ordered`` marks a
+    ranked list; a copy keeps its source's flag unless given one."""
 
     def __init__(self, items=None, *, item_ids=None, item_nums=None, vocabulary: Vocabulary | None = None,
-                 scores=None, **fields):
+                 scores=None, ordered: bool | None = None, **fields):
+        self.ordered = bool(ordered)
         if isinstance(items, ItemList):
+            if ordered is None:
+                self.ordered = items.ordered
             item_ids, item_nums = items._ids, items._nums
             vocabulary = vocabulary or items._vocab
             base = dict(items._fields)
@@ -225,11 +229,13 @@ class UsesTrainer(Trainable):
 
 @dataclass
 class Dataset:
-    """The slice of ``lenskit.data.Dataset`` the two scorers use."""
+    """The slice of ``lenskit.data.Dataset`` the two scorers use, plus optional per-item attributes (name -> one
+    value per item of ``items``, in vocabulary order), which ``FAIRReranker`` reads its protected flags from."""
 
     interactions: Any  # lkpy_b200.data.Interactions
     users: Vocabulary = field(default=None)  # type: ignore[assignment]
     items: Vocabulary = field(default=None)  # type: ignore[assignment]
+    item_attributes: dict[str, Any] = field(default_factory=dict)
 
     def __post_init__(self):
         it = self.interactions

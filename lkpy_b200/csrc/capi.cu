@@ -64,7 +64,7 @@ int sm_count()
 
 extern "C" {
 
-int lk_version(void) { return 113; }
+int lk_version(void) { return 114; }
 
 const char *lk_last_error(void) { return lk::g_err; }
 

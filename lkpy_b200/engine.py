@@ -20,7 +20,8 @@ from . import _lib
 from ._lib import (
     LkAlsArgs, LkAlsRecArgs, LkAssocScoreArgs, LkBiasLearnArgs, LkCoocArgs, LkEaseScoreArgs, LkFlexmfSampleArgs,
     LkFlexmfStepArgs, LkF32SeqSumArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkNmfCdSweepArgs,
-    LkOffsetScoreArgs, LkSlimArgs, LkSpmmArgs, LkStochasticArgs, LkUknnSearchArgs, check, lib, ptr, stream_ptr,
+    LkFairArgs, LkOffsetScoreArgs, LkSlimArgs, LkSpmmArgs, LkStochasticArgs, LkUknnSearchArgs, check, lib, ptr,
+    stream_ptr,
 )  # fmt: skip
 from .data import InteractionCSR
 
@@ -2181,3 +2182,78 @@ def stochastic_topn(
             key[c0:c1] = torch.where(keep, sk[:, :width], float("nan"))
             cnt[c0:c1] = c
     return idx, val, key if with_keys else None, cnt[:B], drawn
+
+
+# ---------------------------------------------------------------------------
+# FA*IR re-ranking (FAIRReranker)
+# ---------------------------------------------------------------------------
+
+
+def fair_rerank(
+    m: np.ndarray, n: int, protected, *, indptr=None, lengths=None, scores: torch.Tensor | None = None,
+    candidates: int | None = None, excl_indptr: torch.Tensor | None = None, excl_items: torch.Tensor | None = None,
+):  # fmt: skip
+    """
+    The FA*IR merge (``lk_fair_rerank``; include/lkpy_b200.h states it) of a batch, to at most ``n`` entries
+    (1..``lk_topn_max()``) under the minimum protected counts ``m`` (the trained ``m_list``, at least ``n`` entries).
+
+    * Lists: ``indptr`` [B + 1] offsets into ``protected`` (one bool per position of the concatenated lists) and
+      ``lengths`` [B], each list's output length (at most ``n`` and its list length).  Returns ``(idx [B, n] int32
+      positions within each list, -1 padding; None; cnt [B] int32)``.
+    * Scores: ``scores`` [B, n_items] f32 on the device (any strides), ``protected`` one bool per item, and
+      ``candidates`` N (1..``lk_topn_max()``): each row's list is argtopn's top N, the items
+      ``excl_items[excl_indptr[b]:excl_indptr[b+1]]`` (any order; repeats and out-of-range numbers are ignored)
+      offered as NaN, and is merged to ``min(n, its length)``.  Returns ``(idx [B, n] int32 item numbers, -1
+      padding; val [B, n] f32 scores, NaN padding; cnt [B] int32)``.
+    """
+    dev = _lib.require_device()
+    n = _check_topn(n)
+    m = np.asarray(m, dtype=np.int64)
+    if m.ndim != 1 or len(m) < n:
+        raise ValueError(f"m must hold at least n={n} entries")
+    a = LkFairArgs()
+    if scores is not None:
+        if scores.dtype != torch.float32 or scores.dim() != 2:
+            raise TypeError("scores must be a 2-D float32 tensor")
+        if candidates is None or not 1 <= int(candidates) <= int(lib().lk_topn_max()):
+            raise ValueError(f"candidates must be in 1..{int(lib().lk_topn_max())}")
+        dev = scores.device
+        B, L = scores.shape
+        if L > 2**31 - 33:
+            raise _lib.EngineError("re-ranking from 2**31 - 32 or more items is not supported")
+        prot = torch.as_tensor(np.asarray(protected, dtype=bool).view(np.uint8)).to(dev)
+        if prot.numel() != L:
+            raise ValueError(f"protected must have one flag per item ({L})")
+        a.mode, a.n_candidates, a.n_items = _lib.LK_FAIR_SCORES, int(candidates), L
+        a.d_scores, a.row_stride, a.item_stride = ptr(scores), scores.stride(0), scores.stride(1)
+        a.d_item_protected = ptr(prot)
+        val = torch.full((B, n), float("nan"), dtype=torch.float32, device=dev)
+        a.d_out_val = ptr(val)
+        if excl_indptr is not None and B > 0:
+            excl_indptr, excl_items = _sorted_exclusions(excl_indptr, excl_items, L, B, dev)
+            a.d_excl_indptr, a.d_excl_items = ptr(excl_indptr), ptr(excl_items)
+    else:
+        indptr = np.asarray(indptr, dtype=np.int64)
+        lengths = np.asarray(lengths, dtype=np.int32)
+        flags = np.asarray(protected, dtype=bool)
+        B = len(indptr) - 1
+        if B < 0 or len(lengths) != B or indptr[0] != 0 or np.any(np.diff(indptr) < 0) or indptr[-1] != len(flags):
+            raise ValueError("indptr must be B + 1 ascending offsets from 0 to the flag count, with B lengths")
+        if np.any(np.diff(indptr) >= 2**31 - 32):
+            raise _lib.EngineError("lists of 2**31 - 32 or more positions are not supported")
+        if np.any(lengths < 0) or np.any(lengths > np.minimum(np.diff(indptr), n)):
+            raise ValueError("each length must be in 0..min(n, its list length)")
+        d_indptr = torch.from_numpy(indptr).to(dev)
+        d_flags = torch.from_numpy(np.concatenate([flags.view(np.uint8), np.zeros(1, np.uint8)])).to(dev)
+        d_len = torch.from_numpy(lengths).to(dev)
+        a.mode, a.d_list_indptr, a.d_list_protected, a.d_list_len = _lib.LK_FAIR_LISTS, ptr(d_indptr), ptr(d_flags), ptr(d_len)
+        val = None
+    idx = torch.full((B, n), -1, dtype=torch.int32, device=dev)
+    cnt = torch.zeros(max(B, 1), dtype=torch.int32, device=dev)
+    if B == 0 or (scores is not None and scores.shape[1] == 0):
+        return idx, val, cnt[:B]
+    d_m = torch.from_numpy(m[:n].astype(np.int32)).to(dev)
+    a.n_queries, a.n, a.d_m = B, n, ptr(d_m)
+    a.d_out_idx, a.d_out_cnt = ptr(idx), ptr(cnt)
+    check(lib().lk_fair_rerank(C.byref(a), stream_ptr()), "lk_fair_rerank")
+    return idx, val, cnt[:B]

@@ -32,7 +32,7 @@ from numpy.random import SeedSequence, default_rng
 from pydantic import BaseModel
 
 from . import _lib, engine
-from .batch import check_exclude, history_csr
+from .batch import check_exclude, history_csr, take
 from .components import Component, ItemList, RecQuery
 
 #: a configured seed: an int, a sequence of ints or None
@@ -141,17 +141,6 @@ def advance(gen: np.random.Generator, draws: int) -> None:
 # ---------------------------------------------------------------------------
 
 
-def _take(items: ItemList, pos: np.ndarray, **extra) -> ItemList:
-    """The entries ``pos`` of ``items``, with every field, plus ``extra`` fields."""
-    fields = {k: v[pos] for k, v in items._fields.items()}
-    fields.update(extra)
-    scores = fields.pop("score", None)
-    return ItemList(
-        item_ids=None if items._ids is None else items._ids[pos], item_nums=None if items._nums is None else items._nums[pos],
-        vocabulary=items._vocab, scores=scores, **fields,
-    )  # fmt: skip
-
-
 class StochasticTopNRanker(Component):
     """
     ``StochasticTopNRanker``: ``__call__(items, query, n)`` samples a ranking of the list's valid items.
@@ -224,7 +213,7 @@ class StochasticTopNRanker(Component):
         for b, items in enumerate(lists):
             c = int(cnt[b])
             extra = {"weight": key[b, :c].copy()} if include_weights else {}
-            out.append(_take(items, idx[b, :c].astype(np.int64), **extra))
+            out.append(take(items, idx[b, :c].astype(np.int64), **extra))
         return out
 
     def rank_scores(self, scores: torch.Tensor, queries, vocabulary, n: int | None = None, *,
