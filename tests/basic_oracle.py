@@ -3,6 +3,8 @@ Host restatements for the bias model and the offset scorers (tests/test_basic*.p
 
 * NumPy's pairwise f32 sum, and the global mean the way ``lk_bias_learn`` evaluates it — the tree cut at
   ``MEAN_DEPTH``, each subtree summed on its own, the inner nodes above combined level by level;
+* ratings on which the order of the learner's entity chains shows in the f32 biases, and the count of biases a
+  reversed chain changes;
 * ``BiasModel.compute_for_items`` (basic/bias.py), statement for statement, for one query: the user bias of its rated
   items (the oracle of ``basic.BiasModel.user_bias_for_items``) and the scores;
 * the host composition a batched ranking must reproduce: scores, exclusions as NaN, ``argtopn``.
@@ -85,6 +87,54 @@ def kernel_mean(r: np.ndarray) -> np.float32:
                 part[s] = np.float32(part[s] + part[s + (1 << (MEAN_DEPTH - d - 1))])
     total = np.float32(np.float32(0.0) + part[0])  # np.add.reduce starts from the identity
     return np.float32(np.float64(total) / np.float64(nnz))
+
+
+def cancelling_ratings(it, rng: np.random.Generator, big: float = 2.0**36) -> np.ndarray:
+    """``it.ratings`` with ``+big`` and ``-big`` added along 4-cycles of the rating matrix, in f32: for every item
+    with two raters (u, v) who also rated the most rated item H, ``+big`` at (u, i) and (v, H), ``-big`` at
+    (v, i) and (u, H) (the pair is drawn with ``rng``).  Every item's and every user's additions sum to zero, so a
+    bias stays small while the partial sums of its chain pass through +-big.  There an f64 add rounds the
+    ratings' low bits, and which ratings are rounded depends on the order of the chain.  A cell that gets an
+    addition holds a multiple of ``big`` exactly (the rating is lost in f32)."""
+    H = int(np.argmax(np.bincount(it.items, minlength=it.n_items)))
+    h_pos = np.full(it.n_users, -1, np.int64)
+    on_h = np.flatnonzero(it.items == H)
+    h_pos[it.users[on_h]] = on_h
+    cand = np.flatnonzero((it.items != H) & (h_pos[it.users] >= 0))
+    cand = cand[rng.permutation(len(cand))]
+    cand = cand[np.argsort(it.items[cand], kind="stable")]  # each item's candidates in a random order
+    first = np.flatnonzero(np.concatenate([[True], it.items[cand[1:]] != it.items[cand[:-1]]]))
+    two = np.diff(np.append(first, len(cand))) >= 2
+    a, b = cand[first[two]], cand[first[two] + 1]
+    d = np.zeros(it.nnz)
+    np.add.at(d, a, big)
+    np.add.at(d, b, -big)
+    np.add.at(d, h_pos[it.users[a]], -big)
+    np.add.at(d, h_pos[it.users[b]], big)
+    return (np.asarray(it.ratings, np.float64) + d).astype(np.float32)
+
+
+def reversed_chain_changes(it, centered_dtype) -> tuple[int, int]:
+    """How many f32 item biases and f32 user biases of ``BiasModel.learn`` (damping 0, both entities) change bits
+    when each entity's ``np.add.at`` chain runs in reverse COO order: ``(items, users)``.  These are the values
+    the tests compare, so a count above zero means that a pass adding that entity's values out of order gives
+    other output on ``it``.  The user values of both orders are centred by the forward item biases, so the user
+    count is the user pass's own."""
+    c = it.ratings.astype(centered_dtype) - float(np.mean(it.ratings))
+    changed, ib = [], None
+    for idx, n in ((it.items, it.n_items), (it.users, it.n_users)):
+        vals = c if ib is None else c - ib[it.items]
+        counts = np.bincount(idx, minlength=n).astype(np.float64)
+        biases = []
+        for order in (slice(None), slice(None, None, -1)):
+            sums = np.zeros(n)
+            np.add.at(sums, idx[order], vals[order])
+            out = np.zeros(n, dtype=np.float32)
+            np.divide(sums, counts, out=out, where=counts > 0, casting="unsafe")
+            biases.append(out)
+        changed.append(int((biases[0].view(np.int32) != biases[1].view(np.int32)).sum()))
+        ib = biases[0]
+    return changed[0], changed[1]
 
 
 def bias_scores(model, users, items, query, targets) -> np.ndarray:

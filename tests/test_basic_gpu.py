@@ -4,6 +4,7 @@ BiasScorer and PopScorer on the device: ``lk_bias_learn`` bit for bit against th
 ``argtopn``), and the trained scorers against the recordings of the reference's own classes.
 """
 
+import math
 import pickle
 
 import numpy as np
@@ -40,6 +41,18 @@ def skewed():
     return Interactions(users, items, r, n_users, n_items)
 
 
+@pytest.fixture(scope="module")
+def cancelling(skewed):
+    """``skewed``'s users and items with ``bo.cancelling_ratings``: the learner input on which the order of the
+    entity chains shows in the f32 biases, with f64 and with f32 centring."""
+    it = Interactions(skewed.users, skewed.items, bo.cancelling_ratings(skewed, np.random.default_rng(8)),
+                      skewed.n_users, skewed.n_items)  # fmt: skip
+    for dtype in (np.float64, np.float32):
+        items_changed, users_changed = bo.reversed_chain_changes(it, dtype)
+        assert items_changed > 1000 and users_changed > 1000, (dtype, items_changed, users_changed)
+    return it
+
+
 def check_same(dev: BiasModel, host: BiasModel) -> None:
     assert dev.global_bias == host.global_bias and dev.damping == host.damping
     for a, b in ((dev.item_biases, host.item_biases), (dev.user_biases, host.user_biases)):
@@ -51,7 +64,7 @@ def check_same(dev: BiasModel, host: BiasModel) -> None:
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
 @pytest.mark.parametrize("damping", DAMPINGS, ids=str)
 @pytest.mark.parametrize("entities", ENTITIES, ids="+".join)
-@pytest.mark.parametrize("which", ["ml_small", "skewed"])
+@pytest.mark.parametrize("which", ["ml_small", "skewed", "cancelling"])
 def test_learn_is_the_host_statements(request, which, entities, damping, dtype):
     it = request.getfixturevalue(which)
     dev = basic.learn(Dataset(it), damping, entities=set(entities), centered_dtype=dtype)
@@ -59,15 +72,37 @@ def test_learn_is_the_host_statements(request, which, entities, damping, dtype):
     check_same(dev, BiasModel.learn(it, pair, dtype, entities))
 
 
-@pytest.mark.parametrize("n", [1, 8, 9, 128, 129, 2**20 + 3])
+@pytest.mark.parametrize("n", [1, 8, 9, 128, 129, 2**20 + 3, 2**23, 2**23 + 8, 25_000_095, 2**27 + 3])
 def test_learn_mean_on_awkward_lengths(n):
+    """Up to 2^20 + 3 every depth-16 subtree is a leaf reached at depth 13 or above.  At 2^23 each of the 2^16
+    subtrees holds exactly 128 values; at 2^23 + 8 some walkers recurse one level; 25,000,095 is the benchmark's
+    count; at 2^27 + 3 every walker recurses four levels or more, and every combine level has inner nodes.
+
+    The ratings are halves with a noise term and a random sign.  With positive ratings only, the total is so much
+    larger than the rounding of the partial sums that every order gives the same bits; with signs the total is a
+    small difference of large partial sums, and the exact sum rounded once differs from NumPy's."""
     rng = np.random.default_rng(n)
     users = np.sort(rng.integers(0, max(n // 50, 1), n)).astype(np.int32)
     items = rng.integers(0, 1000, n).astype(np.int32)
     r = (rng.integers(1, 11, n) * 0.5 + rng.standard_normal(n) * 0.01).astype(np.float32)
+    r = np.where(rng.random(n) < 0.5, -r, r)
     it = Interactions(users, items, r, int(users.max()) + 1, 1000)  # COO order by user is all the mean needs
     m = basic.learn(Dataset(it), 0.0, entities=set())
-    assert np.float32(m.global_bias).view(np.int32) == np.mean(r).view(np.int32)
+    want = np.mean(r)
+    assert np.float32(m.global_bias).view(np.int32) == want.view(np.int32)
+    if n >= 2**20:
+        # the input tells summation orders apart: the exact sum rounded once gives other bits
+        exact = np.float32(np.float64(np.float32(math.fsum(r.astype(np.float64)))) / n)
+        assert exact.view(np.int32) != want.view(np.int32)
+    if n >= 2**23:
+        sizes = np.array([bo.mean_node(n, bo.MEAN_DEPTH, p)[1] for p in range(1 << bo.MEAN_DEPTH)])
+        assert sizes.sum() == n
+        if n == 2**23:
+            assert (sizes == 128).all()
+        else:
+            assert sizes.max() > 128  # the walkers' pairwise sums recurse
+        if n >= 2**27:
+            assert sizes.min() >= 2048  # four levels or more below the cut
 
 
 def trained_bias(ml_small, **cfg) -> BiasScorer:
