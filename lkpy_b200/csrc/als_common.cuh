@@ -436,12 +436,24 @@ __device__ __forceinline__ bool chol_solve(float *As, float *ys, float *dinv, co
     return bad;
 }
 
+// The entries of `this` row that thread tid writes back, for write_row's x_old.  The k = 64 tensor-core kernel
+// reads them before its Cholesky, so that the global load's latency overlaps the solve instead of following it;
+// nothing else writes the row while the CTA solves it.
+template <int KP, int NW>
+__device__ __forceinline__ void read_old_row(const float *thisrow, const int k, const int tid, float (&xold)[KP / (NW * 32)])
+{
+    constexpr int NT = NW * 32;
+#pragma unroll
+    for (int q = 0; q < KP / NT; q++) xold[q] = tid + q * NT < k ? thisrow[tid + q * NT] : 0.0f;
+}
+
 // Write x (in ys) to the row of `this` (and its replicas on peer GPUs) and add
 // |x - x_old|^2 to the delta accumulator; a failed solve leaves the row
-// untouched and records the row in the status word.
+// untouched and records the row in the status word.  x_old is read from the
+// row here, or comes from read_old_row when the kernel read it earlier (xold).
 template <int KP, int NW>
 __device__ __forceinline__ void write_row(const lk_als_args &a, const int row, float *thisrow,
-                                          const float *ys, const int tid, bool bad)
+                                          const float *ys, const int tid, bool bad, const float *xold = nullptr)
 {
     constexpr int NT = NW * 32;
     constexpr int RPT = KP / NT;
@@ -461,7 +473,7 @@ __device__ __forceinline__ void write_row(const lk_als_args &a, const int row, f
         const int i = tid + q * NT;
         if (i < k) {
             const float xn = ys[i];
-            const float d = xn - thisrow[i];
+            const float d = xn - (xold ? xold[q] : thisrow[i]);
             d2 = fmaf(d, d, d2);
             thisrow[i] = xn;
             for (int r = 0; r < a.n_replicas; r++)

@@ -410,8 +410,10 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
         cta_sync<NW>();
 
         // ---- Cholesky + triangular solves in shared memory, then write the row
+        float xold[C::RPT];
+        read_old_row<KP, NW>(thisrow, k, tid, xold);
         const bool bad = chol_solve<KP, NW>(As, ys, dinv, tid);
-        write_row<KP, NW>(a, row, thisrow, ys, tid, bad);
+        write_row<KP, NW>(a, row, thisrow, ys, tid, bad, xold);
         // the next chunk's bulk copies (async proxy) overwrite this buffer
         fence_proxy_async();
         __syncthreads();
