@@ -27,6 +27,41 @@ struct AlsCfg {
     static constexpr int OCC = KP >= 128 ? 3 : 12;
 };
 
+// System layouts of the one-warp solve (KP = 32, 64).  Row-major (FOLD = false): row stride KP + 4.  Folded
+// (FOLD = true, the k = 64 bf16 uniform-confidence route, where the smaller buffer buys residency; the address
+// arithmetic costs the other routes more than they would gain): only the lower 8 x 8 blocks are stored, the
+// diagonal blocks in full (36 blocks at KP = 64, 10 at KP = 32).  Block row b (rows 8 b .. 8 b + 7) has b + 1 blocks and block row
+// KP / 8 - 1 - b has KP / 8 - b, so the two share 8 physical rows of KP + 8 floats: the lower half of the block
+// rows at the start of each physical row, the upper half after its partner's blocks.  The physical rows are
+// CHOL_LD = KP + 12 floats apart, an odd number of 16-byte granules, so the eight rows that one quarter-warp's
+// float4 access touches lie in distinct banks (as the row-major stride KP + 4 did).  The rows of one block row are
+// consecutive physical rows, so (in both layouts) row 8 b + r is chol_off(8 b, jb) + r * CHOL_LD with a
+// compile-time stride, and a row's blocks are contiguous: element (i, j) is at chol_off(i, 0) + j for every
+// j < 8 (i / 8 + 1).  Returns the offset in floats of row i's 8-column block jb (jb <= i / 8 when folded).
+template <int KP, bool FOLD>
+constexpr int CHOL_LD = FOLD ? KP + 12 : KP + 4;
+
+template <int KP, bool FOLD>
+__host__ __device__ __forceinline__ constexpr int chol_off(int i, int jb)
+{
+    if constexpr (!FOLD) return i * CHOL_LD<KP, FOLD> + 8 * jb;
+    constexpr int NB = KP / 8;
+    const int b = i >> 3;
+    const bool low = b < NB / 2;
+    return ((low ? b : NB - 1 - b) * 8 + (i & 7)) * CHOL_LD<KP, FOLD> + 8 * (jb + (low ? 0 : NB - b));
+}
+
+// floats of the system buffer chol_solve<KP, NW, FOLD> factors
+template <int KP, bool FOLD>
+constexpr int SYS_FLOATS = FOLD ? KP / 2 * CHOL_LD<KP, FOLD> : KP * (KP + 4);
+
+// A[i][j] (j <= i, or j in the diagonal 8 x 8 block) in the system buffer chol_solve<KP, NW, FOLD> factors
+template <int KP, bool FOLD>
+__device__ __forceinline__ float *sys_at(float *As, int i, int j)
+{
+    return As + chol_off<KP, FOLD>(i, 0) + j;
+}
+
 template <int NW>
 __device__ __forceinline__ void cta_sync()
 {
@@ -57,17 +92,18 @@ __device__ __forceinline__ float dot4(float a0, float b0, float a1, float b1, fl
 // columns, and read the row's panel entries back from As (the panel step stored exactly the values it holds
 // in registers).  Every element gets the same two dot4 subtractions, in the same order, as in the general
 // tile loop, so the factor's bits do not change.  Rows above the tile are not touched: that part of the
-// upper triangle is never read.
-template <int KP, int W>
+// upper triangle is never read (and not stored when folded).
+template <int KP, int W, bool FOLD>
 __device__ __forceinline__ void chol_tile_shared(float *As, const int tid, const int j0, const int cc)
 {
-    constexpr int LDA = KP + 4, N = 4 * W;
+    constexpr int N = 4 * W;
     static_assert(W == 2 || W == 4, "16 rows x 4 columns or 8 rows x 2 columns per lane pair / quad");
     const int lane = tid & 31;
     const int i = cc + lane % N, c0 = (lane / N) * W;
-    const float4 x0 = *reinterpret_cast<const float4 *>(As + i * LDA + j0);
-    const float4 x1 = *reinterpret_cast<const float4 *>(As + i * LDA + j0 + 4);
-    float *ap = As + i * LDA + cc + c0;
+    const float *xi = As + chol_off<KP, FOLD>(i, j0 >> 3);
+    const float4 x0 = *reinterpret_cast<const float4 *>(xi);
+    const float4 x1 = *reinterpret_cast<const float4 *>(xi + 4);
+    float *ap = As + chol_off<KP, FOLD>(i, cc >> 3) + c0;
     float a[W];
     if constexpr (W == 4) {
         const float4 v = *reinterpret_cast<const float4 *>(ap);
@@ -78,8 +114,9 @@ __device__ __forceinline__ void chol_tile_shared(float *As, const int tid, const
     }
 #pragma unroll
     for (int c = 0; c < W; c++) {
-        const float4 l0 = *reinterpret_cast<const float4 *>(As + (cc + c0 + c) * LDA + j0);
-        const float4 l1 = *reinterpret_cast<const float4 *>(As + (cc + c0 + c) * LDA + j0 + 4);
+        const float *lc = As + chol_off<KP, FOLD>(cc + c0 + c, j0 >> 3);
+        const float4 l0 = *reinterpret_cast<const float4 *>(lc);
+        const float4 l1 = *reinterpret_cast<const float4 *>(lc + 4);
         a[c] -= dot4(x0.x, l0.x, x0.y, l0.y, x0.z, l0.z, x0.w, l0.w);
         a[c] -= dot4(x1.x, l1.x, x1.y, l1.y, x1.z, l1.z, x1.w, l1.w);
     }
@@ -102,27 +139,33 @@ __device__ __forceinline__ void chol_tile_shared(float *As, const int tid, const
 // trailing update subtracts the two halves' dot4s in turn, and the back substitution handles each 8-unknown
 // step as two 4-unknown ones.  So the factor, x and the status are bit-identical to a 4-column solve.  A
 // pivot row runs the same recurrence as the rows below it, which reproduces the broadcast factor's row
-// exactly (same operands in the same order); its entries right of the diagonal are stored as zero.
-template <int KP>
+// exactly (same operands in the same order); its entries right of the diagonal are stored as zero.  As holds
+// the system in the layout FOLD selects (chol_off); the rows of one block row are LD floats apart.
+template <int KP, bool FOLD>
 __device__ __forceinline__ bool chol_solve_warp(float *As, float *ys, float *dinv, const int tid)
 {
-    constexpr int LDA = KP + 4, RPT = KP / 32, P = 8;
+    constexpr int LD = CHOL_LD<KP, FOLD>, RPT = KP / 32, P = 8;
     static_assert(KP % P == 0 && RPT >= 1, "one warp, whole 8-column panels");
     bool bad = false;
     float yv[RPT];
 #pragma unroll
     for (int q = 0; q < RPT; q++) yv[q] = ys[tid + q * 32];
+    // where this lane's row i = tid + 32 q starts: folded, computed once; row-major, i * LD where it is used
+    int ro[RPT];
+#pragma unroll
+    for (int q = 0; q < RPT; q++) ro[q] = FOLD ? chol_off<KP, FOLD>(tid + q * 32, 0) : 0;
 
     for (int j0 = 0; j0 < KP; j0 += P) {
         // pivot block: rows j0..j0+7 of columns j0..j0+7, a diagonal block of the system (only its lower
         // triangle is used)
         float l[P][P], inv[P], z[P];
+        const float *pb = As + chol_off<KP, FOLD>(j0, j0 >> 3);  // the pivot block
 #pragma unroll
         for (int r = 0; r < P; r++)
 #pragma unroll
             for (int h = 0; h < 2; h++) {
                 if (4 * h > r) continue;
-                const float4 v = *reinterpret_cast<const float4 *>(As + (j0 + r) * LDA + j0 + 4 * h);
+                const float4 v = *reinterpret_cast<const float4 *>(pb + r * LD + 4 * h);
                 l[r][4 * h] = v.x, l[r][4 * h + 1] = v.y, l[r][4 * h + 2] = v.z, l[r][4 * h + 3] = v.w;
             }
         {
@@ -165,8 +208,9 @@ __device__ __forceinline__ bool chol_solve_warp(float *As, float *ys, float *din
 #pragma unroll
             for (int c = 0; c < P; c++) x[q][c] = 0.0f;
             if (i < j0) continue;
-            const float4 a0 = *reinterpret_cast<const float4 *>(As + i * LDA + j0);
-            const float4 a1 = *reinterpret_cast<const float4 *>(As + i * LDA + j0 + 4);
+            float *ai = As + (FOLD ? ro[q] : i * LD) + j0;
+            const float4 a0 = *reinterpret_cast<const float4 *>(ai);
+            const float4 a1 = *reinterpret_cast<const float4 *>(ai + 4);
             const float av[P] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
 #pragma unroll
             for (int c = 0; c < P; c++) {
@@ -191,42 +235,45 @@ __device__ __forceinline__ bool chol_solve_warp(float *As, float *ys, float *din
                 yv[q] -= dot4(x[q][4], z[4], x[q][5], z[5], x[q][6], z[6], x[q][7], z[7]);
                 if (i < j0 + 2 * P) ys[i] = yv[q];  // pivot rows of the next panel
             }
-            *reinterpret_cast<float4 *>(As + i * LDA + j0) = make_float4(x[q][0], x[q][1], x[q][2], x[q][3]);
-            *reinterpret_cast<float4 *>(As + i * LDA + j0 + 4) = make_float4(x[q][4], x[q][5], x[q][6], x[q][7]);
+            *reinterpret_cast<float4 *>(ai) = make_float4(x[q][0], x[q][1], x[q][2], x[q][3]);
+            *reinterpret_cast<float4 *>(ai + 4) = make_float4(x[q][4], x[q][5], x[q][6], x[q][7]);
         }
         __syncwarp();
         // Trailing update A[i][cc..cc+7] -= L[i][j0..j0+7] . L[cc..cc+7][j0..j0+7]^T for every row i and every
         // 8-column tile right of the panel, one 4-column half of the panel after the other.  Rows above a tile
-        // (i < cc) only touch the upper triangle, which is never read, so the update is applied without a
-        // per-lane branch.
+        // (i < cc) only touch the upper triangle, which is never read; folded, it is not stored either, so they
+        // skip the tile (row-major, the update is applied without a per-lane branch).
 #pragma unroll 2
         for (int cc = j0 + P; cc < KP - 2 * P; cc += P) {
             float4 L[P][2];
+            const float *lb = As + chol_off<KP, FOLD>(cc, j0 >> 3);
 #pragma unroll
             for (int c = 0; c < P; c++) {
-                L[c][0] = *reinterpret_cast<const float4 *>(As + (cc + c) * LDA + j0);
-                L[c][1] = *reinterpret_cast<const float4 *>(As + (cc + c) * LDA + j0 + 4);
+                L[c][0] = *reinterpret_cast<const float4 *>(lb + c * LD);
+                L[c][1] = *reinterpret_cast<const float4 *>(lb + c * LD + 4);
             }
 #pragma unroll
             for (int q = 0; q < RPT; q++) {
                 if (q * 32 + 31 < cc) continue;  // this whole row group is above the tile (uniform)
                 const int i = tid + q * 32;
+                if (FOLD && i < cc) continue;
                 const float *xq = x[q];
                 auto upd = [&](float a, const float4(&lc)[2]) {
                     a -= dot4(xq[0], lc[0].x, xq[1], lc[0].y, xq[2], lc[0].z, xq[3], lc[0].w);
                     a -= dot4(xq[4], lc[1].x, xq[5], lc[1].y, xq[6], lc[1].z, xq[7], lc[1].w);
                     return a;
                 };
-                float4 a0 = *reinterpret_cast<float4 *>(As + i * LDA + cc);
-                float4 a1 = *reinterpret_cast<float4 *>(As + i * LDA + cc + 4);
+                float *ai = As + (FOLD ? ro[q] : i * LD) + cc;
+                float4 a0 = *reinterpret_cast<float4 *>(ai);
+                float4 a1 = *reinterpret_cast<float4 *>(ai + 4);
                 a0.x = upd(a0.x, L[0]), a0.y = upd(a0.y, L[1]), a0.z = upd(a0.z, L[2]), a0.w = upd(a0.w, L[3]);
                 a1.x = upd(a1.x, L[4]), a1.y = upd(a1.y, L[5]), a1.z = upd(a1.z, L[6]), a1.w = upd(a1.w, L[7]);
-                *reinterpret_cast<float4 *>(As + i * LDA + cc) = a0;
-                *reinterpret_cast<float4 *>(As + i * LDA + cc + 4) = a1;
+                *reinterpret_cast<float4 *>(ai) = a0;
+                *reinterpret_cast<float4 *>(ai + 4) = a1;
             }
         }
-        if (j0 + P <= KP - 2 * P) chol_tile_shared<KP, 4>(As, tid, j0, KP - 2 * P);
-        if (j0 + P <= KP - P) chol_tile_shared<KP, 2>(As, tid, j0, KP - P);
+        if (j0 + P <= KP - 2 * P) chol_tile_shared<KP, 4, FOLD>(As, tid, j0, KP - 2 * P);
+        if (j0 + P <= KP - P) chol_tile_shared<KP, 2, FOLD>(As, tid, j0, KP - P);
         __syncwarp();
     }
 
@@ -239,12 +286,13 @@ __device__ __forceinline__ bool chol_solve_warp(float *As, float *ys, float *din
     __syncwarp();
     for (int j0 = KP - P; j0 >= 0; j0 -= P) {
         float l[P][P], xs[P], di[P];
+        const float *rb = As + chol_off<KP, FOLD>(j0, 0);  // rows j0..j0+7 from column 0
 #pragma unroll
         for (int r = 1; r < P; r++)
 #pragma unroll
             for (int h = 0; h < 2; h++) {
                 if (4 * h >= r) continue;
-                const float4 v = *reinterpret_cast<const float4 *>(As + (j0 + r) * LDA + j0 + 4 * h);
+                const float4 v = *reinterpret_cast<const float4 *>(rb + r * LD + j0 + 4 * h);
                 l[r][4 * h] = v.x, l[r][4 * h + 1] = v.y, l[r][4 * h + 2] = v.z, l[r][4 * h + 3] = v.w;
             }
 #pragma unroll
@@ -274,9 +322,9 @@ __device__ __forceinline__ bool chol_solve_warp(float *As, float *ys, float *din
         for (int q = 0; q < RPT; q++) {
             const int i = tid + q * 32;
             if (i < j0) {
-                const float *col = As + j0 * LDA + i;  // column i of rows j0..j0+7
-                yv[q] -= dot4(col[4 * LDA], xs[4], col[5 * LDA], xs[5], col[6 * LDA], xs[6], col[7 * LDA], xs[7]);
-                yv[q] -= dot4(col[0], xs[0], col[LDA], xs[1], col[2 * LDA], xs[2], col[3 * LDA], xs[3]);
+                const float *col = rb + i;  // column i of rows j0..j0+7
+                yv[q] -= dot4(col[4 * LD], xs[4], col[5 * LD], xs[5], col[6 * LD], xs[6], col[7 * LD], xs[7]);
+                yv[q] -= dot4(col[0], xs[0], col[LD], xs[1], col[2 * LD], xs[2], col[3 * LD], xs[3]);
                 if (i >= j0 - P) ys[i] = yv[q];  // pivot rows of the next (upper) panel
             } else if (i < j0 + P) {
                 const int r = i - j0;
@@ -295,8 +343,9 @@ __device__ __forceinline__ bool chol_solve_warp(float *As, float *ys, float *din
     return bad;
 }
 
-// Solve A x = y for a KP x KP SPD matrix held row-major in shared memory with
-// row stride KP+4 (lower triangle used), rhs in ys, scratch dinv[KP].  Executed
+// Solve A x = y for a KP x KP SPD matrix held in shared memory (sys_at: row-major
+// with row stride KP+4, lower triangle used, or folded lower blocks for one warp
+// with FOLD), rhs in ys, scratch dinv[KP].  Executed
 // by NW warps together.  Thread t owns rows t + q*32*NW and keeps their
 // right-hand-side entries in registers.  On return ys holds x; the result is
 // true when a pivot was not positive (LAPACK info != 0).  Only the lower
@@ -308,10 +357,11 @@ __device__ __forceinline__ bool chol_solve_warp(float *As, float *ys, float *din
 // rows, applies the panel to its right-hand side (the forward substitution is
 // fused into the factorisation), then updates the trailing matrix in 4x4 tiles.
 // The back substitution L^T x = z runs panel by panel from the bottom.
-template <int KP, int NW>
+template <int KP, int NW, bool FOLD = false>
 __device__ __forceinline__ bool chol_solve(float *As, float *ys, float *dinv, const int tid)
 {
-    if constexpr (NW == 1) return chol_solve_warp<KP>(As, ys, dinv, tid);
+    static_assert(!FOLD || NW == 1, "only the one-warp solve has a folded layout");
+    if constexpr (NW == 1) return chol_solve_warp<KP, FOLD>(As, ys, dinv, tid);
     constexpr int NT = NW * 32;
     constexpr int LDA = KP + 4;
     constexpr int RPT = KP / NT;

@@ -14,7 +14,7 @@
 //
 // Each warp owns a 64 x 64 quadrant of G as 4 x 8 m16n8 accumulator tiles (128 floats per lane, the
 // SIMT kernel's register footprint); at k = 64 the one warp keeps only the 20 tiles the Cholesky reads (the
-// lower triangle and the diagonal 16 x 16 blocks, 80 floats per lane), which lets 12 CTAs share an SM.
+// lower triangle and the diagonal 16 x 16 blocks, 80 floats per lane), which lets 11-16 CTAs share an SM.
 // A = Z^T and B = Z are the same staged tile:
 //   * bf16 rows with unweighted / uniformly weighted Gram: mma.m16n8k16 bf16, operands loaded with
 //     ldmatrix.trans (the tile is feature-contiguous, the MMA wants pairs along the gathered rows).
@@ -34,16 +34,22 @@
 
 namespace lk {
 
-template <int KP, typename ET, bool WEIGHTED>
+template <int KP, typename ET, int MODE, bool WEIGHTED>
 struct TcCfg {
     using C = AlsCfg<KP>;
     static constexpr bool BF16MMA = sizeof(ET) == 2 && !WEIGHTED;
+    // k = 64, bf16 rows, implicit feedback with a uniform confidence (the benchmark's route): every row's
+    // right-hand-side weight is the same, so the kernel's rhs loop reads no values (RHS_PAIR in the kernel)
+    static constexpr bool RHS_PAIR = BF16MMA && MODE == LK_ALS_IMPLICIT && KP == 64;
     static constexpr int SROW = KP + 8;  // staged row stride (elements)
     static constexpr int STAGE_ELTS = C::STAGE_ROWS * SROW;
-    static constexpr int CHOL_BYTES = KP * C::LDA * 4;
-    // k = 64 bf16: a third stage still fits in the Cholesky buffer the stages share, and gives the gather two
-    // stages of look-ahead
-    static constexpr int NSTAGE = KP == 64 && 3 * STAGE_ELTS * (int)sizeof(ET) <= CHOL_BYTES ? 3 : C::NSTAGE;
+    // the benchmark's route folds its system (chol_off) to fit 16 CTAs per SM
+    static constexpr bool FOLD = RHS_PAIR;
+    static constexpr int CHOL_BYTES = SYS_FLOATS<KP, FOLD> * 4;
+    // Stages per route.  The benchmark's route keeps two, which with the folded system leaves room for 16 CTAs
+    // per SM (OCC below).  The other k = 64 bf16 routes keep a third stage (two stages of look-ahead for the
+    // gather) at 12 CTAs.
+    static constexpr int NSTAGE = RHS_PAIR ? 2 : KP == 64 && sizeof(ET) == 2 ? 3 : C::NSTAGE;
     static constexpr int STAGES_BYTES = NSTAGE * STAGE_ELTS * (int)sizeof(ET);
     static constexpr int UNI = STAGES_BYTES > CHOL_BYTES ? STAGES_BYTES : CHOL_BYTES;
     static constexpr int ZERO_BYTES = KP * 2;  // one zero bf16 row (ldmatrix target for rows past the end)
@@ -56,9 +62,14 @@ struct TcCfg {
     // of 128).  k = 128 keeps full 64 x 64 quadrants (a warp's quadrant may lie wholly in either triangle).
     static constexpr bool LOWER = KP == 64;
     __device__ static constexpr bool tile(int mi, int nj) { return !LOWER || nj <= 2 * mi + 1; }
-    // operand fragments sit next to the accumulators: fewer resident warps than the SIMT kernel (12 one-warp
-    // CTAs per SM at k = 64, up to 168 registers each; 2 four-warp CTAs at k = 128, up to 255)
-    static constexpr int OCC = KP >= 128 ? 2 : 12;
+    // CTAs per SM the registers allow.  Operand fragments sit next to the accumulators, so there are fewer
+    // resident warps than in the SIMT kernel: at k = 64, 16 one-warp CTAs (128 registers each) on the
+    // benchmark's route and 12 (168 registers) on the others, of which fp32 rows fit only 11 in shared memory;
+    // 2 four-warp CTAs at k = 128 (up to 255 registers).
+    static constexpr int OCC = KP >= 128 ? 2 : RHS_PAIR ? 16 : 12;
+    // the folded route's 16 CTAs must also fit in shared memory: each takes the 1 KB the hardware reserves per
+    // block besides SMEM_BYTES, of the SM's 228 KB
+    static_assert(!FOLD || OCC * (SMEM_BYTES + 1024) <= 233472, "OCC CTAs fit one SM's shared memory");
 };
 
 __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], uint32_t addr)
@@ -100,16 +111,16 @@ __device__ __forceinline__ void split_tf32(float z, uint32_t &hi, uint32_t &lo)
 // mode with per-nonzero confidences (z = sqrt(v) o); otherwise the Gram is unweighted and scaled by the
 // uniform confidence (implicit) or not at all (explicit).
 template <int KP, typename ET, int MODE, bool WEIGHTED>
-__global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)) als_tc_kernel(lk_als_args a)
+__global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, MODE, WEIGHTED>::OCC)) als_tc_kernel(lk_als_args a)
 {
     using C = AlsCfg<KP>;
-    using T = TcCfg<KP, ET, WEIGHTED>;
-    constexpr int NW = C::NW, NT = C::NT, LDA = C::LDA, SROW = T::SROW, NS = T::NSTAGE;
+    using T = TcCfg<KP, ET, MODE, WEIGHTED>;
+    constexpr int NW = C::NW, NT = C::NT, SROW = T::SROW, NS = T::NSTAGE;
     constexpr bool IMPLICIT = MODE == LK_ALS_IMPLICIT;
     // k = 64, bf16 rows, uniform confidence v: every row's right-hand-side weight is the same v + 1, so the
     // loop over the rows needs no shuffle of the values, and lane l accumulates features 2 l and 2 l + 1 from
     // one 32-bit load per row
-    constexpr bool RHS_PAIR = T::BF16MMA && IMPLICIT && KP == 64;
+    constexpr bool RHS_PAIR = T::RHS_PAIR;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     ET *stage0 = reinterpret_cast<ET *>(smem_raw);
     float *As = reinterpret_cast<float *>(smem_raw);
@@ -393,6 +404,8 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
 #pragma unroll
                 for (int h = 0; h < 2; h++) {
                     if (!T::tile(mi, nj)) continue;
+                    // folded: the upper 8 x 8 block of a diagonal 16 x 16 block is not stored (sys_at)
+                    if (T::FOLD && nj == 2 * mi + 1 && h == 0) continue;
                     const int gi = qi + 16 * mi + g + 8 * h, gc = qj + 8 * nj + 2 * t;
                     float v0 = acc[mi][nj][2 * h], v1 = acc[mi][nj][2 * h + 1];
                     if constexpr (IMPLICIT) {
@@ -403,7 +416,7 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
                         if (gi == gc) v0 += regn;  // explicit.rs:106-108
                         if (gi == gc + 1) v1 += regn;
                     }
-                    *reinterpret_cast<float2 *>(As + gi * LDA + gc) = make_float2(v0, v1);
+                    *reinterpret_cast<float2 *>(sys_at<KP, T::FOLD>(As, gi, gc)) = make_float2(v0, v1);
                 }
 #pragma unroll
         for (int q = 0; q < C::YPT; q++) ys[tid + q * NT] = yacc[q];
@@ -412,7 +425,7 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
         // ---- Cholesky + triangular solves in shared memory, then write the row
         float xold[C::RPT];
         read_old_row<KP, NW>(thisrow, k, tid, xold);
-        const bool bad = chol_solve<KP, NW>(As, ys, dinv, tid);
+        const bool bad = chol_solve<KP, NW, T::FOLD>(As, ys, dinv, tid);
         write_row<KP, NW>(a, row, thisrow, ys, tid, bad, xold);
         // the next chunk's bulk copies (async proxy) overwrite this buffer
         fence_proxy_async();
@@ -423,10 +436,10 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, WEIGHTED>::OCC)
 template <int KP, typename ET, int MODE, bool WEIGHTED>
 static int launch_tc(const lk_als_args &a, cudaStream_t st)
 {
-    using T = TcCfg<KP, ET, WEIGHTED>;
+    using T = TcCfg<KP, ET, MODE, WEIGHTED>;
     auto kern = als_tc_kernel<KP, ET, MODE, WEIGHTED>;
     LK_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SMEM_BYTES));
-    // k = 64 needs the whole 228 KB carve-out for 12 resident CTAs
+    // k = 64 needs the whole 228 KB carve-out for 11-16 resident CTAs
     LK_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     int occ = 0;
     LK_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, AlsCfg<KP>::NT, T::SMEM_BYTES));
