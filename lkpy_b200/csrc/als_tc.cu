@@ -3,7 +3,8 @@
 // Same contract as als_half_kernel (als_kernels.cu; reference src/accel/als/implicit.rs:87-125,
 // explicit.rs:80-119) for k = 64 and k = 128, and the same shape of work: a persistent grid pulls
 // chunks from the host plan, one CTA owns one chunk, the gathered rows are staged through shared
-// memory by the TMA engine's bulk-copy path (cp.async.bulk + mbarrier), rows split over several chunks
+// memory (per-lane 16-byte cp.async at k = 64, the TMA engine's cp.async.bulk at k = 128, both completing on
+// mbarriers), rows split over several chunks
 // park partial systems in global memory and the last part sums them in slot order, and the k x k system
 // is factored in shared memory (chol_solve, als_common.cuh).  What changes is the Gram:
 //
@@ -41,6 +42,10 @@ struct TcCfg {
     // k = 64, bf16 rows, implicit feedback with a uniform confidence (the benchmark's route): every row's
     // right-hand-side weight is the same, so the kernel's rhs loop reads no values (RHS_PAIR in the kernel)
     static constexpr bool RHS_PAIR = BF16MMA && MODE == LK_ALS_IMPLICIT && KP == 64;
+    // k = 64 (one warp): the whole warp gathers each stage with per-lane 16-byte cp.async copies, completion
+    // counted on the stage's mbarrier by one arrival per lane.  A per-lane cp.async.bulk (operands in uniform
+    // registers) compiles to a loop that sends one row per pass.  k = 128 keeps the bulk copies from warp 0.
+    static constexpr bool LANE_GATHER = KP == 64;
     static constexpr int SROW = KP + 8;  // staged row stride (elements)
     static constexpr int STAGE_ELTS = C::STAGE_ROWS * SROW;
     // the benchmark's route folds its system (chol_off) to fit 16 CTAs per SM
@@ -140,7 +145,7 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, MODE, WEIGHTED>
     const float scale = (IMPLICIT && !WEIGHTED) ? a.uniform_val : 1.0f;
 
     if (tid == 0) {
-        for (int s = 0; s < NS; s++) mbar_init(&bars[s], 1);
+        for (int s = 0; s < NS; s++) mbar_init(&bars[s], T::LANE_GATHER ? 32 : 1);
         mbar_fence_init();
     }
     for (int i = tid; i < T::ZERO_BYTES / 16; i += NT) reinterpret_cast<uint4 *>(zero_row)[i] = make_uint4(0, 0, 0, 0);
@@ -212,7 +217,22 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, MODE, WEIGHTED>
             const int s = it % NS;
             const int nrows = min(32, len - it * 32);
             ET *dst = stage0 + s * T::STAGE_ELTS;
-            if (warp == 0) {
+            if constexpr (T::LANE_GATHER) {
+                // a row is GPR granules: lane l copies granule l % GPR of rows l / GPR + RPP i, taking each row's
+                // column index from the lane that holds it.  Rows at or past nrows are not copied.  (lane_id():
+                // the per-lane offsets held through the chunk loop would make the fp32 and weighted routes spill.)
+                constexpr int GPR = ROW_BYTES / 16, RPP = 32 / GPR;
+                const int ln = (int)lane_id(), gr = ln % GPR;
+                const unsigned char *src = reinterpret_cast<const unsigned char *>(other) + 16 * gr;
+                unsigned char *dstg = reinterpret_cast<unsigned char *>(dst) + 16 * gr;
+#pragma unroll
+                for (int i = 0; i < GPR; i++) {
+                    const int r = ln / GPR + RPP * i;
+                    const int cr = __shfl_sync(FULL, c, r);
+                    if (r < nrows) cp_async_16(dstg + r * SROW * (int)sizeof(ET), src + (int64_t)cr * ROW_BYTES);
+                }
+                cp_async_mbar_arrive(&bars[s]);  // every lane arrives, copies or not
+            } else if (warp == 0) {
                 if (lane == 0) mbar_arrive_expect_tx(&bars[s], (uint32_t)nrows * ROW_BYTES);
                 if (lane < nrows) bulk_g2s(dst + lane * SROW, other + (size_t)c * k, ROW_BYTES, &bars[s]);
             }
@@ -255,27 +275,39 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, MODE, WEIGHTED>
                 const int lr = lane & 7, lm = lane >> 3;
                 for (int k0 = 0; k0 < nrows; k0 += 16) {
                     // A = Z^T: matrices (rows k0.., m0), (k0.., m0+8), (k0+8.., m0), (k0+8.., m0+8)
-                    uint32_t af[4][4], bfr[4][4];
+                    uint32_t af[4][4];
                     const int ra = k0 + lr + 8 * (lm >> 1);
 #pragma unroll
                     for (int mi = 0; mi < 4; mi++) {
                         const int col = qi + 16 * mi + 8 * (lm & 1);
                         ldmatrix_x4_trans(af[mi], ra < nrows ? sbase + (uint32_t)((ra * SROW + col) * 2) : zaddr);
                     }
-                    // B = Z: matrices (rows k0.., n0), (k0+8.., n0), (k0.., n0+8), (k0+8.., n0+8)
-                    const int rb = k0 + lr + 8 * (lm & 1);
+                    if constexpr (KP == 64) {
+                        // qi == qj == 0: B's four matrices for columns 16 np.. are af[np]'s, B wanting
+                        // (k0.., n0), (k0+8.., n0) for nj = 2 np and (k0.., n0+8), (k0+8.., n0+8) for nj = 2 np + 1
 #pragma unroll
-                    for (int np = 0; np < 4; np++) {
-                        const int col = qj + 16 * np + 8 * (lm >> 1);
-                        ldmatrix_x4_trans(bfr[np], rb < nrows ? sbase + (uint32_t)((rb * SROW + col) * 2) : zaddr);
+                        for (int mi = 0; mi < 4; mi++)
+#pragma unroll
+                            for (int nj = 0; nj < 8; nj++)
+                                if (T::tile(mi, nj))
+                                    mma_bf16_16816(acc[mi][nj], af[mi], af[nj >> 1][nj & 1], af[nj >> 1][(nj & 1) + 2]);
+                    } else {
+                        // B = Z: matrices (rows k0.., n0), (k0+8.., n0), (k0.., n0+8), (k0+8.., n0+8)
+                        uint32_t bfr[4][4];
+                        const int rb = k0 + lr + 8 * (lm & 1);
+#pragma unroll
+                        for (int np = 0; np < 4; np++) {
+                            const int col = qj + 16 * np + 8 * (lm >> 1);
+                            ldmatrix_x4_trans(bfr[np], rb < nrows ? sbase + (uint32_t)((rb * SROW + col) * 2) : zaddr);
+                        }
+#pragma unroll
+                        for (int mi = 0; mi < 4; mi++)
+#pragma unroll
+                            for (int nj = 0; nj < 8; nj++)
+                                if (T::tile(mi, nj))
+                                    mma_bf16_16816(acc[mi][nj], af[mi], bfr[nj >> 1][2 * (nj & 1)],
+                                                   bfr[nj >> 1][2 * (nj & 1) + 1]);
                     }
-#pragma unroll
-                    for (int mi = 0; mi < 4; mi++)
-#pragma unroll
-                        for (int nj = 0; nj < 8; nj++)
-                            if (T::tile(mi, nj))
-                                mma_bf16_16816(acc[mi][nj], af[mi], bfr[nj >> 1][2 * (nj & 1)],
-                                               bfr[nj >> 1][2 * (nj & 1) + 1]);
                 }
             } else {
                 const float sq = WEIGHTED ? sqrtf(vq[0]) : 1.0f;  // rows past the end carry v = 0
@@ -427,8 +459,9 @@ __global__ void __launch_bounds__(AlsCfg<KP>::NT, (TcCfg<KP, ET, MODE, WEIGHTED>
         read_old_row<KP, NW>(thisrow, k, tid, xold);
         const bool bad = chol_solve<KP, NW, T::FOLD>(As, ys, dinv, tid);
         write_row<KP, NW>(a, row, thisrow, ys, tid, bad, xold);
-        // the next chunk's bulk copies (async proxy) overwrite this buffer
-        fence_proxy_async();
+        // the next chunk's bulk copies (async proxy) overwrite this buffer.  cp.async writes through the
+        // generic proxy, which the barrier below already orders after the solve's accesses.
+        if constexpr (!T::LANE_GATHER) fence_proxy_async();
         __syncthreads();
     }
 }

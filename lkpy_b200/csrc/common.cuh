@@ -63,7 +63,7 @@ __device__ __forceinline__ float ld_stream_f32(const float *p)
 }
 
 // ---------------------------------------------------------------------------
-// PTX wrappers: mbarrier + bulk async copy (the TMA engine's 1-D path, SASS UBLKCP)
+// PTX wrappers: mbarrier, bulk async copy (the TMA engine's 1-D path, SASS UBLKCP) and per-lane cp.async
 // ---------------------------------------------------------------------------
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p)
@@ -122,6 +122,29 @@ __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gmem_src, u
         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
         ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
         : "memory");
+}
+
+// global -> shared copy of one 16-byte granule through L2 only (cp.async.cg, SASS LDGSTS; both addresses
+// 16-byte aligned).  Unlike the bulk copy it takes its operands per lane, and it writes through the generic proxy.
+__device__ __forceinline__ void cp_async_16(void *smem_dst, const void *gmem_src)
+{
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
+}
+
+// the lane index, read from %laneid each time: values derived from it are then recomputed where they are used
+// rather than hoisted and held in registers across a whole loop
+__device__ __forceinline__ uint32_t lane_id()
+{
+    uint32_t l;
+    asm volatile("mov.u32 %0, %%laneid;" : "=r"(l));
+    return l;
+}
+
+// arrive on the mbarrier once every cp.async this thread issued before has landed.  .noinc: the arrival counts
+// against the count the barrier was initialised with (one per arriving thread).
+__device__ __forceinline__ void cp_async_mbar_arrive(uint64_t *bar)
+{
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 // generic-proxy writes to smem must be fenced before the async proxy overwrites/reads them
