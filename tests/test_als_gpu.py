@@ -29,7 +29,7 @@ GOLD = Path(__file__).resolve().parent / "golden"
 def _simt_for_fp32_rows(lk_options):
     """This file pins the general SIMT kernel (als_kernels.cu) to "as good as f32 arithmetic": fp32 rows at
     k = 64 are kept off the tf32 tensor-core path, which has its own tests and tolerance
-    (tests/test_als_tcx_gpu.py); bf16 rows at k = 64 still take als_tc.cu."""
+    (tests/test_als_rows_gpu.py); bf16 rows at k = 64 still take als_tc.cu."""
     lk_options("LK_ALS_TF32", 0)
 
 

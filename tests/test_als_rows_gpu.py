@@ -1,9 +1,10 @@
 """
-Row-by-row parity of the ALS half-epoch on every kernel route, at the row lengths where the kernels change
-behaviour.
+The ALS row solve (lk_als_half_epoch) on every kernel route.  The routes are the entries of ROUTES below, and
+every test here takes its routes from that table.
 
-The other ALS GPU tests compare a whole half-step with one relative Frobenius error.  One row in a thousand
-off by 1e-3 moves that number by ~3e-5 and passes.  Here every row r with nonzeros is held to
+Row by row, at the row lengths where the kernels change behaviour.  A matrix-level check compares a whole
+half-step with one relative Frobenius error: one row in a thousand off by 1e-3 moves that number by ~3e-5 and
+passes.  So test_route_rows and the boundary, failing-row and replica tests hold every row r with nonzeros to
 
     e(r) = |x_gpu - x64| / |x64|  <=  max(A, B * f(r)),      f(r) = |x32 - x64| / |x64|
 
@@ -16,6 +17,14 @@ The rows are built by hand: lengths 1 .. 129 around the SIMT kernel's 32-row sta
 steps, lengths around 1, 2 and 3 part lengths, a row of over 40 parts, and empty rows.  The plan is checked
 to really contain each of them.  A larger variant adds ~16k short rows so that every CTA of the persistent grid
 works through many chunks in sequence (mbarrier phases, pad-column re-zeroing, claim-ahead).
+
+Whole matrices, on the tensor-core kernel (als_tc.cu) with small synthetic data, and with OtOr and the bf16
+copy of `other` built on the device by lk_als_otor as the trainers build them: the relative Frobenius error
+against the f64 oracle, agreement with the SIMT kernel on the same inputs, split rows (bit-identical reruns,
+close to the one-part solve), badly conditioned systems, and the LK_ALS_TF32 switch.
+
+Failures: a system that is not positive definite, or that meets an exact zero pivot on any one-warp solver,
+must be reported in the status word and leave its row untouched.
 """
 
 from __future__ import annotations
@@ -30,13 +39,14 @@ import oracle
 from lkpy_b200 import _lib, data, engine
 from lkpy_b200.als import ALSTrainerBase
 
-from helpers import rel_fro
+from helpers import implicit_init, rel_fro, small_synth
 
 pytestmark = pytest.mark.gpu
 
 N_OTHER = 3000
 REG = 0.1
 UNIFORM_CONF = 40.0
+DEFAULT_CHUNK = engine.DEFAULT_CHUNK_NNZ
 BASE_LENGTHS = (1, 2, 7, 8, 9, 15, 16, 17, 31, 32, 33, 63, 64, 65, 95, 96, 97, 127, 128, 129)
 COPIES = 3
 N_EMPTY = 4
@@ -128,43 +138,75 @@ def trainer_chunk(k: int, bf16: bool, kind: str) -> int:
     return ALSTrainerBase._chunk_nnz(SimpleNamespace(MODE=mode, config=cfg), k)
 
 
+def synth_matrices(inter, kind: str, rng) -> tuple[data.InteractionCSR, data.InteractionCSR]:
+    """(ui, iu) of `small_synth` interactions.  kind: "uniform" (one implicit confidence), "weighted"
+    (confidences scaled by the ratings) or "explicit" (ratings drawn from rng)."""
+    if kind == "explicit":
+        coo = inter.coo(rng.standard_normal(inter.nnz).astype(np.float32))
+        return data.InteractionCSR.from_scipy(coo), data.InteractionCSR.from_scipy(coo.T)
+    return data.als_implicit_matrices(inter, UNIFORM_CONF, use_ratings=kind == "weighted")
+
+
+def synth_factors(rng, n_users: int, n_items: int, k: int) -> tuple[np.ndarray, np.ndarray]:
+    """User factors, then item factors, N(0, 0.1^2)."""
+    p = (rng.standard_normal((n_users, k)) * 0.1).astype(np.float32)
+    q = (rng.standard_normal((n_items, k)) * 0.1).astype(np.float32)
+    return p, q
+
+
 # ---------------------------------------------------------------------------
 # device run, oracles, checker
 # ---------------------------------------------------------------------------
 
 
-def run_device(kind, csr, this, other, *, k, bf16, chunk, otor32=None, misaligned=False, replicas=None,
-               replica_row0=0):  # fmt: skip
-    """One half-step through lk_als_half_epoch; returns (x, sqrt(sqdelta), status, plan)."""
+def run_device(kind, csr, this, other, *, k, bf16, chunk=DEFAULT_CHUNK, otor32=None, device_otor=False, reg=REG,
+               misaligned=False, replicas=None, replica_row0=0):  # fmt: skip
+    """One half-step through lk_als_half_epoch; returns (x, sqrt(sqdelta), status, plan).  OtOr is otor32, or
+    with device_otor it and the bf16 copy of `other` are built on the device by lk_als_otor, as the trainers
+    build them."""
     dev = _lib.require_device()
     plan = engine.ALSHalfPlan.create(engine.DeviceCSR.from_host(csr, dev), k, chunk)
     d_this = torch.from_numpy(this.copy()).to(dev)
     src = torch.from_numpy(other).to(dev)
-    if bf16:
-        src = src.to(torch.bfloat16)
+    implicit = kind != "explicit"
+    if device_otor:
+        ws = engine.OtorWorkspace.create(k, dev)
+        obf = torch.empty_like(src, dtype=torch.bfloat16) if bf16 else None
+        otor = engine.als_otor(src, reg, ws, obf)
+        src = obf if bf16 else src
+    else:
+        otor = torch.from_numpy(otor32).to(dev) if implicit else None
+        if bf16:
+            src = src.to(torch.bfloat16)
     if misaligned:  # a contiguous view whose storage starts one element past a 16-byte boundary
         buf = torch.empty(src.numel() + 1, dtype=src.dtype, device=dev)
         buf[1:] = src.reshape(-1)
         src = buf[1:].view(other.shape)
         assert src.is_contiguous() and src.data_ptr() % 16 != 0
-    implicit = kind != "explicit"
-    otor = torch.from_numpy(otor32).to(dev) if implicit else None
     engine.als_half_epoch(
-        plan, _lib.LK_ALS_IMPLICIT if implicit else _lib.LK_ALS_EXPLICIT, d_this, src, otor=otor, reg=REG,
-        replicas=replicas, replica_row0=replica_row0,
+        plan, _lib.LK_ALS_IMPLICIT if implicit else _lib.LK_ALS_EXPLICIT, d_this, src,
+        otor=otor if implicit else None, reg=reg, replicas=replicas, replica_row0=replica_row0,
     )  # fmt: skip
     torch.cuda.synchronize()
     return d_this.cpu().numpy(), float(np.sqrt(plan.sqdelta.item())), int(plan.status.item()), plan
 
 
-def oracles(kind, csr, this, other, *, bf16):
-    """(x64, delta64, x32, otor32): the f64 and f32 oracles on the inputs the device sees."""
+def oracle64(kind, csr, this, other, *, bf16, reg=REG):
+    """(x64, delta64, otor32): the f64 oracle on the inputs the device sees, and the f32 OtOr (None in explicit
+    mode)."""
     mode = "explicit" if kind == "explicit" else "implicit"
     o32 = o64 = None
     if mode == "implicit":
-        o32, o64 = oracle.otor(oracle.bf16_round(other) if bf16 else other, REG)
-    x64, d64 = oracle.als_half_f64(mode, csr, this, other, otor_mat=o64, reg=REG, bf16_other=bf16)
-    x32, _ = oracle.als_half(mode, csr, this, other, otor_mat=o32, reg=REG, bf16_other=bf16)
+        o32, o64 = oracle.otor(oracle.bf16_round(other) if bf16 else other, reg)
+    x64, d64 = oracle.als_half_f64(mode, csr, this, other, otor_mat=o64, reg=reg, bf16_other=bf16)
+    return x64, d64, o32
+
+
+def oracles(kind, csr, this, other, *, bf16, reg=REG):
+    """(x64, delta64, x32, otor32): the f64 and f32 oracles on the inputs the device sees."""
+    x64, d64, o32 = oracle64(kind, csr, this, other, bf16=bf16, reg=reg)
+    mode = "explicit" if kind == "explicit" else "implicit"
+    x32, _ = oracle.als_half(mode, csr, this, other, otor_mat=o32, reg=reg, bf16_other=bf16)
     return x64, d64, x32, o32
 
 
@@ -325,6 +367,24 @@ ROUTES = [
     _r("fallback-negative-conf", 64, False, "simt", kinds=("negative",)),
 ]
 _DEFAULT_OPTS = {"LK_ALS_TC": 1, "LK_ALS_TF32": 1}
+_ROUTE_BY_ID = {(r["id"], r["k"]): r for r in ROUTES}
+assert len(_ROUTE_BY_ID) == len(ROUTES), "a route id appears twice at one k"
+
+
+def route(id_: str, k: int) -> dict:
+    """The ROUTES entry `id_` at k (a KeyError, at collection, if there is none)."""
+    return _ROUTE_BY_ID[id_, k]
+
+
+def route_params(*cases) -> list:
+    """pytest params of (route, value, ...) tuples, named after the route and the values."""
+    return [pytest.param(*c, id="-".join([f"{c[0]['id']}-k{c[0]['k']}", *map(str, c[1:])])) for c in cases]
+
+
+def use_route(lk_options, r: dict) -> None:
+    """Set the kernel switches to their defaults, then to the route's own."""
+    for name, value in {**_DEFAULT_OPTS, **r.get("opts", {})}.items():
+        lk_options(name, value)
 
 
 def route_cases():
@@ -337,10 +397,7 @@ def route_cases():
 @pytest.mark.parametrize("route,kind,which", list(route_cases()))
 def test_route_rows(cuda_lib, lk_options, route, kind, which):
     """Every route, every mode it serves, at the trainers' part length for it and at 32: each row within bound."""
-    for name in _DEFAULT_OPTS:
-        lk_options(name, _DEFAULT_OPTS[name])
-    for name, value in route.get("opts", {}).items():
-        lk_options(name, value)
+    use_route(lk_options, route)
     chunk = 32 if which == "32" else trainer_chunk(route["k"], route["bf16"], kind)
     st = case(route, kind, chunk)
     if route["id"].startswith("fallback"):
@@ -354,10 +411,10 @@ def test_route_rows(cuda_lib, lk_options, route, kind, which):
 
 
 BOUNDARY_ROUTES = [
-    (_r("simt64-f32-bulk", 48, False, "simt"), "explicit"),  # pad columns 48..63 re-zeroed every chunk
-    (_r("simt128-f32-bulk", 100, False, "simt"), "uniform"),
-    (_r("tc-bf16mma", 64, True, "bf16mma"), "uniform"),  # three stages, claim-ahead
-    (_r("tc-tf32", 64, False, "tf32"), "weighted"),
+    (route("simt64-f32-bulk", 48), "explicit"),  # pad columns 48..63 re-zeroed every chunk
+    (route("simt128-f32-bulk", 100), "uniform"),
+    (route("tc-bf16mma", 64), "uniform"),  # three stages, claim-ahead
+    (route("tc-tf32", 64), "weighted"),
 ]
 
 
@@ -366,18 +423,17 @@ BOUNDARY_ROUTES = [
 def test_boundary_rows_many_chunks_per_cta(cuda_lib, lk_options, route, kind, chunk):
     """The boundary lengths among ~16k short rows and a row of over 40 parts, so that each CTA of the persistent
     grid solves many chunks in sequence."""
-    for name in _DEFAULT_OPTS:
-        lk_options(name, _DEFAULT_OPTS[name])
+    use_route(lk_options, route)
     st = case(route, kind, chunk, n_short=N_SHORT, many_parts=True)
     assert st["rows"] > N_SHORT
 
 
 def test_checker_rejects_one_perturbed_row(cuda_lib, lk_options):
     """Self-test: one row of a passing result moved by 1e-3 relative fails the per-row check, while the
-    matrix-level bar the other ALS tests use (relative Frobenius error < 1e-4) still accepts it."""
-    lk_options("LK_ALS_TF32", 0)
-    route = _r("simt64-f32-bulk", 64, False, "simt")
-    st = case(route, "uniform", 4096, n_short=N_SHORT, many_parts=True)
+    matrix-level bar (relative Frobenius error < 1e-4) still accepts it."""
+    r = route("simt64-f32-bulk", 64)
+    use_route(lk_options, r)
+    st = case(r, "uniform", 4096, n_short=N_SHORT, many_parts=True)
     got, x64, x32, csr = st["got"], st["x64"], st["x32"], st["csr"]
     assert rel_fro(got, x64) < 1e-4
     n = np.diff(csr.indptr)
@@ -395,9 +451,9 @@ def test_checker_rejects_one_perturbed_row(cuda_lib, lk_options):
 # ---------------------------------------------------------------------------
 
 FAIL_ROUTES = [
-    pytest.param(_r("simt32-f32-bulk", 32, False, "simt"), id="simt-k32"),
-    pytest.param(_r("tc-bf16mma", 64, True, "bf16mma"), id="bf16mma-k64"),
-    pytest.param(_r("tc-tf32", 64, False, "tf32"), id="tf32-k64"),
+    pytest.param(route("simt32-f32-bulk", 32), id="simt-k32"),
+    pytest.param(route("tc-bf16mma", 64), id="bf16mma-k64"),
+    pytest.param(route("tc-tf32", 64), id="tf32-k64"),
 ]
 
 
@@ -405,8 +461,7 @@ FAIL_ROUTES = [
 def test_one_failing_row_among_good_ones(cuda_lib, lk_options, route):
     """A NaN row of `other` gathered by one whole row and one split row: status names one of them, both keep
     their old values, and every other row is solved, within bound, and counted in the delta."""
-    for name in _DEFAULT_OPTS:
-        lk_options(name, _DEFAULT_OPTS[name])
+    use_route(lk_options, route)
     k, bf16, chunk = route["k"], route["bf16"], 32
     good = boundary_csr(chunk, "explicit", many_parts=True, seed=5)
     n = np.diff(good.indptr)
@@ -453,16 +508,15 @@ def test_one_failing_row_among_good_ones(cuda_lib, lk_options, route):
 @pytest.mark.parametrize(
     "route,kind",
     [
-        pytest.param(_r("simt32-f32-bulk", 32, False, "simt"), "uniform", id="simt-k32"),
-        pytest.param(_r("tc-bf16mma", 64, True, "bf16mma"), "uniform", id="bf16mma-k64"),
-        pytest.param(_r("tc-tf32", 128, False, "tf32"), "explicit", id="tf32-k128"),
+        pytest.param(route("simt32-f32-bulk", 32), "uniform", id="simt-k32"),
+        pytest.param(route("tc-bf16mma", 64), "uniform", id="bf16mma-k64"),
+        pytest.param(route("tc-tf32", 128), "explicit", id="tf32-k128"),
     ],
 )
 def test_replica_rows_match_this(cuda_lib, lk_options, route, kind):
     """replicas=[r], replica_row0=row0: r[row0 + row] holds exactly the bits of this[row] (zeros for empty rows),
     and nothing outside that window is written."""
-    for name in _DEFAULT_OPTS:
-        lk_options(name, _DEFAULT_OPTS[name])
+    use_route(lk_options, route)
     k, bf16, chunk = route["k"], route["bf16"], 32
     csr = boundary_csr(chunk, kind, many_parts=True, seed=9)
     n_rows = csr.shape[0]
@@ -479,3 +533,251 @@ def test_replica_rows_match_this(cuda_lib, lk_options, route, kind):
     assert np.array_equal(r[row0 : row0 + n_rows].view(np.int32), got.view(np.int32))
     assert np.all(r[row0 : row0 + n_rows][np.diff(csr.indptr) == 0] == 0.0)
     assert np.all(r[:row0] == sentinel) and np.all(r[row0 + n_rows :] == sentinel)
+
+
+# ---------------------------------------------------------------------------
+# whole matrices on the tensor-core kernel, OtOr and the bf16 copy of `other` built on the device
+# ---------------------------------------------------------------------------
+
+#: relative Frobenius distance to the SIMT kernel (LK_ALS_TC=0) on the same inputs, by (family, k).  The bounds
+#: are the ones each path was first tested with: bf16mma agrees with the SIMT kernel to rounding; the tf32 x3 Gram
+#: drops the lo.lo term and truncates lo, so it sits a few 1e-5 from f32 arithmetic, inside the 1e-4 bound against
+#: the f64 oracle.  The worst distances over test_parity's cases on an H100 80GB HBM3 (700 W power limit) were
+#: 5.6e-7 / 1.5e-6 for bf16mma and 6.6e-6 / 2.2e-5 for tf32 at k = 64 / 128.
+SIMT_AGREEMENT = {("bf16mma", 64): 2e-5, ("bf16mma", 128): 3e-5, ("tf32", 64): 6e-5, ("tf32", 128): 6e-5}
+
+
+@pytest.mark.parametrize(
+    "route,kind,chunk,seed",
+    route_params(
+        *[(route("tc-bf16mma", 64), kind, chunk, 21)
+          for kind in ("uniform", "explicit") for chunk in (DEFAULT_CHUNK, 256, 64, 32)],
+        *[(route("tc-tf32", k), kind, DEFAULT_CHUNK, 21) for k in (64, 128) for kind in ALL],
+        *[(route("tc-tf32-bf16rows", k), "weighted", DEFAULT_CHUNK, 21) for k in (64, 128)],
+        (route("tc-bf16mma", 128), "explicit", DEFAULT_CHUNK, 21),
+        *[(route("tc-bf16mma", 128), kind, DEFAULT_CHUNK, 31) for kind in ("uniform", "explicit")],
+    ),
+)
+def test_parity(cuda_lib, lk_options, route, kind, chunk, seed):
+    """Both half-steps against the f64 oracle and against the SIMT kernel, for row parts from whole rows down to
+    32 nonzeros (split rows are summed from their partial systems in slot order)."""
+    use_route(lk_options, route)
+    k, bf16 = route["k"], route["bf16"]
+    inter = small_synth(900, 500, 40000, seed=seed)
+    rng = np.random.default_rng(seed)
+    p, q = synth_factors(rng, inter.n_users, inter.n_items, k)
+    ui, iu = synth_matrices(inter, kind, rng)
+    for csr, this, other in ((ui, p, q), (iu, q, p)):
+        got, delta, status, plan = run_device(kind, csr, this, other, k=k, bf16=bf16, chunk=chunk, device_otor=True)
+        assert status == 0
+        assert plan.vals_uniform == (kind == "uniform")
+        if chunk < 64:
+            assert plan.n_split_rows > 0
+        x64, d64, _ = oracle64(kind, csr, this, other, bf16=bf16)
+        assert rel_fro(got, x64) < 1e-4, rel_fro(got, x64)
+        assert delta == pytest.approx(d64, rel=1e-3)
+        assert np.all(got[np.diff(csr.indptr) == 0] == 0.0)
+        lk_options("LK_ALS_TC", 0)
+        simt, _, status, _ = run_device(kind, csr, this, other, k=k, bf16=bf16, chunk=chunk, device_otor=True)
+        lk_options("LK_ALS_TC", 1)
+        assert status == 0
+        assert rel_fro(got, simt) < SIMT_AGREEMENT[route["family"], k], rel_fro(got, simt)
+
+
+@pytest.mark.parametrize(
+    "route,kind,chunk",
+    route_params(
+        *[(route("tc-bf16mma", 64), kind, chunk) for kind in ("uniform", "explicit") for chunk in (32, 64, 96)],
+        *[(route("tc-tf32", k), kind, 32) for k in (64, 128) for kind in ALL],
+        *[(route("tc-bf16mma", 128), kind, 32) for kind in ("uniform", "explicit")],
+    ),
+)
+def test_split_rows_deterministic(cuda_lib, lk_options, route, kind, chunk):
+    """Rows cut into parts of `chunk` nonzeros (96: not a power of two) give the same bits on a rerun, stay within
+    the oracle's bound and close to the one-part solve."""
+    use_route(lk_options, route)
+    k, bf16 = route["k"], route["bf16"]
+    inter = small_synth(300, 200, 20000, seed=5)
+    rng = np.random.default_rng(5)
+    _ui, iu = synth_matrices(inter, kind, rng)
+    p, q = synth_factors(rng, 300, 200, k)
+    a, _, status, plan = run_device(kind, iu, q, p, k=k, bf16=bf16, chunk=chunk, device_otor=True)
+    assert status == 0
+    assert plan.n_split_rows > 0
+    b, _, status, _ = run_device(kind, iu, q, p, k=k, bf16=bf16, chunk=chunk, device_otor=True)
+    assert status == 0
+    assert np.array_equal(a.view(np.int32), b.view(np.int32))
+    x64, _, _ = oracle64(kind, iu, q, p, bf16=bf16)
+    assert rel_fro(a, x64) < 1e-4
+    c, _, status, _ = run_device(kind, iu, q, p, k=k, bf16=bf16, chunk=1 << 20, device_otor=True)
+    assert status == 0
+    # split (parts added with round-to-nearest) vs unsplit (one tensor-core accumulation chain per row): the
+    # accumulation orders differ, and on the tf32 path the 128x128 solve amplifies that more than the 64x64 one
+    assert rel_fro(a, c) < (1e-4 if (route["family"], k) == ("tf32", 128) else 1e-5)
+
+
+@pytest.mark.parametrize(
+    "route,reg",
+    route_params(
+        (route("tc-bf16mma", 64), 1e-2),
+        (route("tc-bf16mma", 64), 1e-3),
+        (route("tc-tf32", 64), 1e-2),
+        (route("tc-bf16mma", 128), 1e-2),
+    ),
+)
+def test_badly_conditioned(cuda_lib, lk_options, route, reg):
+    """Large Gram, small ridge (cond ~1e4 at reg 1e-2, ~1e5 at 1e-3): the tensor-core kernel stays within a small
+    factor of what f32 arithmetic can deliver (the f32 oracle's own distance to the f64 oracle)."""
+    use_route(lk_options, route)
+    k, bf16 = route["k"], route["bf16"]
+    inter = small_synth(400, 300, 60000, seed=9)
+    rng = np.random.default_rng(9)
+    ui, _ = synth_matrices(inter, "uniform", rng)
+    p = (rng.standard_normal((400, k)) * 0.1).astype(np.float32)
+    q = rng.standard_normal((300, k)).astype(np.float32)  # trained-scale-and-beyond item factors
+    got, _, status, _ = run_device("uniform", ui, p, q, k=k, bf16=bf16, device_otor=True, reg=reg)
+    assert status == 0
+    x64, _, x32, _ = oracles("uniform", ui, p, q, bf16=bf16, reg=reg)
+    e_gpu, e_cpu = rel_fro(got, x64), rel_fro(x32, x64)
+    assert e_gpu < max(1e-4, 3.0 * e_cpu), (e_gpu, e_cpu)
+
+
+@pytest.mark.parametrize(
+    "route,kind",
+    route_params(
+        (route("tc-bf16mma", 64), "uniform"),
+        (route("tc-tf32", 64), "uniform"),
+        (route("tc-tf32", 64), "weighted"),
+        (route("tc-bf16mma", 128), "uniform"),
+    ),
+)
+def test_not_positive_definite_is_reported(cuda_lib, lk_options, route, kind):
+    """A system that is not positive definite (the reference's `ALS solve error`, implicit.rs:79) sets the status
+    word and leaves the row untouched, on each Gram path of the tensor-core kernel: bf16 MMAs, tf32 x3 on fp32
+    rows, tf32 x3 on sqrt(v)-scaled rows (per-nonzero confidences)."""
+    use_route(lk_options, route)
+    k, bf16 = route["k"], route["bf16"]
+    ui, _ = synth_matrices(small_synth(60, 40, 600, seed=2), kind, None)
+    this, other = np.full((60, k), 0.5, np.float32), np.zeros((40, k), np.float32)
+    got, _, status, plan = run_device(kind, ui, this, other, k=k, bf16=bf16, otor32=-np.eye(k, dtype=np.float32),
+                                      reg=0.0)  # fmt: skip
+    assert plan.vals_uniform == (kind == "uniform")
+    assert status > 0
+    assert np.all(got[np.diff(ui.indptr) > 0] == 0.5)  # failed solves do not write
+
+
+def test_zero_weight(cuda_lib, lk_options):
+    """weight = 0 makes every confidence 0: A = OtOr, the Gram scaled by zero."""
+    r = route("tc-bf16mma", 64)
+    use_route(lk_options, r)
+    ui, _ = data.als_implicit_matrices(small_synth(200, 150, 5000, seed=3), 0.0)
+    p, q = synth_factors(np.random.default_rng(3), 200, 150, 64)
+    got, _, status, _ = run_device("uniform", ui, p, q, k=64, bf16=r["bf16"], device_otor=True)
+    assert status == 0
+    x64, _, _ = oracle64("uniform", ui, p, q, bf16=r["bf16"])
+    assert np.isfinite(got).all()
+    assert rel_fro(got, x64) < 1e-4
+
+
+@pytest.mark.parametrize("route", route_params(*[(route("tc-tf32", k),) for k in (64, 128)]))
+def test_tf32_switch_off(cuda_lib, lk_options, route):
+    """LK_ALS_TF32=0 sends fp32 rows back to the SIMT kernel (same bits as LK_ALS_TC=0)."""
+    use_route(lk_options, route)
+    k = route["k"]
+    ui, _ = synth_matrices(small_synth(300, 200, 9000, seed=6), "uniform", None)
+    p, q = synth_factors(np.random.default_rng(6), 300, 200, k)
+    lk_options("LK_ALS_TF32", 0)
+    a, _, status_a, _ = run_device("uniform", ui, p, q, k=k, bf16=False, device_otor=True)
+    lk_options("LK_ALS_TF32", 1)
+    lk_options("LK_ALS_TC", 0)
+    b, _, status_b, _ = run_device("uniform", ui, p, q, k=k, bf16=False, device_otor=True)
+    assert status_a == status_b == 0
+    assert np.array_equal(a.view(np.int32), b.view(np.int32))
+
+
+def test_ml_small_half_steps(cuda_lib, lk_options, ml_small):
+    """Config 1 (ml-latest-small, reference init): both half-steps from the init on the fp32 tensor-core path
+    track the f64 oracle as closely as the f32 oracle does (the init makes the first systems ill-conditioned)."""
+    use_route(lk_options, route("tc-tf32", 64))
+    ui, iu = synth_matrices(ml_small, "uniform", None)
+    p, q = implicit_init(np.random.default_rng(42), ml_small.n_items, ml_small.n_users, 64)
+    for csr, this, other in ((ui, p, q), (iu, q, p)):
+        got, _, status, _ = run_device("uniform", csr, this, other, k=64, bf16=False, device_otor=True)
+        assert status == 0
+        x64, _, x32, _ = oracles("uniform", csr, this, other, bf16=False)
+        assert rel_fro(got, x64) < max(1e-4, 1.5 * rel_fro(x32, x64)), (rel_fro(got, x64), rel_fro(x32, x64))
+
+
+def test_short_and_odd_rows(cuda_lib, lk_options):
+    """k = 128 rows of 1..40 nonzeros (not multiples of the 16-row stage), an odd number of chunks, empty rows."""
+    r = route("tc-bf16mma", 128)
+    use_route(lk_options, r)
+    rng = np.random.default_rng(3)
+    n_rows, n_other = 77, 150
+    lens = rng.integers(0, 41, n_rows)
+    lens[[0, 5]] = 0
+    indptr = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
+    cols = np.concatenate([np.sort(rng.choice(n_other, n, replace=False)) for n in lens]).astype(np.int32)
+    csr = data.InteractionCSR(indptr, cols, np.full(len(cols), UNIFORM_CONF, np.float32), (n_rows, n_other))
+    p, q = synth_factors(rng, n_rows, n_other, 128)
+    got, _, status, _ = run_device("uniform", csr, p, q, k=128, bf16=r["bf16"], device_otor=True)
+    assert status == 0
+    x64, _, _ = oracle64("uniform", csr, p, q, bf16=r["bf16"])
+    assert rel_fro(got, x64) < 1e-4
+    assert np.all(got[lens == 0] == 0.0)
+
+
+# ---------------------------------------------------------------------------
+# an exact zero pivot
+# ---------------------------------------------------------------------------
+
+
+@pytest.mark.parametrize(
+    "route",
+    route_params(
+        (route("simt32-f32-bulk", 32),),
+        (route("simt64-f32-bulk", 64),),  # LK_ALS_TF32=0
+        (route("tc-bf16mma", 64),),
+        (route("tc-tf32", 64),),
+    ),
+)
+@pytest.mark.parametrize("where", ["first", "mid", "last"])
+def test_zero_pivot_row_is_reported_and_untouched(cuda_lib, lk_options, route, where):
+    """A row solve whose pivot is exactly zero (not NaN) is reported and leaves its row untouched.
+
+    Explicit mode with reg = 0 makes the system the bare Gram.  Gathered rows of `other` that are zero from feature
+    f0 on give a Gram whose rows and columns from f0 on are exactly zero, so the factorisation meets a zero pivot at
+    column f0 (column 0, the middle of a panel and the last column are tried).  Every other row gathers enough
+    random rows to be well conditioned and must still be solved."""
+    use_route(lk_options, route)
+    k, bf16 = route["k"], route["bf16"]
+    f0 = {"first": 0, "mid": k // 2 + 3, "last": k - 1}[where]
+    rng = np.random.default_rng([k, f0, 11])
+    n_good, n_other, per_row = 40, 400, 3 * k
+    other = (rng.standard_normal((n_other + 8, k)) * 0.5).astype(np.float32)
+    other[n_other:, f0:] = 0.0  # the last 8 rows of `other` span only features 0 .. f0-1
+    bad_row = 17
+    cols, vals, indptr = [], [], [0]
+    for r in range(n_good + 1):
+        if r == bad_row:
+            c = np.arange(n_other, n_other + 8)
+        else:
+            c = np.sort(rng.choice(n_other, per_row, replace=False))
+        cols.append(c)
+        vals.append(rng.uniform(1.0, 5.0, len(c)).astype(np.float32))
+        indptr.append(indptr[-1] + len(c))
+    csr = data.InteractionCSR(np.array(indptr, np.int32), np.concatenate(cols).astype(np.int32),
+                              np.concatenate(vals), (n_good + 1, n_other + 8))  # fmt: skip
+    this = (rng.standard_normal((n_good + 1, k)) * 0.1).astype(np.float32)
+    got, _, status, _ = run_device("explicit", csr, this, other, k=k, bf16=bf16, chunk=1024, reg=0.0)
+
+    assert status == bad_row + 1
+    assert np.array_equal(got[bad_row].view(np.int32), this[bad_row].view(np.int32))
+    # the other rows: A x = O^T v with the (bf16-rounded) gathered rows, in f64
+    o = (oracle.bf16_round(other) if bf16 else other).astype(np.float64)
+    for r in range(n_good + 1):
+        if r == bad_row:
+            continue
+        c, v = csr.indices[csr.indptr[r] : csr.indptr[r + 1]], csr.values[csr.indptr[r] : csr.indptr[r + 1]]
+        x = np.linalg.solve(o[c].T @ o[c], o[c].T @ v.astype(np.float64))
+        assert np.linalg.norm(got[r] - x) <= 1e-3 * np.linalg.norm(x), r
