@@ -37,6 +37,8 @@
  *                                                 src/lenskit/data/_items.py:942-998 lk_stochastic_topn
  *   FAIRReranker.__call__ (and TopNRanker + FAIRReranker)
  *                                                 src/lenskit/reranking/fair.py      lk_fair_rerank
+ *   MeasurementCollector over the ranking metrics (measure_list per list and metric)
+ *                                                 src/lenskit/metrics/ranking/*.py   lk_rank_metrics, lk_item_exposure
  *
  * Conventions
  *   - plain C: pointers and sizes only; no C++/torch types cross this boundary;
@@ -979,6 +981,84 @@ typedef struct lk_fair_args {
 } lk_fair_args;
 
 LK_API int lk_fair_rerank(const lk_fair_args *args, void *stream);
+
+/* ------------------------------------------------------------------------
+ * Ranking metrics (metrics.cu), behind the measure_list of src/lenskit/metrics/ranking's metric classes.
+ *
+ * lk_rank_metrics: B lists, list b the item numbers d_rec_items[d_rec_indptr[b] .. d_rec_indptr[b+1]) in rank
+ *   order (-1: an item the numbering does not know, never good), its test set d_test_items[d_test_indptr[b] ..
+ *   d_test_indptr[b+1]) (known numbers, ascending, unique) and nrel = d_nrel[b], the test list's length as the
+ *   reference counts it (unknown and repeated ids included).  Metric m truncates list b to k = min(L, n) positions
+ *   (n = -1: k = L; every k at most lk_topn_max()), with g good positions among them at 0-based positions p_j:
+ *     HIT          NaN if nrel = 0, else 1 if g > 0 else 0
+ *     PRECISION    NaN if k = 0, else g / k
+ *     RECALL       g / d, d = min(nrel, n) (n = -1: nrel); NaN if d = 0
+ *     RECIP_RANK   NaN if nrel = 0, 0 if g = 0, else 1 / (p_0 + 1)
+ *     DCG          NaN if nrel = 0, else S = pairwise_j(w[p_j])
+ *     NDCG         S / norms[m], m = min(nrel, n) for n > 0, else nrel
+ *     RBP          S / series_sum, S / norms[min(nrel, k)] (LK_RBP_NORM_PREFIX) or S / norms[k] (LK_RBP_NORM_LIST)
+ *     AP           NaN if k = 0, else pairwise_j((j + 1) / (p_j + 1)) / min(nrel, k)
+ *     MEAN_POP_RANK NaN if k = 0, else pairwise_{i < k}(w[item_i], 0 for item -1) / k
+ *   with w = d_weights + weight_offset and norms = d_norms + norm_offset, which the caller sizes for every index
+ *   read; pairwise is NumPy's order (pairwise.cuh) and every operation rounds to nearest.  Output d_out [M][B].
+ * lk_item_exposure: the per-item totals of n_entries (item, rank) entries sorted stably by item (d_sorted_items
+ *   ascending, d_order the sort's permutation of the entries, d_entry_list and d_entry_rank each entry's list and
+ *   0-based rank, in entry order).  Of several entries of one item in one list only the last counts (NumPy's
+ *   `totals[items] += values` with a repeated index).  d_totals[i] = the number of counted entries of item i when
+ *   d_weights is NULL, else 0.0 + w[rank] of its counted entries added one by one in entry order.
+ * ---------------------------------------------------------------------- */
+#define LK_METRIC_HIT 0
+#define LK_METRIC_PRECISION 1
+#define LK_METRIC_RECALL 2
+#define LK_METRIC_RECIP_RANK 3
+#define LK_METRIC_DCG 4
+#define LK_METRIC_NDCG 5
+#define LK_METRIC_RBP 6
+#define LK_METRIC_AP 7
+#define LK_METRIC_MEAN_POP_RANK 8
+#define LK_RBP_NORM_SERIES 0
+#define LK_RBP_NORM_PREFIX 1
+#define LK_RBP_NORM_LIST 2
+#define LK_RANK_METRICS_MAX 32
+
+typedef struct lk_metric_spec {
+    int32_t kind;                      /* LK_METRIC_* */
+    int32_t n;                         /* truncation, -1 for none */
+    int64_t weight_offset;             /* into d_weights */
+    int64_t norm_offset;               /* into d_norms */
+    int32_t norm_mode;                 /* RBP: LK_RBP_NORM_* */
+    int32_t reserved;
+    double series_sum;                 /* RBP with LK_RBP_NORM_SERIES */
+} lk_metric_spec;
+
+typedef struct lk_rank_metrics_args {
+    int64_t n_lists;                   /* B */
+    const int64_t *d_rec_indptr;       /* [B + 1] */
+    const int32_t *d_rec_items;
+    const int64_t *d_test_indptr;      /* [B + 1] */
+    const int32_t *d_test_items;
+    const int64_t *d_nrel;             /* [B] */
+    const double *d_weights;
+    const double *d_norms;
+    double *d_out;                     /* [M][B] */
+    int32_t n_metrics;                 /* M, 0..LK_RANK_METRICS_MAX */
+    int32_t reserved;
+    lk_metric_spec metrics[LK_RANK_METRICS_MAX];
+} lk_rank_metrics_args;
+
+typedef struct lk_item_exposure_args {
+    int64_t n_items;
+    int64_t n_entries;
+    const int32_t *d_sorted_items;     /* [n_entries] ascending */
+    const int64_t *d_order;            /* [n_entries] */
+    const int32_t *d_entry_list;       /* [n_entries], in entry order */
+    const int32_t *d_entry_rank;       /* [n_entries], in entry order */
+    const double *d_weights;           /* by rank, or NULL */
+    double *d_totals;                  /* [n_items] */
+} lk_item_exposure_args;
+
+LK_API int lk_rank_metrics(const lk_rank_metrics_args *args, void *stream);
+LK_API int lk_item_exposure(const lk_item_exposure_args *args, void *stream);
 
 #ifdef __cplusplus
 }

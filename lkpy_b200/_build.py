@@ -18,7 +18,7 @@ CSRC = Path(__file__).resolve().parent / "csrc"
 LIB = CSRC / "liblkpy_b200.so"
 SOURCES = ["capi.cu", "als_kernels.cu", "als_tc.cu", "knn_build.cu", "knn_score.cu", "knn_user.cu", "topn.cu", "prep.cu",
            "als_recommend.cu", "cooc.cu", "ease.cu", "slim.cu", "flexmf.cu",
-           "spmm.cu", "nmf.cu", "basic.cu", "stochastic.cu", "fair.cu"]
+           "spmm.cu", "nmf.cu", "basic.cu", "stochastic.cu", "fair.cu", "metrics.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17", "--extended-lambda",

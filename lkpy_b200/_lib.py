@@ -23,6 +23,10 @@ LK_FLEXMF_REG_NONE, LK_FLEXMF_REG_L2, LK_FLEXMF_REG_ADAMW = 0, 1, 2
 LK_STOCH_NONE, LK_STOCH_SOFTMAX, LK_STOCH_LINEAR = 0, 1, 2
 LK_STOCH_JUMP_WORDS = 4 * (33 + 64)
 LK_FAIR_LISTS, LK_FAIR_SCORES = 0, 1
+(LK_METRIC_HIT, LK_METRIC_PRECISION, LK_METRIC_RECALL, LK_METRIC_RECIP_RANK, LK_METRIC_DCG, LK_METRIC_NDCG,
+ LK_METRIC_RBP, LK_METRIC_AP, LK_METRIC_MEAN_POP_RANK) = range(9)  # fmt: skip
+LK_RBP_NORM_SERIES, LK_RBP_NORM_PREFIX, LK_RBP_NORM_LIST = 0, 1, 2
+LK_RANK_METRICS_MAX = 32
 
 i32p = C.POINTER(C.c_int32)
 i64p = C.POINTER(C.c_int64)
@@ -490,6 +494,48 @@ class LkFairArgs(C.Structure):
     ]
 
 
+class LkMetricSpec(C.Structure):
+    _fields_ = [
+        ("kind", C.c_int32),
+        ("n", C.c_int32),
+        ("weight_offset", C.c_int64),
+        ("norm_offset", C.c_int64),
+        ("norm_mode", C.c_int32),
+        ("reserved", C.c_int32),
+        ("series_sum", C.c_double),
+    ]
+
+
+class LkRankMetricsArgs(C.Structure):
+    _fields_ = [
+        ("n_lists", C.c_int64),
+        ("d_rec_indptr", vp),
+        ("d_rec_items", vp),
+        ("d_test_indptr", vp),
+        ("d_test_items", vp),
+        ("d_nrel", vp),
+        ("d_weights", vp),
+        ("d_norms", vp),
+        ("d_out", vp),
+        ("n_metrics", C.c_int32),
+        ("reserved", C.c_int32),
+        ("metrics", LkMetricSpec * LK_RANK_METRICS_MAX),
+    ]
+
+
+class LkItemExposureArgs(C.Structure):
+    _fields_ = [
+        ("n_items", C.c_int64),
+        ("n_entries", C.c_int64),
+        ("d_sorted_items", vp),
+        ("d_order", vp),
+        ("d_entry_list", vp),
+        ("d_entry_rank", vp),
+        ("d_weights", vp),
+        ("d_totals", vp),
+    ]
+
+
 #: every symbol ``include/lkpy_b200.h`` declares: name -> (restype, argtypes)
 SYMBOLS: dict[str, tuple] = {
     "lk_version": (C.c_int, []),
@@ -548,6 +594,8 @@ SYMBOLS: dict[str, tuple] = {
     "lk_stochastic_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64, C.c_int32]),
     "lk_stochastic_topn": (C.c_int, [C.POINTER(LkStochasticArgs), vp]),
     "lk_fair_rerank": (C.c_int, [C.POINTER(LkFairArgs), vp]),
+    "lk_rank_metrics": (C.c_int, [C.POINTER(LkRankMetricsArgs), vp]),
+    "lk_item_exposure": (C.c_int, [C.POINTER(LkItemExposureArgs), vp]),
 }
 
 _lib = None

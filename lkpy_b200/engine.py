@@ -20,8 +20,8 @@ from . import _lib
 from ._lib import (
     LkAlsArgs, LkAlsRecArgs, LkAssocScoreArgs, LkBiasLearnArgs, LkCoocArgs, LkEaseScoreArgs, LkFlexmfSampleArgs,
     LkFlexmfStepArgs, LkF32SeqSumArgs, LkKnnBuildArgs, LkKnnGeom, LkKnnRankArgs, LkKnnScoreArgs, LkNmfCdSweepArgs,
-    LkFairArgs, LkOffsetScoreArgs, LkSlimArgs, LkSpmmArgs, LkStochasticArgs, LkUknnSearchArgs, check, lib, ptr,
-    stream_ptr,
+    LkFairArgs, LkItemExposureArgs, LkOffsetScoreArgs, LkRankMetricsArgs, LkSlimArgs, LkSpmmArgs, LkStochasticArgs,
+    LkUknnSearchArgs, check, lib, ptr, stream_ptr,
 )  # fmt: skip
 from .data import InteractionCSR
 
@@ -2257,3 +2257,59 @@ def fair_rerank(
     a.d_out_idx, a.d_out_cnt = ptr(idx), ptr(cnt)
     check(lib().lk_fair_rerank(C.byref(a), stream_ptr()), "lk_fair_rerank")
     return idx, val, cnt[:B]
+
+
+# ---------------------------------------------------------------------------
+# ranking metrics (lkpy_b200.metrics)
+# ---------------------------------------------------------------------------
+
+
+def rank_metrics(specs: list[dict], rec_indptr: torch.Tensor, rec_items: torch.Tensor, test_indptr: torch.Tensor,
+                 test_items: torch.Tensor, nrel: torch.Tensor, weights: np.ndarray, norms: np.ndarray) -> torch.Tensor:  # fmt: skip
+    """
+    ``lk_rank_metrics`` (include/lkpy_b200.h states each metric) over B lists: ``rec_indptr`` [B + 1] int64 and
+    ``rec_items`` int32 (-1 for unknown items) on the device, the test sets as a device CSR of ascending unique item
+    numbers, ``nrel`` [B] int64 the test lengths, and one record per metric (the keys of ``lk_metric_spec``) with
+    offsets into the host f64 tables ``weights`` and ``norms``.  Returns ``out [M, B]`` f64 on the device.
+    """
+    dev = rec_indptr.device
+    B, M = rec_indptr.numel() - 1, len(specs)
+    out = torch.empty((M, max(B, 0)), dtype=torch.float64, device=dev)
+    if B <= 0 or M == 0:
+        return out
+    d_w = torch.from_numpy(np.concatenate([np.asarray(weights, np.float64), np.zeros(1)])).to(dev)
+    d_n = torch.from_numpy(np.concatenate([np.asarray(norms, np.float64), np.zeros(1)])).to(dev)
+    for m0 in range(0, M, _lib.LK_RANK_METRICS_MAX):
+        group = specs[m0 : m0 + _lib.LK_RANK_METRICS_MAX]
+        a = LkRankMetricsArgs()
+        a.n_lists, a.n_metrics = B, len(group)
+        a.d_rec_indptr, a.d_rec_items = ptr(rec_indptr), ptr(rec_items)
+        a.d_test_indptr, a.d_test_items, a.d_nrel = ptr(test_indptr), ptr(test_items), ptr(nrel)
+        a.d_weights, a.d_norms, a.d_out = ptr(d_w), ptr(d_n), ptr(out[m0:])
+        for j, sp in enumerate(group):
+            for k, v in sp.items():
+                setattr(a.metrics[j], k, v)
+        check(lib().lk_rank_metrics(C.byref(a), stream_ptr()), "lk_rank_metrics")
+    return out
+
+
+def item_exposure(n_items: int, items: torch.Tensor, lists: torch.Tensor, ranks: torch.Tensor,
+                  weights: np.ndarray | None) -> torch.Tensor:  # fmt: skip
+    """
+    ``lk_item_exposure``: the per-item totals [n_items] f64 of the entries ``items`` / ``lists`` / ``ranks`` (int32 on
+    the device, in list order): 1.0 per entry when ``weights`` is None, else ``weights[rank]`` added one by one in
+    entry order; of an item's entries in one list only the last counts.  The entries are sorted stably by item here.
+    """
+    dev = items.device
+    totals = torch.zeros(n_items, dtype=torch.float64, device=dev)
+    if n_items == 0:
+        return totals
+    sorted_items, order = torch.sort(items, stable=True)
+    d_w = None if weights is None else torch.from_numpy(np.asarray(weights, np.float64)).to(dev)
+    a = LkItemExposureArgs()
+    a.n_items, a.n_entries = n_items, items.numel()
+    a.d_sorted_items, a.d_order = ptr(sorted_items), ptr(order)
+    a.d_entry_list, a.d_entry_rank = ptr(lists), ptr(ranks)
+    a.d_weights, a.d_totals = ptr(d_w), ptr(totals)
+    check(lib().lk_item_exposure(C.byref(a), stream_ptr()), "lk_item_exposure")
+    return totals
