@@ -242,8 +242,10 @@ __device__ __forceinline__ bool chol_solve_warp(float *As, float *ys, float *din
         // Trailing update A[i][cc..cc+7] -= L[i][j0..j0+7] . L[cc..cc+7][j0..j0+7]^T for every row i and every
         // 8-column tile right of the panel, one 4-column half of the panel after the other.  Rows above a tile
         // (i < cc) only touch the upper triangle, which is never read; folded, it is not stored either, so they
-        // skip the tile (row-major, the update is applied without a per-lane branch).
-#pragma unroll 2
+        // skip the tile (row-major, the update is applied without a per-lane branch).  The loop is not unrolled:
+        // unrolled by two it compiled to three copies of the tile body (about 400 more instructions per k = 64
+        // kernel), and the ALS epoch ran 4-5 % slower (H100 80GB HBM3 at 700 W, DESIGN.md section 8).
+#pragma unroll 1
         for (int cc = j0 + P; cc < KP - 2 * P; cc += P) {
             float4 L[P][2];
             const float *lb = As + chol_off<KP, FOLD>(cc, j0 >> 3);
